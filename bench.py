@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- events/sec of the serving hot path on N B200s (one process per GPU).
+"""bench.py -- events/sec of the serving hot path on N H100s (one process per GPU).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload NAME] [--batch B]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload NAME] [--batch B] [--dump-outputs DIR]
 
 Workload (BASELINE.json `metric`): a 3-step serving graph + 4-model ensemble at 64 float32 features:
     Imputer(56 numeric cols) -> OneHotEncoder(8 categorical cols x 4) -> VotingEnsemble(4 linear models)
@@ -11,7 +11,9 @@ A "step" is one pass of the fused plan over one batch of B synthetic events alre
 `wire` leg: V2 JSON body in, JSON out), ingest6 (configs[4]: feature-set ingest over DataFrame columns), enrich_ens4 (online
 feature table gather + ensemble); `--gpus N` under torchrun is configs[3] (event-sharded router, fused P2P ensemble-merge or
 `--merge nccl`).  Every workload prints the same JSON line (roofline of its dominant kernel, cpu_baseline, e2e) and has a
-`--impl reference` arm.  See DESIGN.md "Measurement".
+`--impl reference` arm.  `--dump-outputs DIR` writes what the last timed step computed as DIR/<name>.npy (inputs are seeded:
+the same arguments give the same inputs on every run, so two builds can be compared output for output).  See DESIGN.md
+"Measurement".
 """
 
 import argparse
@@ -58,7 +60,36 @@ def parse():
     ap.add_argument("--merge", default="p2p", choices=["p2p", "nccl"],
                     help="N>1 ensemble-merge: p2p = votes stored into every rank's buffer from the kernel epilogue over "
                          "NVLink peer memory (fused); nccl = a separate all_gather per step")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the outputs of the last timed step as DIR/<name>.npy (float32 / float64, "
+                         "at most 64 MB in all: a fixed sample of rows beyond that)")
     return ap.parse_args()
+
+
+DUMP_CAP_BYTES = 60_000_000  # leaves room for the .npy headers under 64 MB
+NOMINAL_HBM_GBS = 3350.0  # H100 SXM5 data sheet: 3.35 TB/s of HBM3
+
+
+def dump_outputs(path, arrays, whole=None):
+    """write {name: array of rows} as path/<name>.npy in float32 (float64 for wider types); when they hold more than
+    DUMP_CAP_BYTES together, the same fixed, seeded sample of rows is kept from every array and its row numbers are written
+    as path/rows.npy.  `whole`: small arrays that are not per row (counters), written in full as float64."""
+    import re
+
+    os.makedirs(path, exist_ok=True)
+    arrays = {re.sub(r"[^A-Za-z0-9_.-]", "_", k): np.asarray(v) for k, v in arrays.items()}
+    arrays = {k: v.astype(np.float32 if v.dtype.itemsize <= 4 and v.dtype.kind in "fiub" else np.float64) for k, v in arrays.items()}
+    n_rows = len(next(iter(arrays.values())))
+    row_bytes = sum(v.nbytes // max(len(v), 1) for v in arrays.values())
+    if row_bytes * n_rows > DUMP_CAP_BYTES:
+        keep = np.sort(np.random.default_rng(0).choice(n_rows, size=(DUMP_CAP_BYTES - 8 * n_rows // 64) // (row_bytes + 8),
+                                                       replace=False))
+        arrays = {k: v[keep] for k, v in arrays.items()}
+        arrays["rows"] = keep.astype(np.float64)
+    for k, v in arrays.items():
+        np.save(os.path.join(path, f"{k}.npy"), v)
+    for k, v in (whole or {}).items():
+        np.save(os.path.join(path, f"{k}.npy"), np.asarray(v, dtype=np.float64))
 
 
 # ------------------------------------------------------------------------------------------ workloads
@@ -115,7 +146,7 @@ def router8_workload(n_rows, seed=4):
 
 def dense12_workload(n_rows, seed=6):
     """the dense linear-predict path the north_star puts on the tensor cores: a VotingEnsemble of 12 linear scorers over 64 raw
-    float32 features (random float64 weights, like configs[1]'s) -- 12 scores per event, N = 16 on tcgen05 (csrc/b2s_dense.cu)"""
+    float32 features (random float64 weights, like configs[1]'s) -- 12 scores per event, N = 16 on wgmma (csrc/b2s_dense.cu)"""
     from sklearn.linear_model import LinearRegression
 
     wr = np.random.default_rng(seed + 20)
@@ -355,17 +386,6 @@ class ClockSampler:
                 "samples": len(sm), "reasons": sorted(reasons)}
 
 
-def measured_traffic(name, B):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed ncu capture of this workload
-    (profiles/traffic.json, bytes per event), scaled to this launch; None if no capture is on file"""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    try:
-        rec = json.load(open(p)).get(name)
-        return rec["dram_bytes_per_event"] * B if rec else None
-    except (OSError, ValueError, KeyError):
-        return None
-
-
 def measured_peak():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
@@ -373,7 +393,7 @@ def measured_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return NOMINAL_HBM_GBS, "H100 SXM5 data sheet (3.35 TB/s), not measured"
 
 
 # ------------------------------------------------------------------------------------------ reference arm
@@ -413,7 +433,7 @@ def workload_desc(name):
         "router8": "router of 8 scorers (4 linear + 4 GradientBoostingRegressor(100 trees, depth 6)), 64-feat f32, sharded by events "
                    "with the fused ensemble-merge (BASELINE configs[3], SURVEY 8(d) config 4)",
         "dense_ens12": "VotingEnsemble of 12 linear scorers over 64 raw f32 features: the dense linear-predict path on the tensor "
-                       "cores (tcgen05 kind::tf32, exact 3-term splits; north_star)",
+                       "cores (wgmma tf32 over split operands; north_star)",
         "trees_ens4": "VotingEnsemble of 4 GradientBoostingRegressor(100 trees, depth 6, fit on 20 000 rows, all features), "
                       "128-feat f32 (BASELINE configs[2], SURVEY 8(d) config 3)",
         "enrich_ens4": "real-time enrichment: entity keys -> online feature table (4 Mi keys x 64 f32, 1 GiB in HBM) -> $mean imputing "
@@ -434,7 +454,7 @@ def serving_config_bench(nat, torch, name, B, min_ms=60.0, e2e_ms=250.0, seed=2)
     server, plan, names = build_server(name, wl)
     F = wl.X.shape[1]
     row_bytes = F * 4
-    nbuf = max(2, int(np.ceil(2 * 126e6 / (B * row_bytes))) + 1)
+    nbuf = max(2, int(np.ceil(2 * nat.device_info()["l2_bytes"] / (B * row_bytes))) + 1)
     reps = int(np.ceil(nbuf * B / wl.X.shape[0]))
     big = torch.from_numpy(np.tile(wl.X, (reps, 1))[: nbuf * B]).cuda()
     ptrs = [big.data_ptr() + i * B * row_bytes for i in range(nbuf)]
@@ -508,7 +528,7 @@ def config4_leg(rank, world, steps=10, timeout_s=100.0, workload_args=("--worklo
     """BASELINE configs[3] as written -- the 8-model mixed router (4 linear + 4 tree scorers), GLOBAL batch 65 536 split over the
     GPUs (strong scaling), fused P2P ensemble-merge -- measured beside the headline workload so that the driver's 1 / 2 / 4 / 8
     runs carry its curve.  Every rank starts `bench.py --workload router8 --scaling strong --batch 65536` as a CHILD process
-    (the invocation the 2-GPU lab runs used, profiles/lab/gpu18.sh); the children form their own process group (same RANK /
+    (the stand-alone invocation of that config); the children form their own process group (same RANK /
     WORLD_SIZE, MASTER_PORT + 17, torchrun's agent-store variables removed so that child rank 0 hosts the store).  A separate
     process, so a failure or a hang of this leg costs its own row after `timeout_s`, never the parent's line.
     `workload_args` selects another stand-alone invocation the same way (the configs[4] ingest leg).
@@ -598,7 +618,7 @@ def main():
     F = wl.X.shape[1]
     # inputs resident in HBM: NBUF distinct batches, rotated, so that consecutive steps never re-read L2-resident rows
     row_bytes = F * 4
-    nbuf = max(2, int(np.ceil(2 * 126e6 / (B * row_bytes))) + 1)
+    nbuf = max(2, int(np.ceil(2 * info["l2_bytes"] / (B * row_bytes))) + 1)
     reps = int(np.ceil(B / wl.X.shape[0]))
     base = torch.from_numpy(np.tile(wl.X, (reps, 1))[:B])
     bufs = []
@@ -641,9 +661,9 @@ def main():
 
     inner = args.launches_per_step
 
-    def step(i):  # one step = `inner` launches, each over the next of the rotating batches
+    def step(i, first=0):  # one step = `inner` launches, each over the next of the rotating batches
         for j in range(inner):
-            launch(i * inner + j)
+            launch(first + i * inner + j)
 
     def drain():  # pipelined merge: the last launch's votes have to be complete inside the timed region
         if merge == "p2p":
@@ -676,9 +696,10 @@ def main():
     l0 = nat.launch_count()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     t_wall0 = time.perf_counter()
+    first = (1 - args.steps * inner) % nbuf  # the last timed launch reads batch 0, whatever `inner` the probe chose
     e0.record(stream)
     for i in range(args.steps):
-        step(i)
+        step(i, first)
     drain()
     e1.record(stream)
     sync()
@@ -690,6 +711,8 @@ def main():
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         ms = float(t.item())
     clocks = sampler.stop(t_wall0, t_wall1) if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"out": out.cpu().numpy().reshape(B, plan.out_cols).view(plan.out_dtype)})
     merge_check = None
     if merge == "p2p":
         # every rank must now hold every shard: the last step's merged rows against the same launch scored locally
@@ -697,7 +720,7 @@ def main():
         full = np.empty((world * comm.max_rows, plan.out_cols), dtype=np.float32)
         nat.check(nat.load().b2s_memcpy_d2h(full.ctypes.data, last_merged[0], full.nbytes))
         comm.detach(plan)  # the single-GPU measurements below write locally again
-        last = inner * args.steps - 1 if inner > 0 else args.steps - 1
+        last = first + inner * args.steps - 1
         plan.run_device(bufs[last % nbuf].data_ptr(), B, row_bytes, out.data_ptr(), None, stream.cuda_stream)
         torch.cuda.synchronize()
         mine = out.cpu().numpy().reshape(B, plan.out_cols)
@@ -806,16 +829,14 @@ def main():
                                                                            "from the kernel epilogue, completion flags awaited " + ("by the launch's last CTA " if args.merge_wait == "fused" else "by a wait kernel ")
                                                                            + ("each launch)" if args.merge_lag == 0 else "one launch later: pipelined, lag 1)")}[merge],
                        "merge_verified": merge_check,
-                       "l2": f"{nbuf} rotating input buffers of {B * row_bytes / 1e6:.0f} MB (> 126 MB L2 between re-reads)",
+                       "l2": f"{nbuf} rotating input buffers of {B * row_bytes / 1e6:.0f} MB (> {info['l2_bytes'] / 1e6:.0f} MB L2 between re-reads)",
                        "device": info["name"], "kernel": plan.kernel},
             "p50_step_latency_us": {"batch": 4096, "p50": float(np.percentile(lat, 50)), "p99": float(np.percentile(lat, 99)),
                                     "how": "CUDA events around one fused-kernel launch, 1000 samples after 100 warm-ups",
                                     "e2e_p50": float(np.percentile(lat_e2e, 50)), "e2e_p99": float(np.percentile(lat_e2e, 99)),
                                     "e2e_how": "wall clock of DevicePlan.run on 4096 pinned host rows (H2D + kernel + D2H + status), "
                                                "1000 samples after 100 warm-ups"},
-            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "frac_of_nominal_8000": achieved / 8000.0,
-                         "traffic": measured_traffic(name, B), "traffic_source": "from_profile: ncu --set full capture of this "
-                         "kernel (profiles/traffic.json), scaled to this launch; not measured in this run",
+            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "frac_of_nominal_3350": achieved / NOMINAL_HBM_GBS,
                          "kernel": plan.kernel, "algorithmic_bytes_per_event": bpe,
                          "kernel_ms_per_launch": kms, "peak_source": peak_src},
             "gpu_launches": int(launches),
@@ -951,6 +972,11 @@ def main_ingest(args, rank, local_rank, world, emit=True):
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         ms = float(t.item())
     clocks = sampler.stop(t_wall0, t_wall1) if sampler else None
+    if args.dump_outputs and emit and rank == 0:  # the result columns (and validator / map counters) of the last timed step
+        raw = out.cpu().numpy()
+        specs, _extra = iplan._landing()
+        dump_outputs(args.dump_outputs, {name: raw[slot * stride: slot * stride + B * dt.itemsize].view(dt) for name, slot, dt in specs},
+                     whole={"counters": cnt.cpu().numpy()[: plan.n_counters]})
     n_it = max(args.steps, 10)
     kms = plan.time_device([b.data_ptr() for b in bufs], stride, B, out.data_ptr(), stride, cnt.data_ptr(), n_it) / n_it
     lat = []
@@ -1024,13 +1050,13 @@ def main_ingest(args, rank, local_rank, world, emit=True):
             "scaling": "weak", "vs_baseline": None, "dtype": "f32 / int32 / int64 columns, fp64 compares", "data": "synthetic",
             "config": {"workload": workload_desc(name), "batch_per_gpu": B, "global_batch": B * world,
                        "parallelism": f"row-sharded x{world}, no exchange",
-                       "l2": f"{nbuf} rotating columnar inputs of {B * wl.in_bytes_per_row / 1e6:.0f} MB (> 126 MB L2)",
+                       "l2": f"{nbuf} rotating columnar inputs of {B * wl.in_bytes_per_row / 1e6:.0f} MB (> {info['l2_bytes'] / 1e6:.0f} MB L2)",
                        "device": info["name"], "kernel": "columns_kernel (b2s_columns.cuh)",
                        "n_column_ops": len(iplan.out), "out_slots": plan.n_out},
             "p50_step_latency_us": {"batch": 4096, "p50": float(np.percentile(lat, 50)), "p99": float(np.percentile(lat, 99)),
                                     "how": "CUDA events around one columns_kernel launch, 300 samples"},
-            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "frac_of_nominal_8000": achieved / 8000.0,
-                         "traffic": measured_traffic(name, B), "kernel": "columns_kernel", "algorithmic_bytes_per_event": bpe,
+            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "frac_of_nominal_3350": achieved / NOMINAL_HBM_GBS,
+                         "kernel": "columns_kernel", "algorithmic_bytes_per_event": bpe,
                          "kernel_ms_per_launch": kms, "peak_source": peak_src},
             "gpu_launches": int(launches), "clocks": clocks,
         }
@@ -1166,6 +1192,8 @@ def main_enrich(args, rank, local_rank, world, emit=True):
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         ms = float(t.item())
     clocks = sampler.stop(t_wall0, t_wall1) if sampler else None
+    if args.dump_outputs and emit and rank == 0:
+        dump_outputs(args.dump_outputs, {"out": out.cpu().numpy().reshape(B, plan.out_cols).view(plan.out_dtype)})
     n_it = max(args.steps, 10)
     lat = []
     if fused:  # the step IS the kernel: time it alone, and one 4096-key launch for the latency figure
@@ -1218,13 +1246,13 @@ def main_enrich(args, rank, local_rank, world, emit=True):
             "scaling": "weak", "vs_baseline": None, "dtype": "f32 rows / int64 keys, f64 accumulate", "data": "synthetic",
             "config": {"workload": workload_desc(name), "batch_per_gpu": B, "global_batch": B * world,
                        "parallelism": f"event-sharded x{world} (table replicated), no exchange",
-                       "l2": "uniformly random keys over a 1 GiB table + 256 MiB of slots (> 126 MB L2)", "device": info["name"],
+                       "l2": f"uniformly random keys over a 1 GiB table + 256 MiB of slots (> {info['l2_bytes'] / 1e6:.0f} MB L2)", "device": info["name"],
                        "kernel": f"{plan.kernel}, rows gathered from the table by its loader (one launch)" if fused
                        else f"table_lookup_kernel + {plan.kernel}"},
             "p50_step_latency_us": {"batch": 4096, "p50": float(np.percentile(lat, 50)), "p99": float(np.percentile(lat, 99)),
                                     "how": f"CUDA events around one launch ({top}), 300 samples"},
-            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "frac_of_nominal_8000": achieved / 8000.0,
-                         "traffic": None if fused else measured_traffic(name, B), "kernel": top,
+            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "frac_of_nominal_3350": achieved / NOMINAL_HBM_GBS,
+                         "kernel": top,
                          "algorithmic_bytes_per_event": bpe, "kernel_ms_per_launch": kms, "peak_source": peak_src},
             "gpu_launches": int(launches), "clocks": clocks,
         }

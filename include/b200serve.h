@@ -1,5 +1,5 @@
 /*
- * b200serve.h -- C-ABI of the B200 serving-graph engine (libb200serve.so).
+ * b200serve.h -- C-ABI of the H100 serving-graph engine (libb200serve.so).
  *
  * The reference (mlrun/mlrun) has no FFI on this path: its hot path is pure Python.  This header is
  * the boundary a maintainer binds (ctypes/cffi) to replace the per-event Python step loop with a batched

@@ -1,4 +1,4 @@
-"""mlrun_b200 -- a B200-native serving-graph engine behind the mlrun.serving plugin API.
+"""mlrun_b200 -- an H100-native serving-graph engine behind the mlrun.serving plugin API.
 
     import mlrun_b200 as mlrun
     fn = mlrun.new_function("f", kind="serving")

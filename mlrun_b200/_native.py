@@ -150,7 +150,7 @@ def load():
             if not os.path.exists(LIB_PATH):
                 raise NativeError(
                     f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                    "(nvcc, sm_100a). mlrun_b200 has no CPU fallback for device steps."
+                    "(nvcc, sm_90a). mlrun_b200 has no CPU fallback for device steps."
                 )
             lib = C.CDLL(LIB_PATH)
             for name, (res, args) in SIGNATURES.items():

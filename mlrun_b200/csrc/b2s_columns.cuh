@@ -1,4 +1,4 @@
-// b2s_columns.cuh -- columnar feature-set transforms (sm_100a): the device side of the ingest path.
+// b2s_columns.cuh -- columnar feature-set transforms (sm_90a): the device side of the ingest path.
 //
 // Replaces, for DataFrame-shaped input, the reference's row-at-a-time walk of the feature-set graph
 // (feature_store/ingestion.py:38-127: DataFrame -> storey.DataframeSource -> one dict per row -> Imputer /

@@ -1,4 +1,4 @@
-// b2s_dense.cuh -- dense linear head on tcgen05 tensor cores (kernel in b2s_dense.cu): parameters and launcher.
+// b2s_dense.cuh -- dense linear head on the wgmma tensor cores (kernel in b2s_dense.cu): parameters and launcher.
 #pragma once
 #include <cuda.h>
 
@@ -6,7 +6,7 @@
 
 namespace b2s {
 
-constexpr int kDenseTileRows = 128;  // rows per tile == UMMA M
+constexpr int kDenseTileRows = 128;  // rows per tile == two warpgroups of wgmma M = 64
 constexpr int kDenseMaxIn = 128;     // input columns (a multiple of 32: whole TMA boxes / swizzle atoms)
 
 struct DenseParams {
@@ -17,7 +17,6 @@ struct DenseParams {
   const float* fill;   // [n_in] Imputer values (NaN: not imputed)
   const double* bias;  // [n_scores] intercepts
   int32_t n_in, n_scores, n_pad, any_fill;
-  int32_t tmem_cols;   // TMEM columns the CTA allocates (dense_tmem_cols)
   int32_t exact;       // 1: inputs split into three tf32 terms (exact); 0: two terms, the second rounded to nearest (2^-23 |x|)
   // epilogue: the common shapes run in float32 registers (fp64 conversions and local-memory arrays are what the generic
   // epilogue spends its time on); everything else takes the generic link + vote functions
@@ -32,6 +31,5 @@ enum { DENSE_EPI_GENERIC = 0, DENSE_EPI_SCORES = 1, DENSE_EPI_MEAN = 2, DENSE_EP
 cudaError_t dense_launch(const DenseParams& p, const KParams& kp, const CUtensorMap& tmap, int grid, int smem, int smem_optin,
                          cudaStream_t st);
 int dense_smem_bytes(int n_in, int n_pad);
-int dense_tmem_cols(int n_in, int n_pad);
 
 }  // namespace b2s

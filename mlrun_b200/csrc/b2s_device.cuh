@@ -1,4 +1,4 @@
-// b2s_device.cuh -- device-side plan tables and the row kernels (sm_100a).
+// b2s_device.cuh -- device-side plan tables and the row kernels (sm_90a).
 //
 // One kernel family, `rows_kernel<MODE, NS>`, runs a *fused row program* over a batch of events:
 //
@@ -74,7 +74,7 @@ __device__ __forceinline__ void merge_signal(const MergeSig& m) {
   if (m.n <= 0) return;
   // every thread's vote stores -> CTA barrier -> ONE system-scope fence by thread 0 (fences are cumulative: the stores thread 0
   // has observed through the barrier are ordered before everything it writes after the fence).  The fence waits for the CTA's
-  // peer stores to be acknowledged: about one NVLink round trip at the tail of the launch (profiles/r2_kernel_log.md, r2p/r2r).
+  // peer stores to be acknowledged: about one NVLink round trip at the tail of the launch.
   __syncthreads();
   if (threadIdx.x == 0) {
     __threadfence_system();

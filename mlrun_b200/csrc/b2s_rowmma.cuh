@@ -1,7 +1,6 @@
 // b2s_rowmma.cuh -- linear path, round 2: the dot products on the FP64 tensor-core instruction (DMMA m8n8k4).
 //
-// Why: `rowthread_kernel` is issue bound on the metric workload (72 % issue-active at 78 % of the HBM roofline,
-// profiles/ncu_r1p_rowthread_flow3_ens4.txt): 8 DFMA + 7.6 LDCU warp-instructions per event for 64 columns x 4 scores, one
+// Why: `rowthread_kernel` can be issue bound on the metric workload: 8 DFMA + 7.6 LDCU warp-instructions per event for 64 columns x 4 scores, one
 // constant-bank fetch per DFMA.  One `mma.sync.m8n8k4.f64` does 8 events x 4 columns x 8 scores (256 exact fp64 FMAs),
 // with the weights resident in registers as B fragments: 2 warp-instructions per event instead of 15.6, same IEEE fp64
 // arithmetic (every product and sum is a fused fp64 multiply-add; only the order of the additions differs).

@@ -1,4 +1,4 @@
-// b2s_rowwarp.cuh -- the HBM-bound linear path: a register-resident "row-warp" kernel (sm_100a).
+// b2s_rowwarp.cuh -- the HBM-bound linear path: a register-resident "row-warp" kernel (sm_90a).
 //
 // Imputer -> OneHotEncoder -> {linear scorers} -> vote is a (B x F)·(F x NS) product with a tiny NS
 // (1..8 scores), i.e. a streaming, HBM-bound row reduction -- not GEMM-shaped work, so no tensor cores.

@@ -376,7 +376,7 @@ struct RTTables {  // what rt_build needs from finalize
   const int32_t* d_classes;
 };
 
-// threads per row: measured on B200 (profiles/r1_kernel_log.md): 2 beats 1 (more warps) and 4 (combine overhead)
+// threads per row: 2 for wide rows (more warps than 1, less combine overhead than 4); B2S_RT_TPR overrides it for A/B runs
 constexpr int rt_tpr(int NCH) { return NCH >= 8 ? 2 : 1; }
 
 template <int NCH, int NS>
@@ -1445,7 +1445,7 @@ extern "C" int b2s_plan_finalize(b2s_plan_t p) {
         }
       }
     }
-    // ---- dense head (tcgen05): linear scorers with more than 8 scores in total over plain numeric columns.  The float64
+    // ---- dense head (wgmma): linear scorers with more than 8 scores in total over plain numeric columns.  The float64
     // coefficients become three tf32 terms wh + wm + wl (11 significant bits each, 33 in total); W^T rows padded to 16 / 32
     std::vector<float> dense_wh, dense_wm, dense_wl;
     int dense_pad = 0;
@@ -1546,7 +1546,6 @@ extern "C" int b2s_plan_finalize(b2s_plan_t p) {
       d.n_in = n_in;
       d.n_scores = total_scores;
       d.n_pad = dense_pad;
-      d.tmem_cols = dense_tmem_cols(n_in, dense_pad);
       d.exact = (getenv("B2S_DENSE_EXACT") && atoi(getenv("B2S_DENSE_EXACT")) != 0) ? 1 : 0;
       d.any_fill = any_fill ? 1 : 0;
       for (int kk = 0; kk < 32; ++kk) {
@@ -1571,7 +1570,7 @@ extern "C" int b2s_plan_finalize(b2s_plan_t p) {
       }
       p->dense_smem = dense_smem_bytes(n_in, dense_pad);
       if (p->dense_smem <= (int)G.prop.sharedMemPerBlockOptin) {
-        p->dense_grid = G.prop.multiProcessorCount;  // persistent: one CTA per SM (its shared memory and TMEM see to that)
+        p->dense_grid = G.prop.multiProcessorCount;  // persistent: one CTA per SM (its shared memory sees to that)
         p->dense_ok = true;
       }
     }
@@ -1744,7 +1743,7 @@ extern "C" int b2s_plan_finalize(b2s_plan_t p) {
         if (p->rt_smem <= smem_cap && rt_launch(p, nullptr, 0, 0, nullptr, nullptr, 0, nullptr, true, &occ) == cudaSuccess && occ >= 1) {
           p->rt_ok = true;
           p->rt_grid = sms * occ;
-          // DMMA variant, opt-in with B2S_RT_MMA=1 (measured slower than the DFMA kernel: profiles/r2_kernel_log.md): 32 or 64
+          // DMMA variant, opt-in with B2S_RT_MMA=1 (the DFMA kernel is the default): 32 or 64
           // float32 columns, tensor-map loads
           const char* mma_env = getenv("B2S_RT_MMA");
           if (mma_env && atoi(mma_env) != 0 && (p->rt_NCH == 8 || p->rt_NCH == 16) && n_in == p->rt_NCH * 4 && tensor_map_encoder()) {
@@ -1892,7 +1891,7 @@ extern "C" const char* b2s_plan_kernel(b2s_plan_t p) {
   static thread_local char buf[200];
   int lm = rt_load_mode();
   if (lm == 2 && !(p->rt_NCH >= 8 && p->n_in == p->rt_NCH * 4 && tensor_map_encoder())) lm = 1;
-  if (p->dense_ok) snprintf(buf, sizeof(buf), "dense_head_kernel<N=%d> (tcgen05.mma kind::tf32, %s, TMEM accumulator groups; %d scores over %d columns)", p->dense.n_pad, p->dense.exact ? "exact 3-term input split" : "2-term input split", p->dense.n_scores, p->dense.n_in);
+  if (p->dense_ok) snprintf(buf, sizeof(buf), "dense_head_kernel<N=%d> (wgmma tf32, %s, register accumulator groups; %d scores over %d columns)", p->dense.n_pad, p->dense.exact ? "exact 3-term input split" : "2-term input split", p->dense.n_scores, p->dense.n_in);
   else if (p->t3_ok) snprintf(buf, sizeof(buf), "t3_prep_kernel + trees3_kernel<D=%d,%s> + t3_vote_kernel (%d parts resident in shared memory, %d walking warps%s)", p->t3_D, p->t3_miss ? "NaN routing" : "floats", p->t3_parts, p->t3.warps, p->t3_top ? ", top levels in the constant bank" : "");
   else if (p->t2_ok) snprintf(buf, sizeof(buf), "trees_model_kernel<%d> + vote_kernel (models resident in shared memory)", p->t2_NS);
   else if (p->rt_ok && p->rm_ok && lm == 2) snprintf(buf, sizeof(buf), "rowmma_kernel<NCH=%d,NS=%d> (DMMA m8n8k4 fp64, %d warps x %d stages of 32-row TMA tiles per SM)", p->rt_NCH, p->rt_NS, p->rm_warps, p->rm_stages);
@@ -1961,7 +1960,7 @@ static int launch_on(b2s_plan_t p, const void* d_rows, int64_t n_rows, int64_t s
       k.sig.timeout_ns = fused_timeout_ns;
       c->fused_epoch = k.sig.wait_epoch;
     }
-    // lab switches (profiles/lab/comm_lab.py): which part of a merged step costs what.  Results are NOT merged with them.
+    // lab switches: which part of a merged step costs what.  Results are NOT merged with them.
     static const int lab_selfonly = getenv("B2S_LAB_COMM_SELFONLY") ? atoi(getenv("B2S_LAB_COMM_SELFONLY")) : 0;
     static const int lab_nosignal = getenv("B2S_LAB_COMM_NOSIGNAL") ? atoi(getenv("B2S_LAB_COMM_NOSIGNAL")) : 0;
     if (lab_selfonly) {
@@ -2203,7 +2202,7 @@ extern "C" int b2s_run_host(b2s_plan_t p, const void* rows, int64_t n_rows, int6
     // Large pinned batches run as a pipeline of chunks: chunk c+1 crosses PCIe while chunk c is computed, copied back and
     // post-processed on the host, so the call costs about one H2D of the batch.  (Not with merge targets: their row offset
     // is per launch.)
-    static const int64_t pipe_rows = getenv("B2S_HOST_CHUNK") ? atoll(getenv("B2S_HOST_CHUNK")) : 65536;  // measured: 16Ki 162, 32Ki 184, 64Ki 189 M events/s (one piece: 169)
+    static const int64_t pipe_rows = getenv("B2S_HOST_CHUNK") ? atoll(getenv("B2S_HOST_CHUNK")) : 65536;
     if (pinned && pipe_rows > 0 && n_rows >= 2 * pipe_rows && p->peers.empty()) {
       // whole tiles per chunk keep every chunk's base 16-byte (and tensor-map) aligned
       const int64_t chunk = (int64_t)align_up((size_t)std::max<int64_t>(pipe_rows, (n_rows + 63) / 64), 1024);

@@ -1,4 +1,4 @@
-// b2s_table.cu -- device-resident online feature table: entity key -> feature vector (+ imputing), sm_100a.
+// b2s_table.cu -- device-resident online feature table: entity key -> feature vector (+ imputing), sm_90a.
 //
 // Replaces the lookup half of real-time feature enrichment: EnrichmentModelRouter / EnrichmentVotingEnsemble.preprocess
 // (mlrun/serving/routers.py:1189-1196, 1335-1342) call OnlineVectorService.get (mlrun/feature_store/feature_vector.py:

@@ -1,4 +1,4 @@
-// b2s_trees2.cuh -- tree-ensemble scorer with the model resident in shared memory (sm_100a).
+// b2s_trees2.cuh -- tree-ensemble scorer with the model resident in shared memory (sm_90a).
 //
 // A root->leaf walk is a chain of dependent gathers; from L2 (the generic kernel, tables ~1 MB for
 // 4 x 100 depth-6 trees) every level costs ~250 cycles.  Here each persistent CTA owns ONE model of the

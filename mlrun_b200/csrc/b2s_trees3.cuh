@@ -1,6 +1,6 @@
-// b2s_trees3.cuh -- tree-ensemble scorer, round 2 (sm_100a): "parts" resident in shared memory.
+// b2s_trees3.cuh -- tree-ensemble scorer, round 2 (sm_90a): "parts" resident in shared memory.
 //
-// What bounds a root->leaf walk (measured on B200, profiles/r2/trees_lab_r2a*.{txt,csv}): with the model in shared memory
+// What bounds a root->leaf walk: with the model in shared memory
 // and the event tile transposed (xt[feature][row], lanes = 32 consecutive rows walking the same tree) every LDS is
 // conflict free, and the kernel runs exactly at the LSU limit of one 128-byte shared-memory wavefront per cycle and
 // SM -- issue slots are 35-40 % busy.  So the design minimises *wavefronts per visit* and keeps the LSU queue full:
@@ -12,7 +12,7 @@
 //   * nothing but walks runs on the LSU of the walking kernel: the transpose is a kernel of its own (below), tiles arrive
 //     by TMA bulk copies, and the only synchronisation is two mbarriers per tile buffer (no CTA-wide barrier).
 //   (Rounds of this file that transposed inside the walking CTA -- in phases, then with producer warps -- lost 35-40 % of
-//   the LSU cycles to barrier stalls and to loads of the producers queueing behind the walkers': profiles/r2/.)
+//   the LSU cycles to barrier stalls and to loads of the producers queueing behind the walkers'.)
 //
 // Three launches per batch:
 //   t3_prep_kernel   rows (row-major, HBM) -> TMA boxes / cp.async -> transpose in shared memory (+ Imputer, + the non-finite

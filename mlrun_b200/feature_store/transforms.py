@@ -1,4 +1,4 @@
-"""Feature-store transform steps of the B200 engine (plugin-API mirror of mlrun.feature_store.steps).
+"""Feature-store transform steps of the H100 engine (plugin-API mirror of mlrun.feature_store.steps).
 
 Each step is *declarative*: it holds the same constructor arguments as the reference class
 (mlrun/feature_store/steps.py) and is lowered by `mlrun_b200.lowering.ColumnProgram` into a device

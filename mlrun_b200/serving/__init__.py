@@ -1,4 +1,4 @@
-"""mlrun_b200.serving -- drop-in names of mlrun.serving, backed by the B200 engine"""
+"""mlrun_b200.serving -- drop-in names of mlrun.serving, backed by the H100 engine"""
 from .device_models import (  # noqa: F401
     FeatureRowModelServer,
     FeatureRowVotingEnsemble,

@@ -1,4 +1,4 @@
-"""Serving-graph topology and the per-event executors of the B200 engine.
+"""Serving-graph topology and the per-event executors of the H100 engine.
 
 Plugin-API mirror of mlrun/serving/states.py: the same step kinds, builder calls (`to`, `add_step`,
 `add_route`, `error_handler`, `respond`, `set_flow`), wire format (`to_dict` / `from_dict`) and per-event

@@ -1,4 +1,4 @@
-"""Serving host of the B200 engine: GraphContext, GraphServer, mock streams, nuclio-style hooks.
+"""Serving host of the H100 engine: GraphContext, GraphServer, mock streams, nuclio-style hooks.
 
 Plugin-API mirror of mlrun/serving/server.py (GraphServer :86-312, v2_serving_init/handler :315-409,
 create_graph_server :412-434, GraphContext :493-602).  On top of the reference surface the server

@@ -5,8 +5,12 @@ all-zero rows), random impute policies ("*" and per-feature constants and $mean 
 and label features), with and without label column / index columns, single and composite keys; lookups as lists, dicts, a
 single dict, unknown keys, extra columns, malformed asks.  Results, impute tables and exceptions compared.
 
-    python -m tests.golden.diff_online
+    python -m tests.golden.diff_online             # live, needs the reference sources importable (tests/golden/_refshim.py)
+    python -m tests.golden.diff_online --record    # live, and store the reference's answers in ref_online.json.xz
+    python -m tests.golden.diff_online --golden    # against the stored answers: runs anywhere
 """
+import json
+import lzma
 import os
 import random
 import sys
@@ -15,7 +19,6 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspa
 import pandas as pd  # noqa: E402
 
 from tests import api_oracle as ora  # noqa: E402
-from tests.golden import api_reference as ref  # noqa: E402
 from tests.scenarios import _first_line  # noqa: E402
 
 
@@ -38,9 +41,12 @@ def attempt(fn):
         return {"raised": type(exc).__name__, "message": _first_line(str(exc))}
 
 
-def main():
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "ref_online.json.xz")
+
+
+def cases():
+    """the 500 seeded services and lookups, in order"""
     rnd = random.Random(23)
-    n = 0
     for case in range(500):
         nf = rnd.randint(1, 6)
         feats = [f"f{i}" for i in range(nf)]
@@ -69,25 +75,58 @@ def main():
         with_idx = rnd.random() < 0.3
         keys = list(table) + [("nobody", 9) if composite else ("nobody",)]
         asks = [list(rnd.choice(keys)) for _ in range(rnd.randint(1, 4))]
-        out = []
-        for api in (ref, ora):
-            def go(api=api):
-                svc = api.online_service(feats, index, table, stats, label, with_idx, policy)
-                res = {"impute": norm(dict(svc._impute_values)),
-                       "lists": attempt(lambda: svc.get(asks, as_list=True)),
-                       "dicts": attempt(lambda: svc.get([dict(zip(index, a)) for a in asks])),
-                       "one": attempt(lambda: svc.get(dict(zip(index, asks[0])))),
-                       "extra": attempt(lambda: svc.get([{**dict(zip(index, asks[0])), "note": 1}])),
-                       "short": attempt(lambda: svc.get([asks[0][:1]])) if composite else None,
-                       "empty": attempt(lambda: svc.get([])), "string": attempt(lambda: svc.get("k0"))}
-                return res
-            out.append(repr(attempt(go)))
+        yield case, (feats, label, index, table, stats, policy, with_idx, asks, composite)
+
+
+def run(api, feats, label, index, table, stats, policy, with_idx, asks, composite):
+    """repr of everything one service answers (results, impute table, exceptions)"""
+    def go():
+        svc = api.online_service(feats, index, table, stats, label, with_idx, policy)
+        res = {"impute": norm(dict(svc._impute_values)),
+               "lists": attempt(lambda: svc.get(asks, as_list=True)),
+               "dicts": attempt(lambda: svc.get([dict(zip(index, a)) for a in asks])),
+               "one": attempt(lambda: svc.get(dict(zip(index, asks[0])))),
+               "extra": attempt(lambda: svc.get([{**dict(zip(index, asks[0])), "note": 1}])),
+               "short": attempt(lambda: svc.get([asks[0][:1]])) if composite else None,
+               "empty": attempt(lambda: svc.get([])), "string": attempt(lambda: svc.get("k0"))}
+        return res
+    return repr(attempt(go))
+
+
+def reference_outputs():
+    from tests.golden import api_reference as ref
+
+    return [run(ref, *args) for _case, args in cases()]
+
+
+def check(want_all):
+    n = 0
+    for (case, args), want in zip(cases(), want_all, strict=True):
+        mine = run(ora, *args)
         n += 1
-        if out[0] != out[1]:
-            print("DIFF", case, feats, label, index, table, policy, with_idx, asks)
-            print("  ref :", out[0][:1200])
-            print("  mine:", out[1][:1200])
+        if want != mine:
+            print("DIFF", case, *args[:4], *args[5:])
+            print("  ref :", want[:1200])
+            print("  mine:", mine[:1200])
+            return None
+    return n
+
+
+def main():
+    if "--golden" in sys.argv:  # the reference's answers as recorded by --record: no reference tree needed
+        with lzma.open(GOLDEN, "rt") as f:
+            n = check(json.load(f))
+        if n is None:
             return 1
+        print("identical on", n, "random online services (recorded reference answers)")
+        return 0
+    want = reference_outputs()
+    if "--record" in sys.argv:
+        with lzma.open(GOLDEN, "wt") as f:
+            json.dump(want, f)
+    n = check(want)
+    if n is None:
+        return 1
     print("identical on", n, "random online services")
     return 0
 

@@ -6,8 +6,8 @@
 4 x GradientBoostingRegressor(n_estimators=100, max_depth=6, random_state=30+i) and 4 x GradientBoostingClassifier (3
 classes: terciles of y) fit on 20 000 synthetic rows of 128 float32 features, all features considered at every split,
 y = 2*x0 + sin(x1) + x2*x3 + eps.  Fitting takes ~1.2 s per tree, far too long for a test or a bench run, so the fitted
-scikit-learn estimators are stored (cloudpickle + xz; per-node training statistics that predict() never reads are zeroed so
-the files compress to a few MB).  The oracle at test time is still scikit-learn's own predict() on these very objects.
+scikit-learn estimators are stored (cloudpickle + xz; per-node training statistics and split-node values that predict() never
+reads are zeroed so that each file compresses to less than 1 MB).  The oracle at test time is still scikit-learn's own predict() on these very objects.
 """
 
 import lzma
@@ -30,12 +30,16 @@ def fit_data(n_feat=N_FEAT):
 
 
 def _slim(tree):
-    """zero the training statistics of a fitted sklearn Tree (predict / apply never read them)"""
+    """zero the training statistics of a fitted sklearn Tree and the values of its split nodes (predict / apply read the
+    values of leaves only)"""
     state = tree.__getstate__()
     nodes = state["nodes"].copy()
     for field in ("impurity", "n_node_samples", "weighted_n_node_samples"):
         nodes[field] = 0
     state["nodes"] = nodes
+    values = state["values"].copy()
+    values[nodes["left_child"] != -1] = 0
+    state["values"] = values
     tree.__setstate__(state)
 
 

@@ -1,6 +1,8 @@
 // ring_tsan.cpp -- ThreadSanitizer harness for the host side of the coalescing ring (b2s_submit / b2s_wait / b2s_flush,
-// the dispatcher thread) with b2s_run_host running beside it.  Built by profiles/lab/build_tsan.sh against a
-// -fsanitize=thread build of the library; run on a GPU box:  TSAN_OPTIONS="halt_on_error=0" ./ring_tsan
+// the dispatcher thread) with b2s_run_host running beside it.  Built against a -fsanitize=thread build of the library
+// (every unit of mlrun_b200/csrc compiled with `nvcc -gencode arch=compute_90a,code=sm_90a -O1 -g -std=c++17
+// -Xcompiler -fPIC,-fsanitize=thread`, linked with -ltsan), then `g++ -std=c++17 -O1 -g -fsanitize=thread ring_tsan.cpp
+// -lb200serve_tsan -lcudart -lpthread`; run on a GPU machine:  TSAN_OPTIONS="halt_on_error=0" ./ring_tsan
 // Every result is also checked against a single-threaded b2s_run_host of the same rows.
 #include <atomic>
 #include <chrono>

@@ -1,5 +1,5 @@
-"""Dense linear head on the tensor cores (csrc/b2s_dense.cu: tcgen05.mma kind::tf32 over split operands, TMEM accumulator
-groups) vs scikit-learn's own predict().  Needs a B200: `-m gpu`.  Scores rtol 1e-5 (+ atol 1e-5); labels exact (see the tie
+"""Dense linear head on the tensor cores (csrc/b2s_dense.cu: wgmma tf32 over split operands, register accumulator
+groups) vs scikit-learn's own predict().  Needs an H100: `-m gpu`.  Scores rtol 1e-5 (+ atol 1e-5); labels exact (see the tie
 note in the test)."""
 
 import numpy as np
@@ -44,7 +44,7 @@ def test_twelve_regressors_scores(n_rows):
     models = linear_models(12, 64, seed=1)
     X = np.random.default_rng(2).normal(size=(n_rows, 64)).astype(np.float32)
     plan = ColumnProgram(names(64)).build_plan([packing.pack_model(m) for m in models])
-    assert plan.kernel.startswith("dense_head_kernel<N=16> (tcgen05"), plan.kernel
+    assert plan.kernel.startswith("dense_head_kernel<N=16> (wgmma"), plan.kernel
     out, status = plan.run(X, with_status=True)
     want = np.stack([m.predict(X.astype(np.float64)) for m in models], axis=1)
     np.testing.assert_allclose(out, want, rtol=RTOL, atol=ATOL)
@@ -68,8 +68,8 @@ def test_error_against_float64_at_unit_scale(exact, monkeypatch):
     err = np.abs(out - want)
     print("dense head, exact=%d: max |err| %.3e, mean %.3e (max |score| %.1f)" % (exact, err.max(), err.mean(), np.abs(want).max()))
     np.testing.assert_allclose(out, want, rtol=RTOL, atol=ATOL)
-    # measured (r2l): max 9.3e-6 / 1.06e-5 (2-term / exact), mean 1.0e-6 / 0.94e-6 at scores up to |58.8| -- what is left is the
-    # fp32 arithmetic on the accumulators (float32 output rounding alone is 1.9e-6 there), not the input split
+    # what is left is the fp32 arithmetic on the accumulators (float32 output rounding alone is ~2e-6 at scores of ~60), not the
+    # input split
     assert err.max() < 2.5e-7 * np.abs(want).max() and err.mean() < 1.5e-6
 
 

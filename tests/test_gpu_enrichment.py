@@ -1,4 +1,4 @@
-"""Real-time feature enrichment on the device (b2s_table_* + the Enrichment routers) vs the oracle.  Needs a B200."""
+"""Real-time feature enrichment on the device (b2s_table_* + the Enrichment routers) vs the oracle.  Needs an H100."""
 
 import numpy as np
 import pandas as pd

@@ -1,4 +1,4 @@
-"""Feature-set ingest on the device (columns_kernel through the b2s_cols_* C-ABI) vs the oracle.  Needs a B200."""
+"""Feature-set ingest on the device (columns_kernel through the b2s_cols_* C-ABI) vs the oracle.  Needs an H100."""
 
 import contextlib
 import io

@@ -1,6 +1,6 @@
 """rowmma_kernel (fp64 tensor-core dot products, b2s_rowmma.cuh) against the oracle and against the DFMA row kernel it
 replaces: every (columns, scores) instantiation, ragged and tiny batches, NaN / out-of-vocabulary inputs, the generic
-epilogue (classifier links + majority vote), row status.  Needs a B200: `-m gpu`.
+epilogue (classifier links + majority vote), row status.  Needs an H100: `-m gpu`.
 
 Tolerance: rtol 1e-5 + atol 1e-5 against the float64 oracle (both kernels compute exact-product fp64 FMAs; they differ in the
 order of the additions only, which the second half of each test bounds at a few float32 ulps of the result)."""
@@ -28,7 +28,7 @@ def _device():
 
 @pytest.fixture(autouse=True)
 def _opt_in(monkeypatch):
-    """the DMMA variant is opt-in (the DFMA row kernel measured faster on B200: profiles/r2_kernel_log.md)"""
+    """the DMMA variant is opt-in (the DFMA row kernel is the default)"""
     monkeypatch.setenv("B2S_RT_MMA", "1")
     yield
 

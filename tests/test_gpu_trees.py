@@ -1,4 +1,4 @@
-"""Round-2 tree path (csrc/b2s_trees3.cuh) vs the CPU oracles, through the C-ABI.  Needs a B200: `-m gpu`.
+"""Round-2 tree path (csrc/b2s_trees3.cuh) vs the CPU oracles, through the C-ABI.  Needs an H100: `-m gpu`.
 
 Scores rtol 1e-5 (+ atol 1e-5, the north_star's bound); labels, votes and status words exact.
 Oracles: scikit-learn's own predict() (oracle/batch.py) for sklearn estimators -- at BASELINE configs[2]'s full size from
