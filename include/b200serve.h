@@ -152,6 +152,22 @@ int b2s_plan_set_vote(b2s_plan_t plan, int32_t vote_kind, const double* weights,
 int b2s_plan_finalize(b2s_plan_t plan);
 /* name + template parameters of the kernel family the plan launches (diagnostics / bench provenance) */
 const char* b2s_plan_kernel(b2s_plan_t plan);
+/* The kernel family that served the plan's most recent launch (any entry point, any thread), after the run-time
+ * demotions b2s_plan_kernel cannot see: rows in mapped host memory (small b2s_run_host batches), rows that are not
+ * 16-byte aligned or strided, and a tensor map the driver refuses.  B2S_KERNEL_NONE before the first launch. */
+#define B2S_KERNEL_NONE 0
+#define B2S_KERNEL_DENSE 1             /* dense_head_kernel (wgmma tf32, TMA tensor-map loads)            */
+#define B2S_KERNEL_TREES3_TMAP 2       /* t3_prep_kernel with TMA tensor-map loads + trees3 + vote        */
+#define B2S_KERNEL_TREES3 3            /* the same with plain loads                                       */
+#define B2S_KERNEL_TREES2_TMAP 4       /* trees_model_kernel with TMA tensor-map loads + vote_kernel      */
+#define B2S_KERNEL_TREES2 5            /* the same with plain loads                                       */
+#define B2S_KERNEL_ROWTHREAD_TMA 6     /* rowthread / rowmma kernel, TMA tensor-map or bulk-copy loads    */
+#define B2S_KERNEL_ROWTHREAD_LDGSTS 7  /* rowthread kernel, cp.async loads from device memory             */
+#define B2S_KERNEL_ROWTHREAD_HOST 8    /* rowthread kernel, cp.async loads from mapped host memory        */
+#define B2S_KERNEL_ROWWARP 9           /* rowwarp_kernel                                                  */
+#define B2S_KERNEL_ROWS 10             /* generic rows_kernel (fp64, linear or trees)                     */
+#define B2S_KERNEL_STORE 11            /* rows_kernel of a transform-only plan                            */
+int32_t b2s_plan_last_kernel(b2s_plan_t plan);
 /* out_cols 4-byte words per output row; out_is_int != 0 when they are int32 labels */
 int b2s_plan_out_info(b2s_plan_t plan, int32_t* out_cols, int32_t* out_is_int);
 

@@ -203,6 +203,8 @@ struct b2s_plan_s {
   bool dense_ok = false;
   DenseParams dense{};
   int dense_smem = 0, dense_grid = 0;
+  // B2S_KERNEL_* of the most recent launch (launches may come from several threads: the last store wins)
+  std::atomic<int32_t> last_kernel{B2S_KERNEL_NONE};
   // round-2 tree kernel: parts resident in shared memory (b2s_trees3.cuh); scratch = partial sums, column-major
   bool t3_ok = false, t3_miss = false;
   int t3_D = 0, t3_grid = 0, t3_block = 0, t3_smem = 0, t3_cols = 0, t3_parts = 0;
@@ -537,6 +539,8 @@ static cudaError_t rt_launch_tt(b2s_plan_s* p, const void* rows, int64_t stride,
     mode = 1;
     rpt = 1;
   }
+  p->last_kernel.store(mode != 0 ? B2S_KERNEL_ROWTHREAD_TMA : (lc && lc->host_rows) ? B2S_KERNEL_ROWTHREAD_HOST : B2S_KERNEL_ROWTHREAD_LDGSTS,
+                       std::memory_order_relaxed);
   r.tile_rows = tr;
   const int64_t tiles = (n_rows + tr - 1) / tr;
   static const int grid_mul = getenv("B2S_RT_GRIDMUL") ? std::max(1, atoi(getenv("B2S_RT_GRIDMUL"))) : 1;  // CTA waves (1 = persistent)
@@ -1901,6 +1905,10 @@ extern "C" const char* b2s_plan_kernel(b2s_plan_t p) {
   return buf;
 }
 
+extern "C" int32_t b2s_plan_last_kernel(b2s_plan_t p) {
+  return p ? p->last_kernel.load(std::memory_order_relaxed) : B2S_KERNEL_NONE;
+}
+
 extern "C" int b2s_plan_out_info(b2s_plan_t p, int32_t* out_cols, int32_t* out_is_int) {
   try {  // no C++ exception crosses the C boundary
     if (!p || !p->finalized) return fail(B2S_ERR_STATE, "plan not finalized");
@@ -2000,6 +2008,7 @@ static int launch_on(b2s_plan_t p, const void* d_rows, int64_t n_rows, int64_t s
     memset(&tmap, 0, sizeof(tmap));
     static const int t3_tma = getenv("B2S_T3_TMA") ? atoi(getenv("B2S_T3_TMA")) : 1;
     pr.use_tmap = (t3_tma && !host_rows && pr.vec_ok && (p->n_in % 32) == 0 && encode_rows_map(&tmap, d_rows, n_rows, stride, p->n_in, kT3TR)) ? 1 : 0;
+    p->last_kernel.store(pr.use_tmap ? B2S_KERNEL_TREES3_TMAP : B2S_KERNEL_TREES3, std::memory_order_relaxed);
     const int resident = std::max(1, (int)G.prop.sharedMemPerMultiprocessor / std::max(p->t3_prep_smem + 1024, 1));
     const int pgrid = (int)std::max<int64_t>(1, std::min<int64_t>(n_tiles, (int64_t)G.prop.multiProcessorCount * std::min(resident, 4)));
     G.launches.fetch_add(3, std::memory_order_relaxed);
@@ -2053,6 +2062,7 @@ static int launch_on(b2s_plan_t p, const void* d_rows, int64_t n_rows, int64_t s
     memset(&tmap, 0, sizeof(tmap));
     static const int t2_tma = getenv("B2S_T2_TMA") ? atoi(getenv("B2S_T2_TMA")) : 1;
     t.use_tmap = (t2_tma && !host_rows && t.vec_ok && (p->n_in % 32) == 0 && encode_rows_map(&tmap, d_rows, n_rows, stride, p->n_in, t.tile_rows)) ? 1 : 0;
+    p->last_kernel.store(t.use_tmap ? B2S_KERNEL_TREES2_TMAP : B2S_KERNEL_TREES2, std::memory_order_relaxed);
     if (p->t2_NS == 1) trees_model_kernel<1><<<grid2, p->t2_block, p->t2_smem, st>>>(t, tmap);
     else trees_model_kernel<4><<<grid2, p->t2_block, p->t2_smem, st>>>(t, tmap);
     cudaError_t e2 = cudaGetLastError();
@@ -2072,6 +2082,7 @@ static int launch_on(b2s_plan_t p, const void* d_rows, int64_t n_rows, int64_t s
       const int64_t tiles = (n_rows + kDenseTileRows - 1) / kDenseTileRows;
       const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(p->dense_grid, tiles));
       G.launches.fetch_add(1, std::memory_order_relaxed);
+      p->last_kernel.store(B2S_KERNEL_DENSE, std::memory_order_relaxed);
       cudaError_t e = dense_launch(d, k, tmap, grid, p->dense_smem, (int)G.prop.sharedMemPerBlockOptin, st);
       if (e != cudaSuccess) return fail(B2S_ERR_CUDA, "dense head kernel launch failed: %s", cudaGetErrorString(e));
       return B2S_OK;
@@ -2098,6 +2109,7 @@ static int launch_on(b2s_plan_t p, const void* d_rows, int64_t n_rows, int64_t s
     const int64_t groups = (n_rows + (int64_t)u * rpw - 1) / ((int64_t)u * rpw);
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(p->rw_grid, (groups + 3) / 4));
     G.launches.fetch_add(1, std::memory_order_relaxed);
+    p->last_kernel.store(B2S_KERNEL_ROWWARP, std::memory_order_relaxed);
     cudaError_t e = launch_rw(p->rw_L, p->rw_CPL, p->rw_NS, p->rw_CS, r, grid, p->rw_smem, st);
     if (e != cudaSuccess) return fail(B2S_ERR_CUDA, "row-warp kernel launch failed: %s", cudaGetErrorString(e));
     return B2S_OK;
@@ -2112,6 +2124,7 @@ static int launch_on(b2s_plan_t p, const void* d_rows, int64_t n_rows, int64_t s
   }
   const int64_t tiles = (n_rows + k.tile_rows - 1) / k.tile_rows;
   const int grid = (int)std::min<int64_t>(p->grid, tiles);
+  p->last_kernel.store(p->mode == MODE_STORE ? B2S_KERNEL_STORE : B2S_KERNEL_ROWS, std::memory_order_relaxed);
   cudaError_t e = launch_plan(p, k, grid, block, st);
   if (e != cudaSuccess) return fail(B2S_ERR_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
   return B2S_OK;

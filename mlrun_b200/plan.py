@@ -148,6 +148,12 @@ class DevicePlan:
         return self._lib.b2s_plan_kernel(self._h).decode()
 
     @property
+    def last_kernel(self):
+        """which kernel family served the most recent launch (nat.KERNELS: "dense", "rows", "rowthread/tma", ...; None
+        before the first): unlike `kernel`, it shows the run-time fallbacks of small host batches and unaligned rows"""
+        return nat.KERNELS[self._lib.b2s_plan_last_kernel(self._h)]
+
+    @property
     def out_dtype(self):
         return np.int32 if self.out_is_int else np.float32
 

@@ -40,16 +40,21 @@ def linear_models(n_models, n_feat, seed, scale=1.0):
 
 @pytest.mark.parametrize("n_rows", [1, 127, 128, 129, 5000])
 def test_twelve_regressors_scores(n_rows):
-    """12 linear scorers over 64 columns: N = 16 on the tensor core; every model's prediction against X @ coef + intercept"""
+    """12 linear scorers over 64 columns: N = 16 on the tensor core for the 5000-row batch, the fp64 rows kernel for the
+    small ones; every model's prediction against X @ coef + intercept"""
     models = linear_models(12, 64, seed=1)
     X = np.random.default_rng(2).normal(size=(n_rows, 64)).astype(np.float32)
     plan = ColumnProgram(names(64)).build_plan([packing.pack_model(m) for m in models])
     assert plan.kernel.startswith("dense_head_kernel<N=16> (wgmma"), plan.kernel
     out, status = plan.run(X, with_status=True)
+    # up to 64 KB (256 rows) the kernels read the batch from pinned host memory: no TMA, so the fp64 rows kernel serves it
+    assert plan.last_kernel == ("rows" if n_rows <= 256 else "dense"), plan.last_kernel
     want = np.stack([m.predict(X.astype(np.float64)) for m in models], axis=1)
     np.testing.assert_allclose(out, want, rtol=RTOL, atol=ATOL)
     assert not status.any()
-    voted = ColumnProgram(names(64)).build_plan([packing.pack_model(m) for m in models], vote=(nat.VOTE_MEAN, [1 / 12] * 12)).run(X)
+    vplan = ColumnProgram(names(64)).build_plan([packing.pack_model(m) for m in models], vote=(nat.VOTE_MEAN, [1 / 12] * 12))
+    voted = vplan.run(X)
+    assert vplan.last_kernel == plan.last_kernel
     np.testing.assert_allclose(voted[:, 0], obatch.mean_vote(want, [1 / 12] * 12), rtol=RTOL, atol=ATOL)
 
 
@@ -64,6 +69,7 @@ def test_error_against_float64_at_unit_scale(exact, monkeypatch):
     plan = ColumnProgram(names(128)).build_plan([packing.pack_model(m) for m in models])
     assert "dense_head_kernel<N=16>" in plan.kernel and ("exact 3-term" in plan.kernel) == bool(exact), plan.kernel
     out = plan.run(X).astype(np.float64)
+    assert plan.last_kernel == "dense", plan.last_kernel
     want = np.stack([m.predict(X.astype(np.float64)) for m in models], axis=1)
     err = np.abs(out - want)
     print("dense head, exact=%d: max |err| %.3e, mean %.3e (max |score| %.1f)" % (exact, err.max(), err.mean(), np.abs(want).max()))
@@ -86,6 +92,7 @@ def test_sixteen_class_logistic_regression_labels():
     plan = ColumnProgram(names(64)).build_plan([packing.pack_model(model)])
     assert "dense_head_kernel<N=16>" in plan.kernel, plan.kernel
     out = plan.run(X)[:, 0]
+    assert plan.last_kernel == "dense", plan.last_kernel
     want = model.predict(X.astype(np.float64))
     # 3xTF32 scores sit within ~1e-6 of the float64 ones: a label can differ only where the two best classes are closer
     # than that, which no row of this workload is
@@ -111,6 +118,7 @@ def test_ensemble_of_classifiers_with_majority_vote_and_wide_rows():
     per = np.stack([m.predict(X.astype(np.float64)) for m in models], axis=1)
     assert np.array_equal(ColumnProgram(names(128)).build_plan(packed).run(X), per)
     assert np.array_equal(plan.run(X)[:, 0], obatch.majority_vote(per, [0.5, 0.3, 0.2]))
+    assert plan.last_kernel == "dense", plan.last_kernel
 
 
 def test_cancellation_and_large_magnitudes():
@@ -124,6 +132,7 @@ def test_cancellation_and_large_magnitudes():
     plan = ColumnProgram(names(32)).build_plan([packing.pack_model(m) for m in models])
     assert "dense_head_kernel" in plan.kernel
     out = plan.run(X)
+    assert plan.last_kernel == "dense", plan.last_kernel
     want = np.stack([m.predict(X.astype(np.float64)) for m in models], axis=1)
     # relative to the size of the terms that were summed (what any finite-precision dot product is bounded by)
     scale = np.abs(X.astype(np.float64)) @ np.abs(np.stack([m.coef_ for m in models], axis=1))
@@ -142,6 +151,7 @@ def test_imputer_and_flagged_rows():
     plan = prog.build_plan([packing.pack_model(m) for m in models])
     assert "dense_head_kernel" in plan.kernel
     out, status = plan.run(X, with_status=True)
+    assert plan.last_kernel == "dense", plan.last_kernel
     Xi = obatch.impute(X, names(64), mapping)
     ok = np.isfinite(Xi).all(axis=1)
     assert np.array_equal(status != 0, ~ok) and ok.sum() > 100 and (~ok).sum() > 100
@@ -165,6 +175,7 @@ def test_dense_head_beats_the_fp64_path_at_sixteen_scores(monkeypatch):
         assert ("dense_head_kernel" in plan.kernel) == (label == "dense"), plan.kernel
         plan.time_device([d_in.ptr], X.shape[0], 256, d_out.ptr, 5)
         times[label] = plan.time_device([d_in.ptr], X.shape[0], 256, d_out.ptr, 20) / 20
+        assert plan.last_kernel == ("dense" if label == "dense" else "rows"), plan.last_kernel
     os.environ.pop("B2S_DENSE", None)
     print("dense head %.4f ms vs fp64 rows kernel %.4f ms per 1 Mi events" % (times["dense"], times["fp64"]))
     assert times["dense"] < times["fp64"]
