@@ -161,10 +161,10 @@ const char* b2s_plan_kernel(b2s_plan_t plan);
 #define B2S_KERNEL_TREES3 3            /* the same with plain loads                                       */
 #define B2S_KERNEL_TREES2_TMAP 4       /* trees_model_kernel with TMA tensor-map loads + vote_kernel      */
 #define B2S_KERNEL_TREES2 5            /* the same with plain loads                                       */
-#define B2S_KERNEL_ROWTHREAD_TMA 6     /* rowthread / rowmma kernel, TMA tensor-map or bulk-copy loads    */
+#define B2S_KERNEL_ROWTHREAD_TMA 6     /* rowthread kernel, TMA tensor-map or bulk-copy loads             */
 #define B2S_KERNEL_ROWTHREAD_LDGSTS 7  /* rowthread kernel, cp.async loads from device memory             */
 #define B2S_KERNEL_ROWTHREAD_HOST 8    /* rowthread kernel, cp.async loads from mapped host memory        */
-#define B2S_KERNEL_ROWWARP 9           /* rowwarp_kernel                                                  */
+#define B2S_KERNEL_ROWWARP 9           /* retired (rowwarp_kernel): no longer returned                    */
 #define B2S_KERNEL_ROWS 10             /* generic rows_kernel (fp64, linear or trees)                     */
 #define B2S_KERNEL_STORE 11            /* rows_kernel of a transform-only plan                            */
 int32_t b2s_plan_last_kernel(b2s_plan_t plan);

@@ -26,9 +26,6 @@ namespace b2s {
 constexpr int kRTMaxCatCols = 16;
 constexpr int kRTCatsInline = 4;   // categories compared as constant operands
 constexpr int kRTMaxCats = 256;
-#ifndef RT_R2_MINB
-#define RT_R2_MINB 4  // resident CTAs the two-rows-per-thread variant is compiled for
-#endif
 
 template <int NCH, int NS>
 struct RTParams {
@@ -115,11 +112,13 @@ struct RowSwizzled {  // 2-D TMA boxes of 32 floats x TR rows, SWIZZLE_128B: chu
   }
 };
 
-// dot products of the chunks [CH0, CH1) of RPT rows with all NS weight columns (the weights, fills and limits
-// are constant-bank / uniform-register operands: with RPT = 2 each is fetched once for two rows)
-template <int NCH, int NS, int CH0, int CH1, int RPT, typename Row>
-__device__ __forceinline__ void rt_slice(const RTParams<NCH, NS>& p, const Row (&xr)[RPT], double (&acc)[RPT][NS]) {
-  constexpr int BATCH = RPT == 1 ? 4 : 2;  // chunks converted before their DFMAs are issued (ILP)
+// dot products of the chunks [CH0, CH1) of a row with all NS weight columns (the weights, fills and limits
+// are constant-bank / uniform-register operands).  The row is an array of RPT = 1 rows: this form compiles to the
+// same code as the kernel has always had; a scalar row changes its register allocation and stack frame.
+template <int NCH, int NS, int CH0, int CH1, typename Row>
+__device__ __forceinline__ void rt_slice(const RTParams<NCH, NS>& p, const Row (&xr)[1], double (&acc)[1][NS]) {
+  constexpr int RPT = 1;
+  constexpr int BATCH = 4;  // chunks converted before their DFMAs are issued (ILP)
 #pragma unroll
   for (int b = CH0; b < CH1; b += BATCH) {
     double xd[RPT][BATCH * 4];
@@ -175,9 +174,10 @@ __device__ __noinline__ int rt_cat_search(const RTParams<NCH, NS>& p, int cc, fl
 // one-hot columns Q0, Q0+TPR, ... of one row: "onehot(x) . w" is a gather from the shared-memory weight rows.
 // Fully unrolled with literal column slots (the caller's branch on the slice index is warp-uniform), so every
 // table entry is a constant-bank operand and the address arithmetic stays in the uniform datapath.
-template <int NCH, int NS, int Q0, int TPR, int RPT, typename Row>
-__device__ __forceinline__ void rt_cats(const RTParams<NCH, NS>& p, const Row (&xr)[RPT], const double* __restrict__ s_wcat,
-                                        double (&acc)[RPT][NS]) {
+template <int NCH, int NS, int Q0, int TPR, typename Row>
+__device__ __forceinline__ void rt_cats(const RTParams<NCH, NS>& p, const Row (&xr)[1], const double* __restrict__ s_wcat,
+                                        double (&acc)[1][NS]) {
+  constexpr int RPT = 1;
   constexpr int ITERS = (kRTMaxCatCols - Q0 + TPR - 1) / TPR;
   if (p.cats_fast) {  // integer codes first .. first + cnt - 1 in every column: no search, no per-column branch
     const char* wb = reinterpret_cast<const char*>(s_wcat);
@@ -236,9 +236,9 @@ __device__ __forceinline__ void rt_cats(const RTParams<NCH, NS>& p, const Row (&
 // slice q of a row: the dot products over its share of the LIVE leading chunks + its share of the one-hot columns.
 // The slice index is warp-uniform; each case has compile-time column indices (constant operands); the row's one-hot
 // columns are dealt round-robin to its threads.
-template <int NCH, int NS, int TPR, int LIVE, int RPT, typename Row>
-__device__ __forceinline__ void rt_row_slices(const RTParams<NCH, NS>& p, int q, const Row (&xr)[RPT], const double* __restrict__ s_wcat,
-                                              double (&acc)[RPT][NS]) {
+template <int NCH, int NS, int TPR, int LIVE, typename Row>
+__device__ __forceinline__ void rt_row_slices(const RTParams<NCH, NS>& p, int q, const Row (&xr)[1], const double* __restrict__ s_wcat,
+                                              double (&acc)[1][NS]) {
   static_assert(LIVE % TPR == 0, "live chunks must split evenly over the row's threads");
   constexpr int CPT = LIVE / TPR;
   if (TPR == 1 || q == 0) {
@@ -315,12 +315,12 @@ __device__ __noinline__ void rt_generic_epilogue(const RTParams<NCH, NS>& p, con
 }
 
 // LM: how tiles reach shared memory -- 0 LDGSTS (cp.async), 1 one TMA bulk copy per row, 2 TMA tensor-map boxes (swizzled)
-// RPT: rows per thread (2 only with LM = 2): a tile of TR rows is worked on by TR / RPT * TPR threads
-template <int NCH, int NS, int TPR, int LM, int RPT = 1>
-__global__ void __launch_bounds__(128 * TPR / RPT, RPT == 2 ? RT_R2_MINB : (TPR >= 4 ? 2 : (TPR == 2 ? 3 : 4)))
+// RPT = 1 row per thread: kept as an array of one row (see rt_slice); a tile of TR rows is worked on by TR * TPR threads
+template <int NCH, int NS, int TPR, int LM>
+__global__ void __launch_bounds__(128 * TPR, TPR >= 4 ? 2 : (TPR == 2 ? 3 : 4))
     rowthread_kernel(const __grid_constant__ RTParams<NCH, NS> p, const __grid_constant__ CUtensorMap tmap) {
+  constexpr int RPT = 1;
   static_assert(NCH % TPR == 0, "chunks must split evenly over the row's threads");
-  static_assert(RPT == 1 || LM == 2, "two rows per thread needs the tensor-map loader (one issuing thread)");
   constexpr int CPT = NCH / TPR;  // chunks per thread
   extern __shared__ __align__(16) unsigned char smem[];
   uint64_t* s_bar = reinterpret_cast<uint64_t*>(smem);  // 4 mbarriers (bulk variant); 64 bytes reserved

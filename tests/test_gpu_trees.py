@@ -96,9 +96,8 @@ def test_depths(depth, n_trees):
 
 
 @pytest.mark.parametrize("depth,routes_nan", [(3, False), (6, False), (5, True)])
-def test_top_levels_from_the_constant_bank_equal_the_shared_memory_walk(depth, routes_nan, monkeypatch):
-    """B2S_T3_TOPC=1: the walk reads heap nodes 1..7 of every tree from the launch parameters (constant bank) instead of
-    shared memory (the default; measured equal): same comparisons, same fp64 adds in the same order -> bit-identical outputs"""
+def test_shared_memory_walk_matches_sklearn(depth, routes_nan):
+    """depth 3 and 6, and depth 5 with NaN routed to each node's default child"""
     if routes_nan:
         from sklearn.ensemble import RandomForestRegressor
 
@@ -113,14 +112,9 @@ def test_top_levels_from_the_constant_bank_equal_the_shared_memory_walk(depth, r
         wl = tree_workload(n_rows=1500, n_feat=16, n_models=2, n_trees=20, depth=depth, seed=60 + depth, n_fit=3000)
         models, X = wl.models, wl.X
     packed = [packing.pack_model(m) for m in models]
-    monkeypatch.setenv("B2S_T3_TOPC", "1")
     plan = ColumnProgram(names(16)).build_plan(packed)
-    assert "top levels in the constant bank" in plan.kernel, plan.kernel
+    assert "trees3_kernel" in plan.kernel, plan.kernel
     got = plan.run(X)
-    monkeypatch.delenv("B2S_T3_TOPC")
-    shared = ColumnProgram(names(16)).build_plan(packed)
-    assert "constant bank" not in shared.kernel and "trees3_kernel" in shared.kernel, shared.kernel
-    assert np.array_equal(got, shared.run(X))
     np.testing.assert_allclose(got, np.stack([m.predict(X.astype(np.float64)) for m in models], axis=1), rtol=RTOL, atol=ATOL)
 
 
