@@ -121,7 +121,9 @@ int b2s_plan_add_linear_model(b2s_plan_t plan, const double* W, const double* b,
  *   feature[i] < 0 marks a leaf whose value is leaf_value[i]; otherwise go left when
  *   x[feature[i]] <= threshold[i] (sklearn: float32 x vs float64 threshold; thresholds are passed
  *   already rounded toward -inf to float32, which gives the identical decision).
- *   score[tree_slot[t]] += tree_scale[t] * leaf_value;  score[k] starts at init[k]. */
+ *   score[tree_slot[t]] += tree_scale[t] * leaf_value;  score[k] starts at init[k].
+ * Scores: 1..32 per model (tree or linear), as for b2s_plan_add_linear_model; a tree plan holds up to 16 such models, so
+ * up to 512 scores in all.  Every tree kernel holds one model's scores per row at a time. */
 int b2s_plan_add_tree_model(b2s_plan_t plan, int32_t n_trees, const int32_t* tree_offset /* n_trees+1 */,
                             const int32_t* feature, const float* threshold, const int32_t* left,
                             const int32_t* right, const double* leaf_value, const int32_t* tree_slot,

@@ -204,6 +204,8 @@ struct b2s_plan_s {
   int t3_prep_smem = 0;
   char* d_t3_blob = nullptr;
   const int32_t* d_t3_col_score = nullptr;
+  const int32_t* d_t3_col_order = nullptr;   // the columns by score (t3_vote_kernel)
+  const int32_t* d_t3_model_cols = nullptr;  // [n_models + 1] each model's range of d_t3_col_order
   // host staging for run_host
   char* h_stage_in = nullptr;
   char* h_stage_out = nullptr;
@@ -275,7 +277,7 @@ static cudaError_t launch_plan(b2s_plan_s* p, const KParams& kp, int grid, int b
   B2S_CASE(MODE_LINEAR, 1) B2S_CASE(MODE_LINEAR, 2) B2S_CASE(MODE_LINEAR, 4) B2S_CASE(MODE_LINEAR, 8)
   B2S_CASE(MODE_LINEAR, 16) B2S_CASE(MODE_LINEAR, 32)
   B2S_CASE(MODE_TREES, 1) B2S_CASE(MODE_TREES, 4) B2S_CASE(MODE_TREES, 8) B2S_CASE(MODE_TREES, 16)
-  B2S_CASE(MODE_STORE, 1)
+  B2S_CASE(MODE_TREES, 32) B2S_CASE(MODE_STORE, 1)
 #undef B2S_CASE
   return cudaErrorInvalidValue;
 }
@@ -711,7 +713,6 @@ extern "C" int b2s_plan_add_tree_model_ex(b2s_plan_t p, int32_t n_trees, const i
     if (nan_mode != B2S_NAN_ERROR && nan_mode != B2S_NAN_DEFAULT_CHILD) return fail(B2S_ERR_INVALID, "unknown nan_mode %d", nan_mode);  // no C++ exception crosses the C boundary
     if (int rc = check_build(p)) return rc;
     if (int rc = check_link(link, n_scores, classes ? n_classes : 0)) return rc;
-    if (n_scores > 16) return fail(B2S_ERR_UNSUPPORTED, "tree models support at most 16 scores");
     if ((int)p->models.size() >= kMaxModels) return fail(B2S_ERR_UNSUPPORTED, "more than %d models in one plan", kMaxModels);
     if (n_trees < 1) return fail(B2S_ERR_INVALID, "n_trees < 1");
     HostModel m;
@@ -976,6 +977,20 @@ static int t3_build(b2s_plan_s* p, const KParams& k, bool any_fill) {
   }
   const int P = (int)parts.size();
   if (P == 0 || P > sms) return B2S_OK;
+  // ---- the vote kernel's view of the columns: sorted by score (stable: each score keeps its column order), so that a
+  // model's columns are one range and the vote holds one model's scores at a time
+  std::vector<int32_t> col_order(col_score.size()), model_cols(M + 1, 0);
+  for (size_t c = 0; c < col_order.size(); ++c) col_order[c] = (int32_t)c;
+  std::stable_sort(col_order.begin(), col_order.end(), [&](int32_t a, int32_t b) { return col_score[a] < col_score[b]; });
+  {
+    int so = 0, i = 0;
+    for (int mi = 0; mi < M; ++mi) {
+      model_cols[mi] = i;
+      so += p->models[mi].n_scores;
+      while (i < (int)col_order.size() && col_score[col_order[i]] < so) ++i;
+    }
+    model_cols[M] = i;
+  }
   // ---- CTAs per part, proportional to cost (largest-remainder rounding, at least one each)
   std::vector<int> n_ctas(P, 1);
   {
@@ -1010,7 +1025,7 @@ static int t3_build(b2s_plan_s* p, const KParams& k, bool any_fill) {
     o_nodes[i] = tb.add(parts[i].nodes);
     o_leaves[i] = tb.add(parts[i].leaves);
   }
-  const size_t o_cols = tb.add(col_score);
+  const size_t o_cols = tb.add(col_score), o_order = tb.add(col_order), o_mcols = tb.add(model_cols);
   const size_t o_parts = align_up(tb.data.size(), 16);
   tb.data.resize(o_parts + sizeof(T3Part) * P);
   CUDA_TRY(cudaMalloc(&p->d_t3_blob, tb.data.size()));
@@ -1030,6 +1045,8 @@ static int t3_build(b2s_plan_s* p, const KParams& k, bool any_fill) {
   memcpy(tb.data.data() + o_parts, dev.data(), sizeof(T3Part) * P);
   CUDA_TRY(cudaMemcpy(p->d_t3_blob, tb.data.data(), tb.data.size(), cudaMemcpyHostToDevice));
   p->d_t3_col_score = (const int32_t*)(p->d_t3_blob + o_cols);
+  p->d_t3_col_order = (const int32_t*)(p->d_t3_blob + o_order);
+  p->d_t3_model_cols = (const int32_t*)(p->d_t3_blob + o_mcols);
 
   T3Params& t = p->t3;
   memset(&t, 0, sizeof(t));
@@ -1217,7 +1234,8 @@ extern "C" int b2s_plan_finalize(b2s_plan_t p) {
         so += m.n_scores;
       }
     } else if (p->mode == MODE_TREES) {
-      NS = max_scores <= 1 ? 1 : (max_scores <= 4 ? 4 : (max_scores <= 8 ? 8 : 16));
+      // one model's scores per thread: the largest model (check_link: at most kMaxScores) sets the instance
+      NS = max_scores <= 1 ? 1 : (max_scores <= 4 ? 4 : (max_scores <= 8 ? 8 : (max_scores <= 16 ? 16 : 32)));
       bias.assign(std::max(total_scores, 1), 0.0);
     }
     {
@@ -1765,7 +1783,7 @@ static int launch_on(b2s_plan_t p, const void* d_rows, int64_t n_rows, int64_t s
     e3 = t3_launch_walk(t, p->t3_D, p->t3_miss, p->t3_grid, p->t3_block, p->t3_smem, (int)G.prop.sharedMemPerBlockOptin, st);
     if (e3 != cudaSuccess) return fail(B2S_ERR_CUDA, "tree kernel launch failed: %s", cudaGetErrorString(e3));
     const int vgrid = (int)std::max<int64_t>(1, std::min<int64_t>(4 * G.prop.multiProcessorCount, (n_rows + 255) / 256));
-    e3 = t3_launch_vote(k, sc.pred, sc.rows, p->d_t3_col_score, C, sc.row_bad, vgrid, st);
+    e3 = t3_launch_vote(k, sc.pred, sc.rows, p->d_t3_col_score, p->d_t3_col_order, p->d_t3_model_cols, sc.row_bad, vgrid, st);
     if (e3 != cudaSuccess) return fail(B2S_ERR_CUDA, "vote kernel launch failed: %s", cudaGetErrorString(e3));
     return B2S_OK;
   }

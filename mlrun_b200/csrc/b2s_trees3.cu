@@ -43,9 +43,9 @@ cudaError_t t3_launch_walk(const T3Params& t, int depth, bool miss, int grid, in
   return cudaErrorInvalidValue;
 }
 
-cudaError_t t3_launch_vote(const KParams& k, const double* partial, int64_t col_stride, const int32_t* col_score, int n_cols,
-                           const int32_t* row_bad, int grid, cudaStream_t st) {
-  t3_vote_kernel<<<grid, 256, 0, st>>>(k, partial, col_stride, col_score, n_cols, row_bad);
+cudaError_t t3_launch_vote(const KParams& k, const double* partial, int64_t col_stride, const int32_t* col_score,
+                           const int32_t* col_order, const int32_t* model_cols, const int32_t* row_bad, int grid, cudaStream_t st) {
+  t3_vote_kernel<<<grid, 256, 0, st>>>(k, partial, col_stride, col_score, col_order, model_cols, row_bad);
   return cudaGetLastError();
 }
 

@@ -86,8 +86,8 @@ struct T3Params {         // trees3_kernel
 // launchers (b2s_trees3.cu: the kernels are compiled in their own translation unit)
 cudaError_t t3_launch_prep(const T3Prep& pr, const CUtensorMap& tmap, bool miss, int grid, int smem, int smem_optin, cudaStream_t st);
 cudaError_t t3_launch_walk(const T3Params& t, int depth, bool miss, int grid, int block, int smem, int smem_optin, cudaStream_t st);
-cudaError_t t3_launch_vote(const KParams& k, const double* partial, int64_t col_stride, const int32_t* col_score, int n_cols,
-                           const int32_t* row_bad, int grid, cudaStream_t st);
+cudaError_t t3_launch_vote(const KParams& k, const double* partial, int64_t col_stride, const int32_t* col_score,
+                           const int32_t* col_order, const int32_t* model_cols, const int32_t* row_bad, int grid, cudaStream_t st);
 
 #ifdef B2S_T3_KERNELS
 // explicit shared-window loads (32-bit addresses: no generic->shared conversion in the address arithmetic)
@@ -481,22 +481,28 @@ __global__ void __launch_bounds__(1024) trees3_kernel(const __grid_constant__ T3
   t3_walk_body<D, MISS, U>(p);
 }
 
-// Per row: scores = init + the model's columns of `partial` in column order, link, then the VotingEnsemble reduce.
+// Per row and model: scores = init + the model's columns of `partial`, link; then the VotingEnsemble reduce.
+// col_order lists the columns by score, in column order within a score; model m owns col_order[model_cols[m] ..
+// model_cols[m + 1]).  Only one model's scores are held at a time: check_link bounds those by kMaxScores, while the
+// plan's total (up to kMaxModels x kMaxScores) is not bounded.
 __global__ void __launch_bounds__(256) t3_vote_kernel(KParams kp, const double* __restrict__ partial, int64_t col_stride,
-                                                      const int32_t* __restrict__ col_score, int n_cols,
+                                                      const int32_t* __restrict__ col_score,
+                                                      const int32_t* __restrict__ col_order,
+                                                      const int32_t* __restrict__ model_cols,
                                                       const int32_t* __restrict__ row_bad) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; row < kp.n_rows; row += stride) {
-    double sc[kMaxScores];
-    for (int k = 0; k < kp.n_scores; ++k) sc[k] = kp.bias[k];
-    for (int c = 0; c < n_cols; ++c) {
-      const int k = col_score[c];
-      sc[k] = __dadd_rn(sc[k], partial[(int64_t)c * col_stride + row]);
-    }
     double pred[kMaxModels];
     for (int m = 0; m < kp.n_models; ++m) {
       const ModelDesc md = kp.models[m];
-      pred[m] = apply_link(md, sc + md.score_off, kp.classes);
+      double sc[kMaxScores];
+      for (int k = 0; k < md.n_scores; ++k) sc[k] = kp.bias[md.score_off + k];
+      for (int i = model_cols[m]; i < model_cols[m + 1]; ++i) {
+        const int c = col_order[i];
+        const int k = col_score[c] - md.score_off;
+        sc[k] = __dadd_rn(sc[k], partial[(int64_t)c * col_stride + row]);
+      }
+      pred[m] = apply_link(md, sc, kp.classes);
     }
     vote_and_store(kp, pred, row, row_bad[row] ? 1u : 0u);
   }
