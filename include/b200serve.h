@@ -148,6 +148,30 @@ int b2s_plan_add_tree_model_ex(b2s_plan_t plan, int32_t n_trees, const int32_t* 
                                const double* leaf_value, const int32_t* tree_slot, const double* tree_scale,
                                const double* init, int32_t n_scores, int32_t link, const int32_t* classes, int32_t n_classes,
                                int32_t cmp_mode, const uint8_t* default_left, int32_t nan_mode);
+/* The same with categorical splits (xgboost split_type 1, LightGBM decision_type "=="), in one canonical form the
+ * exporters (mlrun_b200/tree_formats.py) normalise both libraries to:
+ *   node_cat[i]    -1: a numeric node (the rules above);  s >= 0: node i tests x against set s, whose bitset is
+ *                  cat_words[cat_offsets[s] .. cat_offsets[s + 1]) -- code c is bit (c % 32) of word (c / 32);
+ *                  `threshold[i]` and `cmp_mode` do not apply to it;
+ *   the node sends x RIGHT iff x is a valid code whose bit is set, and LEFT otherwise: an invalid code, a code past the
+ *                  end of the set, and a value too large for int32 all go left.  NaN follows default_left[i] under
+ *                  B2S_NAN_DEFAULT_CHILD (LightGBM's exporter sets it: NaN takes LightGBM's right child, which it maps to
+ *                  the canonical left), and flags the row under B2S_NAN_ERROR, as for numeric nodes;
+ *   cat_mode       the model's valid codes: B2S_CAT_NONNEG: x >= 0 (xgboost common::Decision);  B2S_CAT_TRUNC:
+ *                  trunc(x) >= 0, i.e. x > -1 (LightGBM Tree::CategoricalDecision, x in (-1, 0) is code 0); the code
+ *                  is trunc(x) in both.
+ * Sets: n_sets entries, cat_offsets has n_sets + 1 non-decreasing entries from 0 to at most n_cat_words.  Each node's set
+ * index must lie in [0, n_sets), and a leaf must have node_cat -1; anything else is B2S_ERR_INVALID.  A model whose
+ * node_cat is NULL or all -1 behaves exactly as with b2s_plan_add_tree_model_ex. */
+#define B2S_CAT_NONNEG 0
+#define B2S_CAT_TRUNC 1
+int b2s_plan_add_tree_model_cat(b2s_plan_t plan, int32_t n_trees, const int32_t* tree_offset /* n_trees+1 */,
+                                const int32_t* feature, const float* threshold, const int32_t* left, const int32_t* right,
+                                const double* leaf_value, const int32_t* tree_slot, const double* tree_scale,
+                                const double* init, int32_t n_scores, int32_t link, const int32_t* classes, int32_t n_classes,
+                                int32_t cmp_mode, const uint8_t* default_left, int32_t nan_mode,
+                                const int32_t* node_cat, const int32_t* cat_offsets /* n_sets+1 */, int32_t n_sets,
+                                const uint32_t* cat_words, int32_t n_cat_words, int32_t cat_mode);
 /* VotingEnsemble reduce over the plan's models (weights in model order; fp64). */
 int b2s_plan_set_vote(b2s_plan_t plan, int32_t vote_kind, const double* weights, int32_t n_weights);
 /* Upload tables to HBM, pick kernels, size staging buffers.  After this the plan is immutable. */
@@ -169,6 +193,9 @@ const char* b2s_plan_kernel(b2s_plan_t plan);
 #define B2S_KERNEL_ROWWARP 9           /* retired (rowwarp_kernel): no longer returned                    */
 #define B2S_KERNEL_ROWS 10             /* generic rows_kernel (fp64, linear or trees)                     */
 #define B2S_KERNEL_STORE 11            /* rows_kernel of a transform-only plan                            */
+#define B2S_KERNEL_TREES3_CAT_TMAP 12  /* B2S_KERNEL_TREES3_TMAP, walk with categorical splits             */
+#define B2S_KERNEL_TREES3_CAT 13       /* B2S_KERNEL_TREES3, walk with categorical splits                  */
+#define B2S_KERNEL_ROWS_CAT 14         /* rows_kernel of a tree plan with categorical splits              */
 int32_t b2s_plan_last_kernel(b2s_plan_t plan);
 /* out_cols 4-byte words per output row; out_is_int != 0 when they are int32 labels */
 int b2s_plan_out_info(b2s_plan_t plan, int32_t* out_cols, int32_t* out_is_int);

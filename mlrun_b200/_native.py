@@ -23,10 +23,12 @@ VOTE_NONE, VOTE_MEAN, VOTE_MAJORITY = 0, 1, 2
 ROW_NONFINITE_INPUT, ROW_BAD_LABEL, ROW_UNKNOWN_KEY = 1, 2, 4
 CMP_LE, CMP_LT = 0, 1          # left when x <= threshold (scikit-learn, LightGBM) | x < threshold (xgboost)
 NAN_ERROR, NAN_DEFAULT_CHILD = 0, 1
+CAT_NONNEG, CAT_TRUNC = 0, 1   # a valid category code is x >= 0 (xgboost) | x > -1, trunc(x) >= 0 (LightGBM)
 COL_F32, COL_I32, COL_I64 = 0, 1, 2
 # B2S_KERNEL_* (b2s_plan_last_kernel) -> name
 KERNELS = {0: None, 1: "dense", 2: "trees3/tma", 3: "trees3", 4: "trees2/tma", 5: "trees2", 6: "rowthread/tma",
-           7: "rowthread/ldgsts", 8: "rowthread/host", 10: "rows", 11: "store"}
+           7: "rowthread/ldgsts", 8: "rowthread/host", 10: "rows", 11: "store", 12: "trees3_cat/tma", 13: "trees3_cat",
+           14: "rows_cat"}
 DATE_PARTS = {"year": 0, "month": 1, "day": 2, "hour": 3, "minute": 4, "second": 5, "day_of_week": 6, "dayofweek": 6,
               "weekday": 6, "day_of_year": 7, "dayofyear": 7, "quarter": 8, "is_leap_year": 9, "days_in_month": 10,
               "daysinmonth": 10, "is_month_start": 11, "is_month_end": 12, "is_quarter_start": 13, "is_quarter_end": 14,
@@ -74,6 +76,9 @@ SIGNATURES = {
                                           _i32, _i32, _pi32, _i32]),
     "b2s_plan_add_tree_model_ex": (C.c_int, [_vp, _i32, _pi32, _pi32, _pf32, _pi32, _pi32, _pf64, _pi32, _pf64, _pf64,
                                              _i32, _i32, _pi32, _i32, _i32, C.POINTER(C.c_uint8), _i32]),
+    "b2s_plan_add_tree_model_cat": (C.c_int, [_vp, _i32, _pi32, _pi32, _pf32, _pi32, _pi32, _pf64, _pi32, _pf64, _pf64,
+                                              _i32, _i32, _pi32, _i32, _i32, C.POINTER(C.c_uint8), _i32,
+                                              _pi32, _pi32, _i32, C.POINTER(C.c_uint32), _i32, _i32]),
     "b2s_plan_set_vote": (C.c_int, [_vp, _i32, _pf64, _i32]),
     "b2s_plan_finalize": (C.c_int, [_vp]),
     "b2s_plan_out_info": (C.c_int, [_vp, _pi32, _pi32]),

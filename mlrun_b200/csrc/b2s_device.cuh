@@ -34,10 +34,23 @@ struct MapEntry {  // MapValues entry: kind 0: v == a -> val ; kind 1: a <= v < 
 };
 
 struct TreeNode {  // 16 B: one LDG.128 per level
-  int32_t feature;  // < 0: leaf
-  float threshold;  // go left when x <= threshold
+  int32_t feature;  // < 0: leaf;  kTreeCatBit | f: a categorical split on column f
+  float threshold;  // go left when x <= threshold;  categorical: the bits are the word offset of its set (tree_cat_right)
   int32_t left, right;
 };
+
+// Categorical nodes of rows_kernel<TREES>.  The sets follow the node table, each as [header][words]: header = number of
+// 32-bit words | (bit 31) the model's code mode (B2S_CAT_TRUNC); `at` is the header's word offset from the start of the
+// table.  The node goes right iff x is a valid code whose bit is set.
+constexpr int32_t kTreeCatBit = 0x40000000;
+__device__ __forceinline__ bool tree_cat_right(const uint32_t* __restrict__ sets, uint32_t at, float x) {
+  const uint32_t hdr = __ldg(sets + at);
+  // valid codes: x >= 0 (xgboost) or x > -1, i.e. trunc(x) >= 0 (LightGBM); past the set (or past int32) is outside it
+  const float lo = (hdr >> 31) ? -0.99999994f : 0.0f;
+  if (!(x >= lo && x < __uint2float_rz(hdr & 0x7fffffffu) * 32.0f)) return false;
+  const int c = __float2int_rz(x);
+  return (__ldg(sets + at + 1 + (c >> 5)) >> (c & 31)) & 1u;
+}
 
 struct ModelDesc {
   int32_t kind;        // ModelKind
@@ -553,10 +566,17 @@ __global__ void __launch_bounds__(512) rows_kernel(const __grid_constant__ KPara
             for (int tr = md.tree_begin; tr < md.tree_end; ++tr) {
               int node = p.tree_root[tr];
               TreeNode nd = load_node(p.nodes + node);
-              // sklearn Tree.apply: go left when X[i, feature] <= threshold (float32 x)
-              while (nd.feature >= 0) {
-                const float x = xr[nd.feature];
-                node = (x <= nd.threshold) ? nd.left : nd.right;
+              for (;;) {
+                // sklearn Tree.apply: go left when X[i, feature] <= threshold (float32 x).  The unsigned compare also
+                // leaves the loop at a leaf (feature < 0) and at a categorical node
+                while ((uint32_t)nd.feature < (uint32_t)kTreeCatBit) {
+                  const float x = xr[nd.feature];
+                  node = (x <= nd.threshold) ? nd.left : nd.right;
+                  nd = load_node(p.nodes + node);
+                }
+                if (nd.feature < 0) break;
+                const float x = xr[nd.feature & (kTreeCatBit - 1)];
+                node = tree_cat_right(reinterpret_cast<const uint32_t*>(p.nodes), __float_as_uint(nd.threshold), x) ? nd.right : nd.left;
                 nd = load_node(p.nodes + node);
               }
               const double v = __dmul_rn(p.tree_scale[tr], __ldg(p.leaf + node));

@@ -101,6 +101,12 @@ struct HostModel {
   std::vector<double> leaf_value, tree_scale, init;
   std::vector<uint8_t> default_left;  // per node: a missing value (NaN) goes to the left child (empty: always right)
   bool nan_ok = false;                // the estimator routes NaN through its trees instead of refusing it
+  // categorical splits (b2s_plan_add_tree_model_cat), empty when the model has none: node_cat per node (-1: numeric),
+  // set s = cat_words[cat_off[s] .. cat_off[s + 1]); a node sends x right iff x is a valid code (cat_mode) whose bit is set
+  std::vector<int32_t> node_cat, cat_off;
+  std::vector<uint32_t> cat_words;
+  int cat_mode = B2S_CAT_NONNEG;
+  bool any_cat() const { return !node_cat.empty(); }
 };
 
 struct Slot {  // one in-flight batch of the coalescing ring
@@ -197,7 +203,8 @@ struct b2s_plan_s {
   // B2S_KERNEL_* of the most recent launch (launches may come from several threads: the last store wins)
   std::atomic<int32_t> last_kernel{B2S_KERNEL_NONE};
   // round-2 tree kernel: parts resident in shared memory (b2s_trees3.cuh); scratch = partial sums, column-major
-  bool t3_ok = false, t3_miss = false;
+  bool t3_ok = false, t3_miss = false, t3_cat = false;
+  bool any_cat = false;  // a tree model has categorical splits: trees3 <CAT = true>, or rows_kernel<TREES>
   int t3_D = 0, t3_grid = 0, t3_block = 0, t3_smem = 0, t3_cols = 0, t3_parts = 0;
   T3Params t3{};
   T3Prep t3_prep{};
@@ -703,6 +710,58 @@ static float threshold_for_less_than(float t) {
   return std::nextafterf(t, -std::numeric_limits<float>::infinity());
 }
 
+// largest set of one categorical node, in 32-bit words: the kernels compare x with the set's bit count as a float32
+constexpr int32_t kMaxCatWords = 1 << 20;
+
+extern "C" int b2s_plan_add_tree_model_cat(b2s_plan_t p, int32_t n_trees, const int32_t* tree_offset, const int32_t* feature,
+                                           const float* threshold, const int32_t* left, const int32_t* right,
+                                           const double* leaf_value, const int32_t* tree_slot, const double* tree_scale,
+                                           const double* init, int32_t n_scores, int32_t link, const int32_t* classes,
+                                           int32_t n_classes, int32_t cmp_mode, const uint8_t* default_left, int32_t nan_mode,
+                                           const int32_t* node_cat, const int32_t* cat_offsets, int32_t n_sets,
+                                           const uint32_t* cat_words, int32_t n_cat_words, int32_t cat_mode) {
+  try {
+    if (cmp_mode != B2S_CMP_LE && cmp_mode != B2S_CMP_LT) return fail(B2S_ERR_INVALID, "unknown cmp_mode %d", cmp_mode);
+    if (cat_mode != B2S_CAT_NONNEG && cat_mode != B2S_CAT_TRUNC) return fail(B2S_ERR_INVALID, "unknown cat_mode %d", cat_mode);
+    if (n_sets < 0 || n_cat_words < 0) return fail(B2S_ERR_INVALID, "negative n_sets %d or n_cat_words %d", n_sets, n_cat_words);
+    if (n_sets > 0 && !cat_offsets) return fail(B2S_ERR_INVALID, "%d sets without cat_offsets", n_sets);
+    if (n_cat_words > 0 && !cat_words) return fail(B2S_ERR_INVALID, "%d set words without cat_words", n_cat_words);
+    for (int s = 0; s < n_sets; ++s) {
+      if (cat_offsets[s] < 0 || cat_offsets[s + 1] < cat_offsets[s])
+        return fail(B2S_ERR_INVALID, "cat_offsets are not monotone at set %d (%d, %d)", s, cat_offsets[s], cat_offsets[s + 1]);
+      if (cat_offsets[s + 1] - cat_offsets[s] > kMaxCatWords)
+        return fail(B2S_ERR_UNSUPPORTED, "set %d has %d words (at most %d)", s, cat_offsets[s + 1] - cat_offsets[s], kMaxCatWords);
+    }
+    if (n_sets > 0 && cat_offsets[n_sets] > n_cat_words)
+      return fail(B2S_ERR_INVALID, "cat_offsets run past cat_words (%d > %d)", cat_offsets[n_sets], n_cat_words);
+    bool any = false;
+    if (node_cat) {
+      if (n_trees < 1 || !tree_offset) return fail(B2S_ERR_INVALID, "n_trees < 1");
+      const int nn = tree_offset[n_trees];
+      for (int i = 0; i < nn; ++i) {
+        if (node_cat[i] < -1 || node_cat[i] >= n_sets)
+          return fail(B2S_ERR_INVALID, "node %d: set index %d out of range [0, %d)", i, node_cat[i], n_sets);
+        if (node_cat[i] >= 0 && feature[i] < 0) return fail(B2S_ERR_INVALID, "node %d: a leaf marked categorical", i);
+        any |= node_cat[i] >= 0;
+      }
+    }
+    if (int rc = b2s_plan_add_tree_model_ex(p, n_trees, tree_offset, feature, threshold, left, right, leaf_value, tree_slot,
+                                            tree_scale, init, n_scores, link, classes, n_classes, cmp_mode, default_left, nan_mode))
+      return rc;
+    if (any) {  // a model without a categorical node is exactly what b2s_plan_add_tree_model_ex added
+      HostModel& m = p->models.back();
+      const int nn = tree_offset[n_trees];
+      m.node_cat.assign(node_cat, node_cat + nn);
+      m.cat_off.assign(cat_offsets, cat_offsets + n_sets + 1);
+      m.cat_words.assign(cat_words, cat_words + cat_offsets[n_sets]);
+      m.cat_mode = cat_mode;
+    }
+    return B2S_OK;
+  } catch (const std::exception& e) {
+    return fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
+  }
+}
+
 extern "C" int b2s_plan_add_tree_model_ex(b2s_plan_t p, int32_t n_trees, const int32_t* tree_offset, const int32_t* feature,
                                           const float* threshold, const int32_t* left, const int32_t* right,
                                           const double* leaf_value, const int32_t* tree_slot, const double* tree_scale,
@@ -822,6 +881,15 @@ static int t3_build(b2s_plan_s* p, const KParams& k, bool any_fill) {
   }
   if (!any_trees || n_lin_cols > kT3MaxLin) return B2S_OK;
   const bool miss = all_nan_ok;
+  // categorical sets: every part holds all the sets of its model (node word: 16-bit first word, 15-bit word count)
+  size_t cat_bytes = 0;
+  for (auto& m : p->models) {
+    if (!m.any_cat()) continue;
+    if (m.cat_off.back() > 0xffff) return B2S_OK;
+    for (size_t s = 0; s + 1 < m.cat_off.size(); ++s)
+      if (m.cat_off[s + 1] - m.cat_off[s] > 0x7fff) return B2S_OK;
+    cat_bytes = std::max(cat_bytes, align_up((size_t)m.cat_off.back() * 4, 16));
+  }
   const int NN = 1 << D;
   const int n_in4 = (int)align_up(n_in, 4);
   const int xt_words = n_in4 * TR;
@@ -833,7 +901,7 @@ static int t3_build(b2s_plan_s* p, const KParams& k, bool any_fill) {
   const size_t lin_bytes = (size_t)n_lin_cols * n_in * 8;
   // walking kernel: tables | two partial-sum buffers | two tiles (filled by TMA bulk copies) | four mbarriers
   auto fixed_bytes = [&](int w) {
-    return 2 * (size_t)std::max(w, kT3MaxLin) * TR * 8 + 2 * (size_t)xt_words * 4 + 128 /* tile alignment */ + 64;
+    return 2 * (size_t)std::max(w, kT3MaxLin) * TR * 8 + 2 * (size_t)xt_words * 4 + 128 /* tile alignment */ + 64 + cat_bytes;
   };
   auto capacity = [&](int w) {  // trees one CTA can hold with w walking warps (0: the plan does not fit at all)
     const size_t fixed = fixed_bytes(w);
@@ -878,7 +946,7 @@ static int t3_build(b2s_plan_s* p, const KParams& k, bool any_fill) {
   const int cap_trees = capacity(W);
   // ---- parts: per (tree model, score slot) the trees of that slot, split evenly when they exceed a CTA's capacity
   struct HostPart {
-    int model, slot, n_trees = 0, n_cols = 1, col0 = 0;
+    int model, slot, n_trees = 0, n_cols = 1, col0 = 0, n_cat_words = 0;
     std::vector<uint2> nodes;
     std::vector<double> leaves;
     double cost = 0.0;
@@ -929,7 +997,12 @@ static int t3_build(b2s_plan_s* p, const KParams& k, bool any_fill) {
                   const float thr = m.threshold[base + it.src];
                   const bool dl = !m.default_left.empty() && m.default_left[base + it.src] != 0;
                   nd.x = (uint32_t)(m.feature[base + it.src] * TR * 4) | ((miss && dl) ? 0x80000000u : 0u);
-                  if (miss) {
+                  const int cs = m.any_cat() ? m.node_cat[base + it.src] : -1;
+                  if (cs >= 0) {  // categorical: {first word, word count, code mode} of its set (b2s_trees3.cuh)
+                    nd.x |= 0x40000000u;
+                    nd.y = (uint32_t)m.cat_off[cs] | ((uint32_t)(m.cat_off[cs + 1] - m.cat_off[cs]) << 16) |
+                           (m.cat_mode == B2S_CAT_TRUNC ? 0x80000000u : 0u);
+                  } else if (miss) {
                     // the walk tests key(x) + d > key(t) + d with d = 1 for "missing goes left": NaN's key INT_MAX wraps
                     // to INT_MIN.  NaN threshold ("x < -inf" of an xgboost model): every value goes right
                     const uint32_t d = dl ? 1u : 0u;
@@ -942,6 +1015,11 @@ static int t3_build(b2s_plan_s* p, const KParams& k, bool any_fill) {
                 }
                 hp.nodes[(size_t)q * NN + it.heap] = nd;
               }
+            }
+            if (m.any_cat()) {  // the model's sets, right behind the node table (two words per uint2)
+              hp.n_cat_words = (int)m.cat_words.size();
+              for (size_t w = 0; w < m.cat_words.size(); w += 2)
+                hp.nodes.push_back(make_uint2(m.cat_words[w], w + 1 < m.cat_words.size() ? m.cat_words[w + 1] : 0u));
             }
             hp.cost = 0.5 + hp.n_trees * (2.0 + 3.0 * D) / 32.0 * 2.0;  // shared-memory wavefronts per row (the walks)
             hp.col0 = (int)col_score.size();
@@ -1040,6 +1118,7 @@ static int t3_build(b2s_plan_s* p, const KParams& k, bool any_fill) {
     d.col0 = parts[i].col0;
     d.cta0 = cta0;
     d.n_ctas = n_ctas[i];
+    d.n_cat_words = parts[i].n_cat_words;
     cta0 += n_ctas[i];
   }
   memcpy(tb.data.data() + o_parts, dev.data(), sizeof(T3Part) * P);
@@ -1070,6 +1149,7 @@ static int t3_build(b2s_plan_s* p, const KParams& k, bool any_fill) {
   t.sm_part = take(2 * (size_t)t.part_words * 8, 16);
   t.sm_xt = take(2 * (size_t)xt_words * 4, 128);
   t.sm_bar = take(64, 16);
+  if (cat_bytes > 0) t.sm_cat = take(cat_bytes, 16);
   if (n_lin_cols > 0) {
     // feature slices of the linear part: as many walking warps as fit -- either behind the weights, in the room the tree
     // parts use for their tables, or (small tree tables) in the per-warp partial-sum buffers
@@ -1118,6 +1198,7 @@ static int t3_build(b2s_plan_s* p, const KParams& k, bool any_fill) {
   p->t3_smem = (int)align_up(off, 16);
   p->t3_D = D;
   p->t3_miss = miss;
+  p->t3_cat = p->any_cat;
   p->t3_block = (W + kT3Service) * 32;
   p->t3_grid = cta0;
   p->t3_cols = (int)col_score.size();
@@ -1166,6 +1247,8 @@ extern "C" int b2s_plan_finalize(b2s_plan_t p) {
       // regression outputs voted as labels: allowed (VotingEnsemble casts to int, routers.py:778-780)
     }
     p->mode = M == 0 ? MODE_STORE : (any_tree ? MODE_TREES : MODE_LINEAR);
+    p->any_cat = false;
+    for (auto& m : p->models) p->any_cat = p->any_cat || m.any_cat();
     p->out_is_int = (M > 0 && (any_class || p->vote_kind == B2S_VOTE_MAJORITY)) ? 1 : 0;
     if (p->vote_kind == B2S_VOTE_MEAN) p->out_is_int = 0;
     p->out_cols = M == 0 ? n_out : (p->vote_kind == B2S_VOTE_NONE ? M : 1);
@@ -1197,6 +1280,7 @@ extern "C" int b2s_plan_finalize(b2s_plan_t p) {
     std::vector<ModelDesc> descs(std::max(M, 1));
     std::vector<int32_t> classes, tree_root, tree_slot;
     std::vector<TreeNode> nodes;
+    std::vector<uint32_t> tree_cat;  // rows_kernel<TREES>: the sets of the categorical nodes, [header][words] each
 
     if (p->mode == MODE_LINEAR) {
       NS = pow2_at_least(total_scores);
@@ -1255,6 +1339,12 @@ extern "C" int b2s_plan_finalize(b2s_plan_t p) {
           if (m.kind == MK_TREES) {
             d.tree_begin = (int)tree_root.size();
             const int nt = (int)m.tree_slot.size();
+            std::vector<uint32_t> set_at;
+            for (size_t s = 0; m.any_cat() && s + 1 < m.cat_off.size(); ++s) {
+              set_at.push_back((uint32_t)tree_cat.size());
+              tree_cat.push_back((uint32_t)(m.cat_off[s + 1] - m.cat_off[s]) | (m.cat_mode == B2S_CAT_TRUNC ? 0x80000000u : 0u));
+              tree_cat.insert(tree_cat.end(), m.cat_words.begin() + m.cat_off[s], m.cat_words.begin() + m.cat_off[s + 1]);
+            }
             for (int t = 0; t < nt; ++t) {
               const int base = (int)nodes.size();
               tree_root.push_back(base);
@@ -1266,6 +1356,10 @@ extern "C" int b2s_plan_finalize(b2s_plan_t p) {
                 nd.threshold = m.threshold[i];
                 nd.left = nd.feature >= 0 ? base + m.left[i] : 0;
                 nd.right = nd.feature >= 0 ? base + m.right[i] : 0;
+                if (m.any_cat() && m.node_cat[i] >= 0) {
+                  nd.feature |= kTreeCatBit;
+                  memcpy(&nd.threshold, &set_at[m.node_cat[i]], 4);
+                }
                 nodes.push_back(nd);
                 leaf.push_back(m.leaf_value[i]);
               }
@@ -1283,6 +1377,22 @@ extern "C" int b2s_plan_finalize(b2s_plan_t p) {
       }
     }
     if (bias.empty()) bias.assign(1, 0.0);
+    if (!tree_cat.empty()) {
+      // the sets follow the node table (tree_cat_right reads them through KParams::nodes): the categorical nodes' set
+      // indices become word offsets from the start of the table
+      const uint32_t base = (uint32_t)nodes.size() * 4u;
+      for (TreeNode& nd : nodes)
+        if (nd.feature >= kTreeCatBit) {
+          uint32_t at;
+          memcpy(&at, &nd.threshold, 4);
+          at += base;
+          memcpy(&nd.threshold, &at, 4);
+        }
+      tree_cat.resize(align_up(tree_cat.size(), 4), 0u);
+      const size_t n0 = nodes.size();
+      nodes.resize(n0 + tree_cat.size() / 4);
+      memcpy(nodes.data() + n0, tree_cat.data(), tree_cat.size() * 4);
+    }
 
     std::vector<uint8_t> chunk_kind((n_in + 3) / 4, 1);
     for (int ch = 0; ch < (int)chunk_kind.size(); ++ch) {
@@ -1546,7 +1656,7 @@ extern "C" int b2s_plan_finalize(b2s_plan_t p) {
       if (int rc = t3_build(p, k, any_fill)) return rc;
     }
     // ---- round-1 tree path, for the plans t3_build declines (trees deeper than kT3MaxDepth, or tables too large for it)
-    if (!p->t3_ok && p->mode == MODE_TREES && !need_expand) {
+    if (!p->t3_ok && p->mode == MODE_TREES && !need_expand && !p->any_cat) {  // trees_model_kernel has no categorical walk
       // re-pack every model as complete heap-ordered trees; one model must fit one CTA's shared memory
       bool ok = true;
       std::vector<int> depth(M, 0);
@@ -1668,10 +1778,10 @@ extern "C" const char* b2s_plan_kernel(b2s_plan_t p) {
   static thread_local char buf[200];
   const bool tmap = p->rt_NCH >= 8 && p->n_in == p->rt_NCH * 4 && tensor_map_encoder();
   if (p->dense_ok) snprintf(buf, sizeof(buf), "dense_head_kernel<N=%d> (wgmma tf32, %s, register accumulator groups; %d scores over %d columns)", p->dense.n_pad, p->dense.exact ? "exact 3-term input split" : "2-term input split", p->dense.n_scores, p->dense.n_in);
-  else if (p->t3_ok) snprintf(buf, sizeof(buf), "t3_prep_kernel + trees3_kernel<D=%d,%s> + t3_vote_kernel (%d parts resident in shared memory, %d walking warps)", p->t3_D, p->t3_miss ? "NaN routing" : "floats", p->t3_parts, p->t3.warps);
+  else if (p->t3_ok) snprintf(buf, sizeof(buf), "t3_prep_kernel + trees3_kernel<D=%d,%s%s> + t3_vote_kernel (%d parts resident in shared memory, %d walking warps)", p->t3_D, p->t3_miss ? "NaN routing" : "floats", p->t3_cat ? ",categorical" : "", p->t3_parts, p->t3.warps);
   else if (p->t2_ok) snprintf(buf, sizeof(buf), "trees_model_kernel<%d> + vote_kernel (models resident in shared memory)", p->t2_NS);
   else if (p->rt_ok) snprintf(buf, sizeof(buf), "rowthread_kernel<NCH=%d,NS=%d,TPR=%d,%s>", p->rt_NCH, p->rt_NS, rt_tpr(p->rt_NCH), tmap ? "TMA tensor-map loads" : "TMA bulk loads");
-  else snprintf(buf, sizeof(buf), "rows_kernel<%s,NS=%d>", p->mode == MODE_LINEAR ? "LINEAR" : (p->mode == MODE_TREES ? "TREES" : "STORE"), p->NS);
+  else snprintf(buf, sizeof(buf), "rows_kernel<%s,NS=%d>%s", p->mode == MODE_LINEAR ? "LINEAR" : (p->mode == MODE_TREES ? "TREES" : "STORE"), p->NS, p->any_cat ? " (categorical splits)" : "");
   return buf;
 }
 
@@ -1769,7 +1879,8 @@ static int launch_on(b2s_plan_t p, const void* d_rows, int64_t n_rows, int64_t s
     alignas(64) CUtensorMap tmap;
     memset(&tmap, 0, sizeof(tmap));
     pr.use_tmap = (!host_rows && pr.vec_ok && (p->n_in % 32) == 0 && encode_rows_map(&tmap, d_rows, n_rows, stride, p->n_in, kT3TR)) ? 1 : 0;
-    p->last_kernel.store(pr.use_tmap ? B2S_KERNEL_TREES3_TMAP : B2S_KERNEL_TREES3, std::memory_order_relaxed);
+    p->last_kernel.store(p->t3_cat ? (pr.use_tmap ? B2S_KERNEL_TREES3_CAT_TMAP : B2S_KERNEL_TREES3_CAT)
+                                   : (pr.use_tmap ? B2S_KERNEL_TREES3_TMAP : B2S_KERNEL_TREES3), std::memory_order_relaxed);
     const int resident = std::max(1, (int)G.prop.sharedMemPerMultiprocessor / std::max(p->t3_prep_smem + 1024, 1));
     const int pgrid = (int)std::max<int64_t>(1, std::min<int64_t>(n_tiles, (int64_t)G.prop.multiProcessorCount * std::min(resident, 4)));
     G.launches.fetch_add(3, std::memory_order_relaxed);
@@ -1780,7 +1891,7 @@ static int launch_on(b2s_plan_t p, const void* d_rows, int64_t n_rows, int64_t s
     t.n_rows = n_rows;
     t.partial = sc.pred;
     t.col_stride = sc.rows;
-    e3 = t3_launch_walk(t, p->t3_D, p->t3_miss, p->t3_grid, p->t3_block, p->t3_smem, (int)G.prop.sharedMemPerBlockOptin, st);
+    e3 = t3_launch_walk(t, p->t3_D, p->t3_miss, p->t3_cat, p->t3_grid, p->t3_block, p->t3_smem, (int)G.prop.sharedMemPerBlockOptin, st);
     if (e3 != cudaSuccess) return fail(B2S_ERR_CUDA, "tree kernel launch failed: %s", cudaGetErrorString(e3));
     const int vgrid = (int)std::max<int64_t>(1, std::min<int64_t>(4 * G.prop.multiProcessorCount, (n_rows + 255) / 256));
     e3 = t3_launch_vote(k, sc.pred, sc.rows, p->d_t3_col_score, p->d_t3_col_order, p->d_t3_model_cols, sc.row_bad, vgrid, st);
@@ -1867,7 +1978,7 @@ static int launch_on(b2s_plan_t p, const void* d_rows, int64_t n_rows, int64_t s
   }
   const int64_t tiles = (n_rows + k.tile_rows - 1) / k.tile_rows;
   const int grid = (int)std::min<int64_t>(p->grid, tiles);
-  p->last_kernel.store(p->mode == MODE_STORE ? B2S_KERNEL_STORE : B2S_KERNEL_ROWS, std::memory_order_relaxed);
+  p->last_kernel.store(p->mode == MODE_STORE ? B2S_KERNEL_STORE : (p->any_cat ? B2S_KERNEL_ROWS_CAT : B2S_KERNEL_ROWS), std::memory_order_relaxed);
   cudaError_t e = launch_plan(p, k, grid, block, st);
   if (e != cudaSuccess) return fail(B2S_ERR_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
   return B2S_OK;

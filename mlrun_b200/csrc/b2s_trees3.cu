@@ -23,21 +23,27 @@ cudaError_t t3_launch_prep(const T3Prep& pr, const CUtensorMap& tmap, bool miss,
   return cudaGetLastError();
 }
 
-template <int D, bool MISS, int U>
+template <int D, bool MISS, int U, bool CAT>
 static cudaError_t walk(const T3Params& t, int grid, int block, int smem, int smem_optin, cudaStream_t st) {
   static std::atomic<bool> attr{false};
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(trees3_kernel<D, MISS, U>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin);
+    cudaError_t e = cudaFuncSetAttribute(trees3_kernel<D, MISS, U, CAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin);
     if (e != cudaSuccess) return e;
     attr = true;
   }
-  trees3_kernel<D, MISS, U><<<grid, block, smem, st>>>(t);
+  trees3_kernel<D, MISS, U, CAT><<<grid, block, smem, st>>>(t);
   return cudaGetLastError();
 }
 
-cudaError_t t3_launch_walk(const T3Params& t, int depth, bool miss, int grid, int block, int smem, int smem_optin, cudaStream_t st) {
-#define B2S_T3_CASE(DD) \
-  if (depth == DD) return miss ? walk<DD, true, kT3U>(t, grid, block, smem, smem_optin, st) : walk<DD, false, kT3U>(t, grid, block, smem, smem_optin, st);
+// CAT = true only for plans with a categorical split: the other plans keep the walk without the set test
+cudaError_t t3_launch_walk(const T3Params& t, int depth, bool miss, bool cat, int grid, int block, int smem, int smem_optin, cudaStream_t st) {
+#define B2S_T3_CASE(DD)                                                                                                \
+  if (depth == DD) {                                                                                                   \
+    if (cat) return miss ? walk<DD, true, kT3U, true>(t, grid, block, smem, smem_optin, st)                            \
+                         : walk<DD, false, kT3U, true>(t, grid, block, smem, smem_optin, st);                          \
+    return miss ? walk<DD, true, kT3U, false>(t, grid, block, smem, smem_optin, st)                                    \
+                : walk<DD, false, kT3U, false>(t, grid, block, smem, smem_optin, st);                                  \
+  }
   B2S_T3_CASE(2) B2S_T3_CASE(3) B2S_T3_CASE(4) B2S_T3_CASE(5) B2S_T3_CASE(6) B2S_T3_CASE(7) B2S_T3_CASE(8)
 #undef B2S_T3_CASE
   return cudaErrorInvalidValue;

@@ -34,6 +34,12 @@
 // its threshold key is stored as key + d; the walk tests key(x) + d > key(t) + d, and INT_MAX + 1 wraps to INT_MIN exactly
 // when a missing value must go left.  `x < t` (xgboost) is `x <= prev(t)`: thresholds are converted when the model is
 // added, not in the kernel.
+//
+// Categorical splits (plans with one, CAT = true): bit 30 of a node's x offset marks it, and its threshold word holds
+// {bits 0-15: first word of its set in the part's set region at sm_cat, bits 16-30: words in the set, bit 31: the model's
+// code mode}.  The node goes right iff x is a valid code (x >= 0, or x > -1 under B2S_CAT_TRUNC) whose bit is set; under
+// MISS the value is recovered from its key (the key map is its own inverse) and NaN takes the default bit.  Each part
+// holds all the sets of its model, behind its node table in global memory (T3Part::n_cat_words).
 #pragma once
 #include "b2s_device.cuh"
 
@@ -55,6 +61,7 @@ struct T3Part {           // one per part, in global memory
   int32_t n_cols;         // columns of `partial` this part writes (trees: 1)
   int32_t col0;
   int32_t cta0, n_ctas;   // the CTAs [cta0, cta0 + n_ctas) of the grid work on this part
+  int32_t n_cat_words;    // CAT: words of the model's sets, stored right after `nodes` (n_trees << D entries)
 };
 
 struct T3Prep {           // t3_prep_kernel
@@ -74,7 +81,7 @@ struct T3Params {         // trees3_kernel
   double* partial;        // [n_cols_total][col_stride]
   int64_t col_stride;
   const T3Part* parts;
-  int32_t n_in, n_parts, warps, pad0;  // warps: walking warps (the CTA has kT3Service more)
+  int32_t n_in, n_parts, warps, sm_cat;  // warps: walking warps (the CTA has kT3Service more); sm_cat: CAT's set region
   int32_t xt_words;              // words of one tile (n_in rounded up to 4, times TR); two tiles are resident
   int32_t part_words;            // doubles of one partial-sum buffer; two are resident
   int32_t sm_leaf, sm_part, sm_xt, sm_bar;  // byte offsets into dynamic shared memory
@@ -85,7 +92,7 @@ struct T3Params {         // trees3_kernel
 
 // launchers (b2s_trees3.cu: the kernels are compiled in their own translation unit)
 cudaError_t t3_launch_prep(const T3Prep& pr, const CUtensorMap& tmap, bool miss, int grid, int smem, int smem_optin, cudaStream_t st);
-cudaError_t t3_launch_walk(const T3Params& t, int depth, bool miss, int grid, int block, int smem, int smem_optin, cudaStream_t st);
+cudaError_t t3_launch_walk(const T3Params& t, int depth, bool miss, bool cat, int grid, int block, int smem, int smem_optin, cudaStream_t st);
 cudaError_t t3_launch_vote(const KParams& k, const double* partial, int64_t col_stride, const int32_t* col_score,
                            const int32_t* col_order, const int32_t* model_cols, const int32_t* row_bad, int grid, cudaStream_t st);
 
@@ -122,10 +129,22 @@ __device__ __forceinline__ int32_t t3_key(float x) {
   return b ^ ((b >> 31) & 0x7fffffff);
 }
 
+template <bool MISS, bool CAT>
+__device__ __forceinline__ uint32_t t3_xoff(uint32_t foff) { return CAT ? (foff & 0x3fffffffu) : MISS ? (foff & 0x7fffffffu) : foff; }
+// a categorical node: right iff x is a valid code whose bit is set in the node's set (cbase: shared address of the sets)
 template <bool MISS>
-__device__ __forceinline__ uint32_t t3_xoff(uint32_t foff) { return MISS ? (foff & 0x7fffffffu) : foff; }
-template <bool MISS>
-__device__ __forceinline__ bool t3_right(uint32_t x, uint2 nd) {
+__device__ __forceinline__ bool t3_cat_right(uint32_t x, uint2 nd, uint32_t cbase) {
+  const int32_t k = (int32_t)x;
+  const float f = MISS ? __int_as_float(k ^ ((k >> 31) & 0x7fffffff)) : __uint_as_float(x);
+  if (MISS && f != f) return (nd.x >> 31) == 0u;  // NaN: the default child
+  const float lo = (nd.y >> 31) ? -0.99999994f : 0.0f;  // x > -1 (trunc(x) >= 0) or x >= 0
+  if (!(f >= lo && f < __uint2float_rz((nd.y >> 16) & 0x7fffu) * 32.0f)) return false;
+  const int c = __float2int_rz(f);
+  return (t3_lds32<0>(cbase + (((nd.y & 0xffffu) + (uint32_t)(c >> 5)) << 2)) >> (c & 31)) & 1u;
+}
+template <bool MISS, bool CAT>
+__device__ __forceinline__ bool t3_right(uint32_t x, uint2 nd, uint32_t cbase) {
+  if (CAT && (nd.x & 0x40000000u)) return t3_cat_right<MISS>(x, nd, cbase);
   // floats: sklearn's rule "left when x <= threshold"; keys: the same order on integers, shifted by the node's default bit
   return MISS ? ((int32_t)(x + (nd.x >> 31)) > (int32_t)nd.y) : !(__uint_as_float(x) <= __uint_as_float(nd.y));
 }
@@ -254,7 +273,7 @@ __global__ void __launch_bounds__(kT3PrepThreads) t3_prep_kernel(const __grid_co
 }
 
 // ------------------------------------------------------------------------------------------ walk
-template <int D, bool MISS, int U>
+template <int D, bool MISS, int U, bool CAT>
 __device__ __forceinline__ void t3_walk_body(const T3Params& p) {
   extern __shared__ __align__(1024) unsigned char smem3[];
   unsigned char* const smem = smem3;
@@ -291,6 +310,11 @@ __device__ __forceinline__ void t3_walk_body(const T3Params& p) {
     for (int i = tid; i < NT * NN; i += n_all) {
       sn[i] = part.nodes[i];
       s_leaf[i] = part.leaves[i];
+    }
+    if (CAT) {
+      const uint32_t* cw = reinterpret_cast<const uint32_t*>(part.nodes + NT * NN);
+      uint32_t* sc = reinterpret_cast<uint32_t*>(smem + p.sm_cat);
+      for (int i = tid; i < part.n_cat_words; i += n_all) sc[i] = cw[i];
     }
   } else {
     double* sw = reinterpret_cast<double*>(s_nodes);
@@ -348,6 +372,7 @@ __device__ __forceinline__ void t3_walk_body(const T3Params& p) {
 
   // ============================================================================================= walking warps
   const uint32_t sbase = (uint32_t)__cvta_generic_to_shared(smem);
+  const uint32_t cbase = CAT ? sbase + (uint32_t)p.sm_cat : 0u;
   const uint32_t leaf0 = (uint32_t)p.sm_leaf - (uint32_t)(NN * 8);  // leaf address = node address + leaf0
   const int TPW = (NT + W - 1) / W;                                 // trees per warp
   for (int k = 0; k < K; ++k) {
@@ -383,28 +408,28 @@ __device__ __forceinline__ void t3_walk_body(const T3Params& p) {
           }
 #pragma unroll
           for (int u = 0; u < U; ++u) {
-            x[u][0] = t3_lds32<0>(xls + t3_xoff<MISS>(n1[u].x));
-            if (RPT > 1) x[u][1] = t3_lds32<128>(xls + t3_xoff<MISS>(n1[u].x));
+            x[u][0] = t3_lds32<0>(xls + t3_xoff<MISS, CAT>(n1[u].x));
+            if (RPT > 1) x[u][1] = t3_lds32<128>(xls + t3_xoff<MISS, CAT>(n1[u].x));
           }
           bool r0[U][RPT];
 #pragma unroll
           for (int u = 0; u < U; ++u)
 #pragma unroll
             for (int j = 0; j < RPT; ++j) {
-              r0[u][j] = t3_right<MISS>(x[u][j], n1[u]);
+              r0[u][j] = t3_right<MISS, CAT>(x[u][j], n1[u], cbase);
               nd[u][j].x = r0[u][j] ? n3[u].x : n2[u].x;
               nd[u][j].y = r0[u][j] ? n3[u].y : n2[u].y;
             }
 #pragma unroll
           for (int u = 0; u < U; ++u) {
-            x[u][0] = t3_lds32<0>(xls + t3_xoff<MISS>(nd[u][0].x));
-            if (RPT > 1) x[u][1] = t3_lds32<128>(xls + t3_xoff<MISS>(nd[u][1].x));
+            x[u][0] = t3_lds32<0>(xls + t3_xoff<MISS, CAT>(nd[u][0].x));
+            if (RPT > 1) x[u][1] = t3_lds32<128>(xls + t3_xoff<MISS, CAT>(nd[u][1].x));
           }
 #pragma unroll
           for (int u = 0; u < U; ++u)
 #pragma unroll
             for (int j = 0; j < RPT; ++j) {
-              const bool r1 = t3_right<MISS>(x[u][j], nd[u][j]);
+              const bool r1 = t3_right<MISS, CAT>(x[u][j], nd[u][j], cbase);
               a[u][j] = tba[u] + 32u + (r0[u][j] ? 16u : 0u) + (r1 ? 8u : 0u);
             }
         }
@@ -416,13 +441,13 @@ __device__ __forceinline__ void t3_walk_body(const T3Params& p) {
             for (int j = 0; j < RPT; ++j) nd[u][j] = t3_lds64(a[u][j]);
 #pragma unroll
           for (int u = 0; u < U; ++u) {
-            x[u][0] = t3_lds32<0>(xls + t3_xoff<MISS>(nd[u][0].x));
-            if (RPT > 1) x[u][1] = t3_lds32<128>(xls + t3_xoff<MISS>(nd[u][1].x));
+            x[u][0] = t3_lds32<0>(xls + t3_xoff<MISS, CAT>(nd[u][0].x));
+            if (RPT > 1) x[u][1] = t3_lds32<128>(xls + t3_xoff<MISS, CAT>(nd[u][1].x));
           }
 #pragma unroll
           for (int u = 0; u < U; ++u)
 #pragma unroll
-            for (int j = 0; j < RPT; ++j) a[u][j] = a[u][j] + a[u][j] + (t3_right<MISS>(x[u][j], nd[u][j]) ? cr[u] : cl[u]);
+            for (int j = 0; j < RPT; ++j) a[u][j] = a[u][j] + a[u][j] + (t3_right<MISS, CAT>(x[u][j], nd[u][j], cbase) ? cr[u] : cl[u]);
         }
 #pragma unroll
         for (int u = 0; u < U; ++u)
@@ -476,9 +501,9 @@ __device__ __forceinline__ void t3_walk_body(const T3Params& p) {
   }
 }
 
-template <int D, bool MISS, int U>
+template <int D, bool MISS, int U, bool CAT>
 __global__ void __launch_bounds__(1024) trees3_kernel(const __grid_constant__ T3Params p) {
-  t3_walk_body<D, MISS, U>(p);
+  t3_walk_body<D, MISS, U, CAT>(p);
 }
 
 // Per row and model: scores = init + the model's columns of `partial`, link; then the VotingEnsemble reduce.

@@ -28,7 +28,8 @@ class PackedTrees:
     """SoA tree ensemble in the layout b2s_plan_add_tree_model takes (children are tree-relative)"""
 
     def __init__(self, tree_offset, feature, threshold, left, right, leaf_value, tree_slot, tree_scale, init,
-                 link=nat.LINK_IDENTITY, classes=None, cmp_mode=nat.CMP_LE, default_left=None, nan_ok=False):
+                 link=nat.LINK_IDENTITY, classes=None, cmp_mode=nat.CMP_LE, default_left=None, nan_ok=False,
+                 node_cat=None, cat_offsets=None, cat_words=None, cat_mode=nat.CAT_NONNEG):
         self.tree_offset = _i32(tree_offset)
         self.feature = _i32(feature)
         self.threshold = _f32(threshold)
@@ -44,6 +45,12 @@ class PackedTrees:
         self.cmp_mode = int(cmp_mode)  # nat.CMP_LE (scikit-learn, LightGBM) | nat.CMP_LT (xgboost)
         self.default_left = None if default_left is None else np.ascontiguousarray(default_left, dtype=np.uint8)
         self.nan_ok = bool(nan_ok)     # predict() routes NaN to the default child instead of refusing it
+        # categorical splits (b2s_plan_add_tree_model_cat): node i with node_cat[i] = s >= 0 goes right iff x is a valid
+        # code (cat_mode) whose bit is set in cat_words[cat_offsets[s]:cat_offsets[s + 1]]; None: every node is numeric
+        self.node_cat = None if node_cat is None else _i32(node_cat)
+        self.cat_offsets = None if cat_offsets is None else _i32(cat_offsets)
+        self.cat_words = None if cat_words is None else np.ascontiguousarray(cat_words, dtype=np.uint32)
+        self.cat_mode = int(cat_mode)  # nat.CAT_NONNEG (xgboost: x >= 0) | nat.CAT_TRUNC (LightGBM: x > -1)
 
     @property
     def n_trees(self):
@@ -118,13 +125,20 @@ class DevicePlan:
 
     def add_trees(self, t: PackedTrees):
         cls = t.classes
-        nat.check(self._lib.b2s_plan_add_tree_model_ex(
-            self._h, t.n_trees, nat._p(t.tree_offset, C.c_int32), nat._p(t.feature, C.c_int32),
-            nat._p(t.threshold, C.c_float), nat._p(t.left, C.c_int32), nat._p(t.right, C.c_int32),
-            nat._p(t.leaf_value, C.c_double), nat._p(t.tree_slot, C.c_int32), nat._p(t.tree_scale, C.c_double),
-            nat._p(t.init, C.c_double), t.n_scores, t.link, nat._p(cls, C.c_int32), 0 if cls is None else len(cls),
-            getattr(t, "cmp_mode", nat.CMP_LE), nat._p(getattr(t, "default_left", None), C.c_uint8),
-            nat.NAN_DEFAULT_CHILD if getattr(t, "nan_ok", False) else nat.NAN_ERROR))
+        args = (self._h, t.n_trees, nat._p(t.tree_offset, C.c_int32), nat._p(t.feature, C.c_int32),
+                nat._p(t.threshold, C.c_float), nat._p(t.left, C.c_int32), nat._p(t.right, C.c_int32),
+                nat._p(t.leaf_value, C.c_double), nat._p(t.tree_slot, C.c_int32), nat._p(t.tree_scale, C.c_double),
+                nat._p(t.init, C.c_double), t.n_scores, t.link, nat._p(cls, C.c_int32), 0 if cls is None else len(cls),
+                getattr(t, "cmp_mode", nat.CMP_LE), nat._p(getattr(t, "default_left", None), C.c_uint8),
+                nat.NAN_DEFAULT_CHILD if getattr(t, "nan_ok", False) else nat.NAN_ERROR)
+        node_cat = getattr(t, "node_cat", None)
+        if node_cat is None:
+            nat.check(self._lib.b2s_plan_add_tree_model_ex(*args))
+        else:
+            offs, words = getattr(t, "cat_offsets", None), getattr(t, "cat_words", None)
+            nat.check(self._lib.b2s_plan_add_tree_model_cat(
+                *args, nat._p(node_cat, C.c_int32), nat._p(offs, C.c_int32), 0 if offs is None else len(offs) - 1,
+                nat._p(words, C.c_uint32), 0 if words is None else len(words), getattr(t, "cat_mode", nat.CAT_NONNEG)))
         self.n_models += 1
         return self
 
