@@ -187,7 +187,7 @@ const char* b2s_plan_kernel(b2s_plan_t plan);
 #define B2S_KERNEL_TREES3 3            /* the same with plain loads                                       */
 #define B2S_KERNEL_TREES2_TMAP 4       /* trees_model_kernel with TMA tensor-map loads + vote_kernel      */
 #define B2S_KERNEL_TREES2 5            /* the same with plain loads                                       */
-#define B2S_KERNEL_ROWTHREAD_TMA 6     /* rowthread kernel, TMA tensor-map or bulk-copy loads             */
+#define B2S_KERNEL_ROWTHREAD_TMA 6     /* rowthread kernel, TMA tensor-map loads (swizzled 2-D boxes)     */
 #define B2S_KERNEL_ROWTHREAD_LDGSTS 7  /* rowthread kernel, cp.async loads from device memory             */
 #define B2S_KERNEL_ROWTHREAD_HOST 8    /* rowthread kernel, cp.async loads from mapped host memory        */
 #define B2S_KERNEL_ROWWARP 9           /* retired (rowwarp_kernel): no longer returned                    */
@@ -196,6 +196,7 @@ const char* b2s_plan_kernel(b2s_plan_t plan);
 #define B2S_KERNEL_TREES3_CAT_TMAP 12  /* B2S_KERNEL_TREES3_TMAP, walk with categorical splits             */
 #define B2S_KERNEL_TREES3_CAT 13       /* B2S_KERNEL_TREES3, walk with categorical splits                  */
 #define B2S_KERNEL_ROWS_CAT 14         /* rows_kernel of a tree plan with categorical splits              */
+#define B2S_KERNEL_ROWTHREAD_BULK 15   /* rowthread kernel, one TMA bulk copy per row (also the gather)   */
 int32_t b2s_plan_last_kernel(b2s_plan_t plan);
 /* out_cols 4-byte words per output row; out_is_int != 0 when they are int32 labels */
 int b2s_plan_out_info(b2s_plan_t plan, int32_t* out_cols, int32_t* out_is_int);

@@ -474,7 +474,9 @@ static cudaError_t rt_launch_t(b2s_plan_s* p, const void* rows, int64_t stride, 
   alignas(64) CUtensorMap tmap;
   memset(&tmap, 0, sizeof(tmap));
   if (mode == 2 && !encode_rows_map(&tmap, rows, n_rows, stride, p->n_in, tr)) mode = 1;
-  p->last_kernel.store(mode != 0 ? B2S_KERNEL_ROWTHREAD_TMA : (lc && lc->host_rows) ? B2S_KERNEL_ROWTHREAD_HOST : B2S_KERNEL_ROWTHREAD_LDGSTS,
+  p->last_kernel.store(mode == 2 ? B2S_KERNEL_ROWTHREAD_TMA
+                       : mode == 1 ? B2S_KERNEL_ROWTHREAD_BULK
+                       : (lc && lc->host_rows) ? B2S_KERNEL_ROWTHREAD_HOST : B2S_KERNEL_ROWTHREAD_LDGSTS,
                        std::memory_order_relaxed);
   r.tile_rows = tr;
   const int64_t tiles = (n_rows + tr - 1) / tr;

@@ -21,7 +21,7 @@ from mlrun_b200.lowering import ColumnProgram  # noqa: E402
 from mlrun_b200.plan import DevicePlan  # noqa: E402
 from tests import device_emulator as emu  # noqa: E402
 from tests import tree_cat_fixtures as fx  # noqa: E402
-from tests.test_gpu_tree_paths import U32, U64, Rows, assert_kernel, check_close, names, run_device  # noqa: E402
+from tests.device_check import U32, U64, Rows, assert_kernel, check_close, names, run_device  # noqa: E402
 
 CARDS = {0: 40, 3: 8, 5: 1001, 6: 33}
 
