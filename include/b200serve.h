@@ -390,6 +390,9 @@ int b2s_table_create(const int64_t* keys, int64_t n_keys, const float* values, i
                      b2s_table_t* out);
 int b2s_table_destroy(b2s_table_t table);
 int b2s_table_info(b2s_table_t table, int64_t* n_keys, int32_t* n_features, int64_t* capacity);
+/* Device keys -> device rows.  row_stride_bytes >= 4 * n_features and a multiple of 4.  B2S_ERR_INVALID, before any
+ * launch, when d_keys is NULL (n > 0) or not 8-byte aligned, or d_rows / d_found is not 4-byte aligned.  Rows are
+ * stored 16 bytes at a time only when n_features, row_stride_bytes and d_rows all allow it (4-byte words otherwise). */
 int b2s_table_lookup_device(b2s_table_t table, const int64_t* d_keys, int64_t n, float* d_rows, int64_t row_stride_bytes,
                             int32_t* d_found, void* stream);
 int b2s_table_lookup_host(b2s_table_t table, const int64_t* keys, int64_t n, float* rows, int32_t* found, b2s_stats* stats);
@@ -400,7 +403,8 @@ int b2s_table_lookup_host(b2s_table_t table, const int64_t* keys, int64_t n, flo
 /* The same for device-resident keys, as ONE launch: the scoring kernel's tile loader finds each key in the table and
  * fetches the row from there (one TMA bulk copy per row), so the gathered rows never travel to HBM and back; the table's
  * impute policy folds into the kernel's Imputer operands.  B2S_ERR_UNSUPPORTED for plans the loader does not cover (tree
- * ensembles, MapValues, one-hot sources under an impute policy): use b2s_table_lookup_device + b2s_run_device then. */
+ * ensembles, MapValues, one-hot sources under an impute policy): use b2s_table_lookup_device + b2s_run_device then.
+ * B2S_ERR_INVALID, before any launch, when d_keys is not 8-byte aligned or d_out / d_status is not 4-byte aligned. */
 int b2s_table_enrich_device(b2s_table_t table, b2s_plan_t plan, const int64_t* d_keys, int64_t n, void* d_out,
                             int32_t* d_status, void* stream);
 int b2s_table_enrich_host(b2s_table_t table, b2s_plan_t plan, const int64_t* keys, int64_t n, void* out, int64_t out_bytes,

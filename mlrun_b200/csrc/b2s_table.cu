@@ -45,6 +45,7 @@ struct LookupParams {
   int32_t n_feat;
   int32_t any_impute;
   int32_t lanes_per_row;    // n_feat / 4 when that is a power of two <= 32 (rows are copied by sub-warps), else 0
+  int32_t vec;              // 1: every output row is 16-byte aligned (n_feat % 4 == 0, out and out_stride 16-byte multiples)
   const int64_t* keys;      // [n]
   int64_t n;
   float* out;               // row i at out + i * out_stride (bytes)
@@ -56,7 +57,7 @@ __global__ void __launch_bounds__(256) table_lookup_kernel(const __grid_constant
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  const bool vec = (p.n_feat & 3) == 0 && (p.out_stride & 15) == 0;
+  const bool vec = p.vec != 0;
   for (int64_t base = warp * 32; base < p.n; base += n_warps * 32) {
     const int64_t q = base + lane;
     int64_t row = -1;
@@ -226,6 +227,9 @@ static int launch_lookup(b2s_table_t t, const int64_t* d_keys, int64_t n, float*
   p.n = n;
   p.out = d_rows;
   p.out_stride = row_stride;
+  // 16-byte stores only where every row starts on a 16-byte boundary: a caller may gather into a column offset of a
+  // wider row matrix (stride a multiple of 16, base 4 bytes off), which takes the scalar path
+  p.vec = (t->n_feat % 4) == 0 && (row_stride % 16) == 0 && ((uintptr_t)d_rows % 16) == 0;
   p.found = d_found;
   const int64_t warps = (n + 31) / 32;
   const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(t->grid, (warps + 7) / 8));
@@ -236,11 +240,18 @@ static int launch_lookup(b2s_table_t t, const int64_t* d_keys, int64_t n, float*
   return B2S_OK;
 }
 
+// the kernels load keys as 8-byte words and store rows, flags and status words as 4-byte words (rows also as 16-byte
+// words where the base allows): a pointer off those boundaries is refused before anything is launched
+static bool misaligned(const void* ptr, uintptr_t bytes) { return ((uintptr_t)ptr & (bytes - 1)) != 0; }
+
 extern "C" int b2s_table_lookup_device(b2s_table_t t, const int64_t* d_keys, int64_t n, float* d_rows, int64_t row_stride_bytes,
                                        int32_t* d_found, void* stream) {
   try {  // no C++ exception crosses the C boundary
     if (!t) return b2s_int_fail(B2S_ERR_INVALID, "null table");
     if (n < 0 || row_stride_bytes < (int64_t)t->n_feat * 4 || (row_stride_bytes & 3)) return b2s_int_fail(B2S_ERR_INVALID, "bad n / row stride");
+    if (n > 0 && (!d_keys || !d_rows)) return b2s_int_fail(B2S_ERR_INVALID, "null keys / rows");
+    if (misaligned(d_keys, 8) || misaligned(d_rows, 4) || misaligned(d_found, 4))
+      return b2s_int_fail(B2S_ERR_INVALID, "keys must be 8-byte aligned, rows and found 4-byte aligned");
     if (n == 0) return B2S_OK;
     TAB_TRY(cudaSetDevice(b2s_int_device()));
     return launch_lookup(t, d_keys, n, d_rows, row_stride_bytes, d_found, stream ? (cudaStream_t)stream : b2s_int_stream());
@@ -306,6 +317,8 @@ extern "C" int b2s_table_enrich_device(b2s_table_t t, b2s_plan_t plan, const int
                                        int32_t* d_status, void* stream) {
   try {  // no C++ exception crosses the C boundary
     if (!t || !plan || !d_keys || !d_out || n < 0) return b2s_int_fail(B2S_ERR_INVALID, "bad arguments");
+    if (misaligned(d_keys, 8) || misaligned(d_out, 4) || misaligned(d_status, 4))
+      return b2s_int_fail(B2S_ERR_INVALID, "keys must be 8-byte aligned, out and status 4-byte aligned");
     if (n == 0) return B2S_OK;
     TAB_TRY(cudaSetDevice(b2s_int_device()));
     return launch_fused(t, plan, d_keys, n, d_out, d_status, stream ? (cudaStream_t)stream : b2s_int_stream());
