@@ -415,6 +415,52 @@ int b2s_table_time_device(b2s_table_t table, const int64_t* const* d_keys, int32
  * string-valued entity.  Host code. */
 int b2s_hash_strings(const char* bytes, const int64_t* offsets, int64_t n, int64_t* keys_out);
 
+/* ---- point-in-time training sets: as-of joins of entity rows onto feature-set indexes ---------------------------
+ * get_offline_features on the local engine (feature_store/retrieval/base.py:412-468, local_merger.py:29-81) merges
+ * each feature set of a vector onto the entity frame with pandas.merge_asof: equal keys, the set's last row whose
+ * timestamp is <= the entity row's (backward, exact matches allowed, no tolerance), NaN / NaT where there is none.
+ * A b2s_pit index holds one feature set in HBM: its rows sorted by (64-bit key, int64 nanosecond timestamp), equal
+ * pairs in input order, the feature columns as rows of 4-byte words, and each key's run in an open-addressing slot
+ * array.  Built once from host columns (each 4 or 8 bytes wide; column c takes words [sum of earlier widths / 4, ...)). */
+typedef struct b2s_pit_s* b2s_pit_t;
+int b2s_pit_index_create(const int64_t* keys, const int64_t* ts_ns, int64_t n_rows, const void* const* cols,
+                         const int32_t* col_bytes, int32_t n_cols, b2s_pit_t* out);
+int b2s_pit_index_destroy(b2s_pit_t index);
+/* longest_run 1: every key has one row, so the index can also serve exact-key joins */
+int b2s_pit_index_info(b2s_pit_t index, int64_t* n_rows, int64_t* n_keys, int64_t* longest_run, int32_t* row_words,
+                       int64_t* capacity);
+typedef struct b2s_pit_out {
+  int32_t src_word;   /* first word of the column in the index's rows */
+  int32_t bytes;      /* 4 or 8 */
+  uint64_t miss;      /* bits stored for an entity row without a match (a NaN, NaT or 0) */
+  void* out;          /* [n] elements of `bytes` bytes, in sorted order */
+} b2s_pit_out;
+typedef struct b2s_pit_set {
+  b2s_pit_t index;
+  const int64_t* keys;   /* [n] the entity rows' keys, input order */
+  int32_t asof;          /* 1: as-of join on the entity timestamps; 0: exact key (the index must have one row per key) */
+  int32_t n_out;
+  const b2s_pit_out* outs;  /* host array of n_out descriptors */
+  int64_t* ts_out;       /* [n] the matched row's timestamp, INT64_MIN (NaT) on a miss; may be NULL */
+  uint8_t* found;        /* [n] 1 / 0; may be NULL */
+} b2s_pit_set;
+typedef struct b2s_pit_col {
+  const void* src;       /* [n] entity column, input order */
+  void* dst;             /* [n] the same column in sorted order */
+  int32_t bytes;         /* 1, 2, 4 or 8 */
+} b2s_pit_col;
+/* Join n entity rows onto n_sets indexes.  With ts (int64 nanoseconds) the rows are ordered by timestamp, ties in input
+ * order (a stable radix sort); without it they keep input order (then no set may be as-of).  Every output, the entity
+ * columns in `cols` and order[q] (the input row at sorted position q; may be NULL) are written in that order; miss[s]
+ * counts the rows without a match in set s.  _device: every array is device memory, miss accumulates (zero it first),
+ * asynchronous on `stream`.  _host: host arrays; the join runs in row ranges whose results are copied back while the next
+ * range is joined; miss is written.  B2S_ERR_INVALID before any launch for a misaligned or null array, an output word
+ * outside the index's rows, or an exact-key join on an index with more than one row per key. */
+int b2s_pit_join_device(const int64_t* d_ts, int64_t n, const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols,
+                        int32_t n_cols, int64_t* d_order, uint64_t* d_miss, void* stream);
+int b2s_pit_join_host(const int64_t* ts, int64_t n, const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols,
+                      int32_t n_cols, int64_t* order, uint64_t* miss, b2s_stats* stats);
+
 #ifdef __cplusplus
 }
 #endif

@@ -57,6 +57,19 @@ class DevInfo(C.Structure):
 _vp, _i32, _i64, _u64 = C.c_void_p, C.c_int32, C.c_int64, C.c_uint64
 _pi32, _pf32, _pf64 = C.POINTER(C.c_int32), C.POINTER(C.c_float), C.POINTER(C.c_double)
 
+
+class PitOut(C.Structure):
+    _fields_ = [("src_word", _i32), ("bytes", _i32), ("miss", _u64), ("out", _vp)]
+
+
+class PitSet(C.Structure):
+    _fields_ = [("index", _vp), ("keys", _vp), ("asof", _i32), ("n_out", _i32), ("outs", C.POINTER(PitOut)),
+                ("ts_out", _vp), ("found", _vp)]
+
+
+class PitCol(C.Structure):
+    _fields_ = [("src", _vp), ("dst", _vp), ("bytes", _i32)]
+
 # name -> (restype, argtypes); the single source of truth for the exported surface
 SIGNATURES = {
     "b2s_version": (C.c_int, []),
@@ -137,6 +150,12 @@ SIGNATURES = {
     "b2s_table_enrich_host": (C.c_int, [_vp, _vp, C.POINTER(_i64), _i64, _vp, _i64, _pi32, C.POINTER(Stats)]),
     "b2s_table_time_device": (C.c_int, [_vp, C.POINTER(_vp), _i32, _i64, _vp, _i64, _vp, _i32, _pf32]),
     "b2s_hash_strings": (C.c_int, [C.c_char_p, C.POINTER(_i64), _i64, C.POINTER(_i64)]),
+    # point-in-time (as-of) joins
+    "b2s_pit_index_create": (C.c_int, [_vp, _vp, _i64, C.POINTER(_vp), _pi32, _i32, C.POINTER(_vp)]),
+    "b2s_pit_index_destroy": (C.c_int, [_vp]),
+    "b2s_pit_index_info": (C.c_int, [_vp, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_i64), _pi32, C.POINTER(_i64)]),
+    "b2s_pit_join_device": (C.c_int, [_vp, _i64, C.POINTER(PitSet), _i32, C.POINTER(PitCol), _i32, _vp, _vp, _vp]),
+    "b2s_pit_join_host": (C.c_int, [_vp, _i64, C.POINTER(PitSet), _i32, C.POINTER(PitCol), _i32, _vp, _vp, C.POINTER(Stats)]),
     # body codec
     "b2s_json_parse_inputs": (C.c_int, [C.c_char_p, _i64, _pf32, _i64, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_i64),
                                         C.POINTER(_i64)]),

@@ -1,0 +1,632 @@
+// b2s_pit.cu -- point-in-time correct training sets on the device, sm_90a.
+//
+// Replaces the local engine's get_offline_features (mlrun/feature_store/retrieval/base.py:412-468 BaseMerger.merge,
+// local_merger.py:29-81 _asof_join): for each feature set, pandas.merge_asof of the entity frame onto the set's rows by
+// key, taking the set's last row whose timestamp is <= the entity row's.  Here a feature set is indexed once: its rows are
+// radix-sorted by (key, timestamp) on the device, their timestamps and feature words laid out in that order, and each key's
+// run (start, length) recorded in an open-addressing slot array (b2s_hash.cuh).  A query sorts the entity rows by timestamp
+// (stable: ties keep input order), then one launch per feature set resolves every entity row -- probe the key's run,
+// binary-search it for the last timestamp <= t, gather the selected feature words into columnar outputs at the row's sorted
+// position -- and permutes the entity frame's own columns into the same order.
+// Bound: HBM, random row reads (one 4 * row_words-byte row per hit) plus sequential column writes.
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <cstdint>
+#include <cstring>
+#include <exception>
+#include <vector>
+
+#include "../../include/b200serve.h"
+#include "b2s_internal.h"
+#include "b2s_pit.cuh"
+
+#define PIT_TRY(expr)                                                                                                  \
+  do {                                                                                                                 \
+    cudaError_t _e = (expr);                                                                                           \
+    if (_e != cudaSuccess)                                                                                             \
+      return b2s_int_fail(B2S_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
+  } while (0)
+
+using namespace b2s_pit;
+using b2s::TableSlot;
+
+namespace {
+
+// ---- radix sort ---------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kSortThreads) radix_hist_kernel(const uint64_t* __restrict__ keys, int64_t n, int shift,
+                                                                  uint32_t* __restrict__ hist, int n_blocks) {
+  __shared__ uint32_t s_hist[256];
+  s_hist[threadIdx.x] = 0;
+  __syncthreads();
+  const int64_t base = (int64_t)blockIdx.x * kSortTile;
+#pragma unroll 4
+  for (int j = 0; j < kSortItems; ++j) {
+    const int64_t e = base + (int64_t)j * kSortThreads + threadIdx.x;
+    if (e < n) atomicAdd(&s_hist[radix_digit(keys[e], shift)], 1u);
+  }
+  __syncthreads();
+  hist[(int64_t)threadIdx.x * n_blocks + blockIdx.x] = s_hist[threadIdx.x];  // digit-major: the scan yields global offsets
+}
+
+// exclusive scan of m counters in place, one block (m = 256 * n_blocks is a few hundred thousand at most)
+__global__ void __launch_bounds__(kScanThreads) radix_scan_kernel(uint32_t* __restrict__ v, int64_t m) {
+  __shared__ uint32_t s_sum[kScanThreads];
+  const int64_t chunk = (m + kScanThreads - 1) / kScanThreads;
+  const int64_t b = threadIdx.x * chunk, e = (b + chunk < m) ? b + chunk : m;
+  uint32_t sum = 0;
+  for (int64_t i = b; i < e; ++i) sum += v[i];
+  s_sum[threadIdx.x] = sum;
+  __syncthreads();
+  for (int off = 1; off < kScanThreads; off <<= 1) {  // Hillis-Steele over the per-thread sums
+    const uint32_t add = threadIdx.x >= off ? s_sum[threadIdx.x - off] : 0u;
+    __syncthreads();
+    s_sum[threadIdx.x] += add;
+    __syncthreads();
+  }
+  uint32_t run = s_sum[threadIdx.x] - sum;
+  for (int64_t i = b; i < e; ++i) {
+    const uint32_t c = v[i];
+    v[i] = run;
+    run += c;
+  }
+}
+
+__global__ void __launch_bounds__(kSortThreads) radix_scatter_kernel(const uint64_t* __restrict__ kin, const uint32_t* __restrict__ vin,
+                                                                     uint64_t* __restrict__ kout, uint32_t* __restrict__ vout,
+                                                                     int64_t n, int shift, const uint32_t* __restrict__ hist, int n_blocks) {
+  __shared__ uint32_t s_base[256];              // next free output position of each digit for this block
+  __shared__ uint32_t s_warp[kSortWarps][256];  // per item: count, then first position, of each digit per warp
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  s_base[tid] = hist[(int64_t)tid * n_blocks + blockIdx.x];
+  const unsigned lt_mask = (1u << lane) - 1u;
+  const int64_t base = (int64_t)blockIdx.x * kSortTile;
+  for (int j = 0; j < kSortItems; ++j) {
+#pragma unroll
+    for (int w = 0; w < kSortWarps; ++w) s_warp[w][tid] = 0;
+    __syncthreads();
+    const int64_t e = base + (int64_t)j * kSortThreads + tid;
+    const bool valid = e < n;
+    uint64_t k = 0;
+    uint32_t d = 256;  // out-of-range items form their own group and are never stored
+    if (valid) {
+      k = kin[e];
+      d = radix_digit(k, shift);
+    }
+    const unsigned peers = __match_any_sync(0xffffffffu, d);
+    const unsigned rank = __popc(peers & lt_mask);
+    if (valid && rank == 0) s_warp[warp][d] = __popc(peers);
+    __syncthreads();
+    {  // thread tid owns digit tid: warp counts -> positions, in warp order
+      uint32_t run = s_base[tid];
+#pragma unroll
+      for (int w = 0; w < kSortWarps; ++w) {
+        const uint32_t c = s_warp[w][tid];
+        s_warp[w][tid] = run;
+        run += c;
+      }
+      s_base[tid] = run;
+    }
+    __syncthreads();
+    if (valid) {
+      const uint32_t pos = s_warp[warp][d] + rank;
+      kout[pos] = k;
+      vout[pos] = vin ? vin[e] : (uint32_t)e;  // no payload: the input position
+    }
+    __syncthreads();
+  }
+}
+
+struct SortBufs {
+  uint64_t* k[2];
+  uint32_t* v[2];
+  uint32_t* hist;
+};
+
+// stable sort of k[0] (signed 64-bit keys) carrying v[0] (null: the payload is the input position); the result ends in
+// k[0] / v[0] (an even number of passes)
+int radix_sort(SortBufs& b, bool payload, int64_t n, cudaStream_t st) {
+  const int n_blocks = (int)((n + kSortTile - 1) / kSortTile);
+  for (int pass = 0; pass < 8; ++pass) {
+    const int src = pass & 1, shift = pass * 8;
+    radix_hist_kernel<<<n_blocks, kSortThreads, 0, st>>>(b.k[src], n, shift, b.hist, n_blocks);
+    radix_scan_kernel<<<1, kScanThreads, 0, st>>>(b.hist, (int64_t)n_blocks * 256);
+    radix_scatter_kernel<<<n_blocks, kSortThreads, 0, st>>>(b.k[src], (pass == 0 && !payload) ? nullptr : b.v[src], b.k[src ^ 1],
+                                                            b.v[src ^ 1], n, shift, b.hist, n_blocks);
+  }
+  b2s_int_count_launches(24);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return b2s_int_fail(B2S_ERR_CUDA, "radix sort launch failed: %s", cudaGetErrorString(e));
+  return B2S_OK;
+}
+
+int alloc_sort(SortBufs& b, int64_t n, cudaStream_t st) {
+  const int64_t n_blocks = (n + kSortTile - 1) / kSortTile;
+  b = SortBufs{};
+  for (int i = 0; i < 2; ++i) {
+    PIT_TRY(cudaMallocAsync(&b.k[i], n * 8, st));
+    PIT_TRY(cudaMallocAsync(&b.v[i], n * 4, st));
+  }
+  PIT_TRY(cudaMallocAsync(&b.hist, n_blocks * 256 * 4, st));
+  return B2S_OK;
+}
+
+void free_sort(SortBufs& b, cudaStream_t st) {
+  for (int i = 0; i < 2; ++i) {
+    if (b.k[i]) cudaFreeAsync(b.k[i], st);
+    if (b.v[i]) cudaFreeAsync(b.v[i], st);
+  }
+  if (b.hist) cudaFreeAsync(b.hist, st);
+  b = SortBufs{};
+}
+
+// ---- index build ----------------------------------------------------------------------------------------------------------
+__global__ void gather_keys_kernel(const int64_t* __restrict__ src, const uint32_t* __restrict__ perm, uint64_t* __restrict__ dst, int64_t n) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    dst[i] = (uint64_t)src[perm[i]];
+}
+
+// rows[i] = the words of input row perm[i]: column c is (bytes[c] / 4) words from word woff[c]
+struct LayoutParams {
+  const void* cols[kMaxOuts];
+  int32_t words[kMaxOuts];
+  int32_t n_cols, row_words;
+};
+
+__global__ void layout_rows_kernel(const __grid_constant__ LayoutParams p, const uint32_t* __restrict__ perm, uint32_t* __restrict__ rows,
+                                   int64_t n) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = perm[i];
+    uint32_t* dst = rows + i * p.row_words;
+    int w = 0;
+    for (int c = 0; c < p.n_cols; ++c) {
+      const uint32_t* src = static_cast<const uint32_t*>(p.cols[c]) + r * p.words[c];
+      for (int k = 0; k < p.words[c]; ++k) dst[w++] = src[k];
+    }
+  }
+}
+
+__global__ void count_runs_kernel(const uint64_t* __restrict__ keys, int64_t n, unsigned long long* __restrict__ n_runs) {
+  unsigned long long c = 0;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    c += (i == 0 || keys[i] != keys[i - 1]) ? 1 : 0;
+  for (int off = 16; off; off >>= 1) c += __shfl_down_sync(0xffffffffu, c, off);
+  if ((threadIdx.x & 31) == 0 && c) atomicAdd(n_runs, c);
+}
+
+// every run head finds its run's end by binary search and claims a slot (keys are distinct: only the row word is contended)
+__global__ void insert_runs_kernel(const uint64_t* __restrict__ keys, int64_t n, TableSlot* slots, uint64_t mask,
+                                   unsigned long long* __restrict__ longest) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const uint64_t k = keys[i];
+    if (i > 0 && keys[i - 1] == k) continue;
+    int64_t lo = i + 1, hi = n;  // first position past the run
+    while (lo < hi) {
+      const int64_t mid = (lo + hi) >> 1;
+      if (keys[mid] == k) lo = mid + 1; else hi = mid;
+    }
+    const unsigned long long len = (unsigned long long)(lo - i);
+    const unsigned long long row = ((unsigned long long)i << 32) | len;
+    uint64_t h = b2s::mix64(k) & mask;
+    for (;;) {
+      unsigned long long* rw = reinterpret_cast<unsigned long long*>(&slots[h].row);
+      if (atomicCAS(rw, ~0ull, row) == ~0ull) {
+        slots[h].key = (long long)k;
+        break;
+      }
+      h = (h + 1) & mask;
+    }
+    atomicMax(longest, len);
+  }
+}
+
+// ---- join ---------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void copy_elem(const EntCol& c, int64_t dst, int64_t src) {
+  switch (c.bytes) {
+    case 1: static_cast<uint8_t*>(c.dst)[dst] = static_cast<const uint8_t*>(c.src)[src]; break;
+    case 2: static_cast<uint16_t*>(c.dst)[dst] = static_cast<const uint16_t*>(c.src)[src]; break;
+    case 4: static_cast<uint32_t*>(c.dst)[dst] = static_cast<const uint32_t*>(c.src)[src]; break;
+    default: static_cast<uint64_t*>(c.dst)[dst] = static_cast<const uint64_t*>(c.src)[src]; break;
+  }
+}
+
+__global__ void __launch_bounds__(256) pit_join_kernel(const __grid_constant__ JoinParams p) {
+  __shared__ unsigned long long s_miss[kMaxSets];
+  if (threadIdx.x < kMaxSets) s_miss[threadIdx.x] = 0;
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t q = p.q0 + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < p.q1; q += stride) {
+    const int64_t r = p.order ? (int64_t)p.order[q] : q;
+    if (p.order_out) p.order_out[q] = r;
+    const int64_t t = p.sorted_ts ? p.sorted_ts[q] : 0;
+    for (int c = 0; c < p.n_cols; ++c) copy_elem(p.cols[c], q, r);
+    const unsigned active = __activemask();
+    for (int s = 0; s < p.n_sets; ++s) {
+      const SetDesc& d = p.sets[s];
+      const long long slot = b2s::table_find(d.slots, d.mask, d.keys[r]);
+      int64_t pos = -1;
+      if (slot >= 0) {
+        const int64_t start = slot >> 32, len = slot & 0xffffffffll;
+        if (d.asof) {  // merge_asof(direction="backward", allow_exact_matches=True): last ts <= t
+          int64_t lo = start, hi = start + len;
+          while (lo < hi) {
+            const int64_t mid = (lo + hi) >> 1;
+            if (__ldg(d.ts + mid) <= t) lo = mid + 1; else hi = mid;
+          }
+          pos = lo > start ? lo - 1 : -1;
+        } else {
+          pos = start;  // exact-key join: the index has one row per key
+        }
+      }
+      if (d.found) d.found[q] = pos >= 0 ? 1 : 0;
+      if (d.ts_out) d.ts_out[q] = pos >= 0 ? __ldg(d.ts + pos) : INT64_MIN;
+      const uint32_t* row = d.rows + (pos >= 0 ? pos : 0) * d.row_words;
+      for (int j = d.out0; j < d.out0 + d.n_out; ++j) {
+        const OutCol& o = p.outs[j];
+        if (o.bytes == 4) {
+          static_cast<uint32_t*>(o.out)[q] = pos >= 0 ? row[o.src_word] : (uint32_t)o.miss;
+        } else {
+          const uint64_t v = pos >= 0 ? ((uint64_t)row[o.src_word] | ((uint64_t)row[o.src_word + 1] << 32)) : o.miss;
+          static_cast<uint64_t*>(o.out)[q] = v;
+        }
+      }
+      const unsigned missed = __ballot_sync(active, pos < 0);
+      if (missed && lane == __ffs(active) - 1) atomicAdd(&s_miss[s], (unsigned long long)__popc(missed));
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x < p.n_sets && s_miss[threadIdx.x]) atomicAdd(&p.miss[threadIdx.x], s_miss[threadIdx.x]);
+}
+
+int grid_for(int64_t n, int threads) {
+  return (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)b2s_int_sm_count() * 8, (n + threads - 1) / threads));
+}
+
+bool misaligned(const void* ptr, uintptr_t bytes) { return ((uintptr_t)ptr & (bytes - 1)) != 0; }
+
+}  // namespace
+
+struct b2s_pit_s {
+  int64_t n_rows = 0;
+  int64_t n_keys = 0;
+  int64_t longest_run = 0;
+  int32_t row_words = 0;
+  uint64_t cap = 0;
+  TableSlot* d_slots = nullptr;
+  int64_t* d_ts = nullptr;
+  uint32_t* d_rows = nullptr;
+};
+
+extern "C" int b2s_pit_index_destroy(b2s_pit_t ix) {
+  try {  // no C++ exception crosses the C boundary
+    if (!ix) return B2S_OK;
+    if (ix->d_slots) cudaFree(ix->d_slots);
+    if (ix->d_ts) cudaFree(ix->d_ts);
+    if (ix->d_rows) cudaFree(ix->d_rows);
+    delete ix;
+    return B2S_OK;
+  } catch (const std::exception& e) {
+    return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
+  }
+}
+
+static int index_build(b2s_pit_s* ix, const int64_t* keys, const int64_t* ts, int64_t n, const void* const* cols,
+                       const int32_t* col_bytes, int32_t n_cols, cudaStream_t st) {
+  LayoutParams lp{};
+  lp.n_cols = n_cols;
+  for (int c = 0; c < n_cols; ++c) {
+    lp.words[c] = col_bytes[c] / 4;
+    lp.row_words += lp.words[c];
+  }
+  ix->row_words = lp.row_words;
+  SortBufs sb{};
+  int64_t* d_keys = nullptr;
+  int64_t* d_ts_in = nullptr;
+  std::vector<void*> d_cols(n_cols, nullptr);
+  unsigned long long* d_stat = nullptr;  // [0] runs, [1] longest run
+  int rc = B2S_OK;
+  do {
+    if ((rc = alloc_sort(sb, n, st))) break;
+    PIT_TRY(cudaMallocAsync(&d_keys, n * 8, st));
+    PIT_TRY(cudaMallocAsync(&d_ts_in, n * 8, st));
+    PIT_TRY(cudaMallocAsync(&d_stat, 16, st));
+    PIT_TRY(cudaMemsetAsync(d_stat, 0, 16, st));
+    PIT_TRY(cudaMemcpyAsync(d_keys, keys, n * 8, cudaMemcpyHostToDevice, st));
+    PIT_TRY(cudaMemcpyAsync(d_ts_in, ts, n * 8, cudaMemcpyHostToDevice, st));
+    PIT_TRY(cudaMemcpyAsync(sb.k[0], ts, n * 8, cudaMemcpyHostToDevice, st));
+    for (int c = 0; c < n_cols; ++c) {
+      PIT_TRY(cudaMallocAsync(&d_cols[c], (size_t)n * col_bytes[c], st));
+      PIT_TRY(cudaMemcpyAsync(d_cols[c], cols[c], (size_t)n * col_bytes[c], cudaMemcpyHostToDevice, st));
+      lp.cols[c] = d_cols[c];
+    }
+    // by timestamp, then (stably) by key: rows ordered by (key, timestamp), equal pairs in input order
+    if ((rc = radix_sort(sb, false, n, st))) break;
+    const int g = grid_for(n, 256);
+    gather_keys_kernel<<<g, 256, 0, st>>>(d_keys, sb.v[0], sb.k[0], n);
+    if ((rc = radix_sort(sb, true, n, st))) break;
+    PIT_TRY(cudaMalloc(&ix->d_ts, n * 8));
+    PIT_TRY(cudaMalloc(&ix->d_rows, (size_t)n * std::max(lp.row_words, 1) * 4));
+    gather_keys_kernel<<<g, 256, 0, st>>>(d_ts_in, sb.v[0], reinterpret_cast<uint64_t*>(ix->d_ts), n);
+    layout_rows_kernel<<<g, 256, 0, st>>>(lp, sb.v[0], ix->d_rows, n);
+    count_runs_kernel<<<g, 256, 0, st>>>(sb.k[0], n, d_stat);
+    b2s_int_count_launches(4);
+    unsigned long long runs = 0;
+    PIT_TRY(cudaMemcpyAsync(&runs, d_stat, 8, cudaMemcpyDeviceToHost, st));
+    PIT_TRY(cudaStreamSynchronize(st));
+    uint64_t cap = 16;
+    while (cap < runs * 2) cap <<= 1;  // load factor <= 0.5: table_find's walk always meets an empty slot
+    ix->cap = cap;
+    ix->n_keys = (int64_t)runs;
+    PIT_TRY(cudaMalloc(&ix->d_slots, cap * sizeof(TableSlot)));
+    PIT_TRY(cudaMemsetAsync(ix->d_slots, 0xff, cap * sizeof(TableSlot), st));  // row -1: empty
+    insert_runs_kernel<<<g, 256, 0, st>>>(sb.k[0], n, ix->d_slots, cap - 1, d_stat + 1);
+    b2s_int_count_launches(1);
+    unsigned long long longest = 0;
+    PIT_TRY(cudaMemcpyAsync(&longest, d_stat + 1, 8, cudaMemcpyDeviceToHost, st));
+    PIT_TRY(cudaStreamSynchronize(st));
+    ix->longest_run = (int64_t)longest;
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) rc = b2s_int_fail(B2S_ERR_CUDA, "index build failed: %s", cudaGetErrorString(e));
+  } while (0);
+  free_sort(sb, st);
+  if (d_keys) cudaFreeAsync(d_keys, st);
+  if (d_ts_in) cudaFreeAsync(d_ts_in, st);
+  if (d_stat) cudaFreeAsync(d_stat, st);
+  for (void* p : d_cols)
+    if (p) cudaFreeAsync(p, st);
+  cudaStreamSynchronize(st);
+  return rc;
+}
+
+extern "C" int b2s_pit_index_create(const int64_t* keys, const int64_t* ts_ns, int64_t n_rows, const void* const* cols,
+                                    const int32_t* col_bytes, int32_t n_cols, b2s_pit_t* out) {
+  try {  // no C++ exception crosses the C boundary
+    if (!keys || !ts_ns || !out || n_rows <= 0 || n_rows > 0x7fffffffll || n_cols < 0 || n_cols > kMaxOuts || (n_cols && (!cols || !col_bytes)))
+      return b2s_int_fail(B2S_ERR_INVALID, "bad arguments");
+    for (int c = 0; c < n_cols; ++c)
+      if (!cols[c] || (col_bytes[c] != 4 && col_bytes[c] != 8)) return b2s_int_fail(B2S_ERR_INVALID, "column %d: null or not 4 / 8 bytes wide", c);
+    if (!b2s_int_inited()) return b2s_int_fail(B2S_ERR_STATE, "b2s_init was not called (no CUDA device: there is no CPU fallback)");
+    PIT_TRY(cudaSetDevice(b2s_int_device()));
+    auto* ix = new b2s_pit_s();
+    ix->n_rows = n_rows;
+    if (int rc = index_build(ix, keys, ts_ns, n_rows, cols, col_bytes, n_cols, b2s_int_stream())) {
+      b2s_pit_index_destroy(ix);
+      return rc;
+    }
+    *out = ix;
+    return B2S_OK;
+  } catch (const std::exception& e) {
+    return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
+  }
+}
+
+extern "C" int b2s_pit_index_info(b2s_pit_t ix, int64_t* n_rows, int64_t* n_keys, int64_t* longest_run, int32_t* row_words, int64_t* capacity) {
+  try {  // no C++ exception crosses the C boundary
+    if (!ix) return b2s_int_fail(B2S_ERR_INVALID, "null index");
+    if (n_rows) *n_rows = ix->n_rows;
+    if (n_keys) *n_keys = ix->n_keys;
+    if (longest_run) *longest_run = ix->longest_run;
+    if (row_words) *row_words = ix->row_words;
+    if (capacity) *capacity = (int64_t)ix->cap;
+    return B2S_OK;
+  } catch (const std::exception& e) {
+    return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
+  }
+}
+
+static int check_sets(const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols, int32_t n_cols, const int64_t* ts, int64_t n) {
+  if (n < 0 || n > 0x7fffffffll || n_sets < 0 || n_cols < 0 || (n_sets && !sets) || (n_cols && !cols))
+    return b2s_int_fail(B2S_ERR_INVALID, "bad arguments");
+  if (misaligned(ts, 8)) return b2s_int_fail(B2S_ERR_INVALID, "timestamps must be 8-byte aligned");
+  for (int s = 0; s < n_sets; ++s) {
+    const b2s_pit_set& d = sets[s];
+    if (!d.index || (n && !d.keys) || d.n_out < 0 || d.n_out > kMaxOuts || (d.n_out && !d.outs))
+      return b2s_int_fail(B2S_ERR_INVALID, "set %d: null index / keys / outputs", s);
+    if (d.asof && !ts) return b2s_int_fail(B2S_ERR_INVALID, "set %d is an as-of join: entity timestamps are required", s);
+    if (!d.asof && d.index->longest_run > 1)
+      return b2s_int_fail(B2S_ERR_INVALID, "set %d: an exact-key join needs one row per key (a key has %lld)", s, (long long)d.index->longest_run);
+    if (misaligned(d.keys, 8) || misaligned(d.ts_out, 8)) return b2s_int_fail(B2S_ERR_INVALID, "set %d: keys / ts_out must be 8-byte aligned", s);
+    for (int j = 0; j < d.n_out; ++j) {
+      const b2s_pit_out& o = d.outs[j];
+      if ((o.bytes != 4 && o.bytes != 8) || o.src_word < 0 || o.src_word + o.bytes / 4 > d.index->row_words || (n && !o.out) ||
+          misaligned(o.out, o.bytes))
+        return b2s_int_fail(B2S_ERR_INVALID, "set %d output %d: bad width / word / pointer", s, j);
+    }
+  }
+  for (int c = 0; c < n_cols; ++c) {
+    const int b = cols[c].bytes;
+    if ((b != 1 && b != 2 && b != 4 && b != 8) || (n && (!cols[c].src || !cols[c].dst)) || misaligned(cols[c].src, b) || misaligned(cols[c].dst, b))
+      return b2s_int_fail(B2S_ERR_INVALID, "entity column %d: bad width / pointer", c);
+  }
+  return B2S_OK;
+}
+
+// sort (when ts is given) and launch the join over sorted positions [q0, q1); sets / cols hold device pointers.  Sets and
+// columns beyond one launch's parameter block go to further launches over the same range.
+static int launch_join(const int64_t* d_sorted_ts, const uint32_t* d_order, int64_t* d_order_out, int64_t q0, int64_t q1,
+                       const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols, int32_t n_cols, unsigned long long* d_miss,
+                       cudaStream_t st) {
+  int s = 0, c = 0;
+  bool first = true;
+  while (first || s < n_sets || c < n_cols) {
+    JoinParams p{};
+    p.sorted_ts = d_sorted_ts;
+    p.order = d_order;
+    p.order_out = first ? d_order_out : nullptr;
+    p.q0 = q0;
+    p.q1 = q1;
+    p.miss = d_miss + s;
+    int outs = 0;
+    while (s < n_sets && p.n_sets < kMaxSets && outs + sets[s].n_out <= kMaxOuts) {
+      const b2s_pit_set& d = sets[s];
+      SetDesc& sd = p.sets[p.n_sets++];
+      sd.slots = d.index->d_slots;
+      sd.mask = d.index->cap - 1;
+      sd.ts = d.index->d_ts;
+      sd.rows = d.index->d_rows;
+      sd.row_words = d.index->row_words;
+      sd.asof = d.asof;
+      sd.keys = d.keys;
+      sd.ts_out = d.ts_out;
+      sd.found = d.found;
+      sd.out0 = outs;
+      sd.n_out = d.n_out;
+      for (int j = 0; j < d.n_out; ++j) p.outs[outs++] = OutCol{d.outs[j].src_word, d.outs[j].bytes, d.outs[j].miss, d.outs[j].out};
+      ++s;
+    }
+    while (c < n_cols && p.n_cols < kMaxCols) {
+      p.cols[p.n_cols++] = EntCol{cols[c].src, cols[c].dst, cols[c].bytes};
+      ++c;
+    }
+    first = false;
+    if (q1 > q0) {
+      pit_join_kernel<<<grid_for(q1 - q0, 256), 256, 0, st>>>(p);
+      b2s_int_count_launches(1);
+    }
+  }
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return b2s_int_fail(B2S_ERR_CUDA, "join launch failed: %s", cudaGetErrorString(e));
+  return B2S_OK;
+}
+
+static int sort_entities(const int64_t* d_ts, int64_t n, SortBufs& sb, cudaStream_t st) {
+  if (int rc = alloc_sort(sb, n, st)) return rc;
+  PIT_TRY(cudaMemcpyAsync(sb.k[0], d_ts, n * 8, cudaMemcpyDeviceToDevice, st));
+  return radix_sort(sb, false, n, st);
+}
+
+extern "C" int b2s_pit_join_device(const int64_t* d_ts, int64_t n, const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols,
+                                   int32_t n_cols, int64_t* d_order, uint64_t* d_miss, void* stream) {
+  try {  // no C++ exception crosses the C boundary
+    if (int rc = check_sets(sets, n_sets, cols, n_cols, d_ts, n)) return rc;
+    if (n_sets && !d_miss) return b2s_int_fail(B2S_ERR_INVALID, "null miss counters");
+    if (misaligned(d_order, 8) || misaligned(d_miss, 8)) return b2s_int_fail(B2S_ERR_INVALID, "order / miss must be 8-byte aligned");
+    if (n == 0) return B2S_OK;
+    PIT_TRY(cudaSetDevice(b2s_int_device()));
+    cudaStream_t st = stream ? (cudaStream_t)stream : b2s_int_stream();
+    SortBufs sb{};
+    int rc = B2S_OK;
+    if (d_ts) rc = sort_entities(d_ts, n, sb, st);
+    if (!rc)
+      rc = launch_join(d_ts ? reinterpret_cast<const int64_t*>(sb.k[0]) : nullptr, d_ts ? sb.v[0] : nullptr, d_order, 0, n, sets, n_sets,
+                       cols, n_cols, reinterpret_cast<unsigned long long*>(d_miss), st);
+    free_sort(sb, st);
+    return rc;
+  } catch (const std::exception& e) {
+    return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
+  }
+}
+
+extern "C" int b2s_pit_join_host(const int64_t* ts, int64_t n, const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols,
+                                 int32_t n_cols, int64_t* order, uint64_t* miss, b2s_stats* stats) {
+  try {  // no C++ exception crosses the C boundary
+    if (int rc = check_sets(sets, n_sets, cols, n_cols, ts, n)) return rc;
+    if (n_sets && !miss) return b2s_int_fail(B2S_ERR_INVALID, "null miss counters");
+    if (n == 0) {
+      for (int s = 0; s < n_sets; ++s) miss[s] = 0;
+      return B2S_OK;
+    }
+    PIT_TRY(cudaSetDevice(b2s_int_device()));
+    cudaStream_t st = b2s_int_stream(), cs = b2s_int_copy_stream();
+    // device mirrors of every input and output: one block, each array 256-byte aligned
+    std::vector<std::pair<const void*, size_t>> ins;   // host source, bytes
+    std::vector<std::pair<void*, size_t>> outs;        // host destination, element bytes (copied back per row range)
+    std::vector<b2s_pit_set> dsets(sets, sets + n_sets);
+    std::vector<std::vector<b2s_pit_out>> douts(n_sets);
+    std::vector<b2s_pit_col> dcols(cols, cols + n_cols);
+    size_t total = 0;
+    auto reserve = [&](size_t bytes) {
+      const size_t off = total;
+      total += (bytes + 255) / 256 * 256;
+      return off;
+    };
+    std::vector<size_t> in_off, out_off;
+    auto add_in = [&](const void* h, size_t bytes) { ins.push_back({h, bytes}); in_off.push_back(reserve(bytes)); };
+    auto add_out = [&](void* h, size_t elem) { outs.push_back({h, elem}); out_off.push_back(reserve((size_t)n * elem)); };
+    if (ts) add_in(ts, (size_t)n * 8);
+    for (int s = 0; s < n_sets; ++s) {
+      add_in(sets[s].keys, (size_t)n * 8);
+      for (int j = 0; j < sets[s].n_out; ++j) add_out(sets[s].outs[j].out, sets[s].outs[j].bytes);
+      if (sets[s].ts_out) add_out(sets[s].ts_out, 8);
+      if (sets[s].found) add_out(sets[s].found, 1);
+    }
+    for (int c = 0; c < n_cols; ++c) {
+      add_in(cols[c].src, (size_t)n * cols[c].bytes);
+      add_out(cols[c].dst, cols[c].bytes);
+    }
+    if (order) add_out(order, 8);
+    const size_t miss_off = reserve(8 * (size_t)std::max(n_sets, 1));
+    char* d_block = nullptr;
+    SortBufs sb{};
+    int rc = B2S_OK;
+    cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
+    std::vector<cudaEvent_t> range_ev;
+    do {
+      for (auto& e : ev) PIT_TRY(cudaEventCreate(&e));
+      PIT_TRY(cudaMallocAsync(&d_block, total, st));
+      PIT_TRY(cudaMemsetAsync(d_block + miss_off, 0, 8 * (size_t)std::max(n_sets, 1), st));
+      PIT_TRY(cudaEventRecord(ev[0], st));
+      for (size_t i = 0; i < ins.size(); ++i) PIT_TRY(cudaMemcpyAsync(d_block + in_off[i], ins[i].first, ins[i].second, cudaMemcpyHostToDevice, st));
+      PIT_TRY(cudaEventRecord(ev[1], st));
+      // the same descriptors over the device mirrors
+      size_t ii = ts ? 1 : 0, oi = 0;
+      for (int s = 0; s < n_sets; ++s) {
+        dsets[s].keys = reinterpret_cast<const int64_t*>(d_block + in_off[ii++]);
+        douts[s].assign(sets[s].outs, sets[s].outs + sets[s].n_out);
+        for (auto& o : douts[s]) o.out = d_block + out_off[oi++];
+        dsets[s].outs = douts[s].data();
+        if (sets[s].ts_out) dsets[s].ts_out = reinterpret_cast<int64_t*>(d_block + out_off[oi++]);
+        if (sets[s].found) dsets[s].found = reinterpret_cast<uint8_t*>(d_block + out_off[oi++]);
+      }
+      for (int c = 0; c < n_cols; ++c) {
+        dcols[c].src = d_block + in_off[ii++];
+        dcols[c].dst = d_block + out_off[oi++];
+      }
+      int64_t* d_order = order ? reinterpret_cast<int64_t*>(d_block + out_off[oi++]) : nullptr;
+      const int64_t* d_ts = ts ? reinterpret_cast<const int64_t*>(d_block + in_off[0]) : nullptr;
+      if (d_ts && (rc = sort_entities(d_ts, n, sb, st))) break;
+      // row ranges of sorted positions: range k's results go back on the copy stream while range k + 1 is joined
+      const int64_t kRange = 1 << 20;
+      const int n_ranges = (int)((n + kRange - 1) / kRange);
+      range_ev.assign(n_ranges, nullptr);
+      for (auto& e : range_ev) PIT_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+      auto* d_miss = reinterpret_cast<unsigned long long*>(d_block + miss_off);
+      for (int k = 0; k < n_ranges && !rc; ++k) {
+        const int64_t q0 = (int64_t)k * kRange, q1 = std::min<int64_t>(n, q0 + kRange);
+        rc = launch_join(d_ts ? reinterpret_cast<const int64_t*>(sb.k[0]) : nullptr, d_ts ? sb.v[0] : nullptr, d_order, q0, q1, dsets.data(),
+                         n_sets, dcols.data(), n_cols, d_miss, st);
+        if (rc) break;
+        PIT_TRY(cudaEventRecord(range_ev[k], st));
+        PIT_TRY(cudaStreamWaitEvent(cs, range_ev[k], 0));
+        for (size_t i = 0; i < outs.size(); ++i) {
+          const size_t el = outs[i].second;
+          PIT_TRY(cudaMemcpyAsync(static_cast<char*>(outs[i].first) + q0 * el, d_block + out_off[i] + q0 * el, (size_t)(q1 - q0) * el,
+                                  cudaMemcpyDeviceToHost, cs));
+        }
+      }
+      if (rc) break;
+      PIT_TRY(cudaEventRecord(ev[2], st));
+      if (n_sets) PIT_TRY(cudaMemcpyAsync(miss, d_miss, 8 * (size_t)n_sets, cudaMemcpyDeviceToHost, cs));
+      PIT_TRY(cudaStreamSynchronize(cs));
+      PIT_TRY(cudaStreamSynchronize(st));
+      if (stats) {
+        memset(stats, 0, sizeof(*stats));
+        stats->rows = n;
+        cudaEventElapsedTime(&stats->h2d_ms, ev[0], ev[1]);
+        cudaEventElapsedTime(&stats->kernel_ms, ev[1], ev[2]);  // sort + join (the copies back overlap the join)
+        stats->kernels = n_ranges;
+      }
+    } while (0);
+    free_sort(sb, st);
+    if (d_block) cudaFreeAsync(d_block, st);
+    cudaStreamSynchronize(st);
+    for (auto& e : ev)
+      if (e) cudaEventDestroy(e);
+    for (auto& e : range_ev)
+      if (e) cudaEventDestroy(e);
+    return rc;
+  } catch (const std::exception& e) {
+    return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
+  }
+}

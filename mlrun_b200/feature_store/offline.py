@@ -1,0 +1,415 @@
+"""Point-in-time correct training sets on the device: `get_offline_features` as one as-of join per feature set.
+
+Plugin-API mirror of mlrun.feature_store.get_offline_features (feature_store/api.py:99, feature_vector.py:727) on the local
+engine, whose BaseMerger.merge (retrieval/base.py:412-468) merges each feature set of the vector onto the entity frame with
+pandas.merge_asof (retrieval/local_merger.py:29-81).  Storage is out of scope, as for the online table: a feature set's offline
+frame is registered beside its `FeatureSet` mirror (`register_offline_frame`), which builds the set's device index once
+(`b2s_pit_index_*`, include/b200serve.h).  A query sorts the entity rows by timestamp and joins every feature set in one
+`b2s_pit_join_host` call; the host only assembles the columns the reference's frame has, with its names and dtypes.
+
+Divergences (DESIGN.md §2): entity rows with equal timestamps keep their input order (pandas' quicksort may reorder them), and
+of feature-set rows with equal (key, timestamp) the last in input order is taken.
+"""
+
+import ctypes as C
+
+import numpy as np
+
+from .. import _native as nat
+from ..lowering import LoweringError
+from ..serving.resolve import MLRunInvalidArgumentError
+from .ingest import _INT_DTYPES
+from .online import _hash_strings
+
+_OFFLINE = {}  # feature-set name -> OfflineSource
+_NAN32 = 0x7FC00000
+_NAT = -(1 << 63)
+_UNIT_NS = {"s": 10**9, "ms": 10**6, "us": 10**3, "ns": 1}
+
+
+class PitIndex:
+    """b2s_pit index of one feature set: int64 keys, int64 nanosecond timestamps, 4- / 8-byte feature columns"""
+
+    def __init__(self, keys, ts_ns, cols):
+        nat.init()
+        self._lib = nat.load()
+        keys = np.ascontiguousarray(keys, dtype=np.int64)
+        ts_ns = np.ascontiguousarray(ts_ns, dtype=np.int64)
+        cols = [np.ascontiguousarray(c) for c in cols]
+        ptrs = (C.c_void_p * max(len(cols), 1))(*[c.ctypes.data for c in cols])
+        widths = np.array([c.dtype.itemsize for c in cols] or [0], dtype=np.int32)
+        self._h = C.c_void_p()
+        nat.check(self._lib.b2s_pit_index_create(keys.ctypes.data, ts_ns.ctypes.data, len(keys), ptrs, nat._p(widths, C.c_int32),
+                                                 len(cols), C.byref(self._h)))
+        n_rows, n_keys, longest, cap = C.c_int64(), C.c_int64(), C.c_int64(), C.c_int64()
+        words = C.c_int32()
+        nat.check(self._lib.b2s_pit_index_info(self._h, C.byref(n_rows), C.byref(n_keys), C.byref(longest), C.byref(words),
+                                               C.byref(cap)))
+        self.n_rows, self.n_keys, self.longest_run, self.row_words = n_rows.value, n_keys.value, longest.value, words.value
+
+    def close(self):
+        if self._h:
+            self._lib.b2s_pit_index_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def pit_join(ts, sets, cols, with_stats=False):
+    """ts: int64 ns [n] or None (input order kept); sets: [(PitIndex, int64 keys [n], asof, [(src_word, dtype, miss bits)])];
+    cols: entity arrays [n] (1, 2, 4 or 8 bytes) -> (order int64 [n], [(outputs, ts_out, found bool)] per set, permuted cols,
+    misses per set)"""
+    lib = nat.init()
+    n = len(ts) if ts is not None else len(cols[0]) if cols else len(sets[0][1]) if sets else 0
+    ts = None if ts is None else np.ascontiguousarray(ts, dtype=np.int64)
+    keep = []  # arrays the descriptors point into
+    c_sets = (nat.PitSet * max(len(sets), 1))()
+    results = []
+    for i, (index, keys, asof, outs) in enumerate(sets):
+        keys = np.ascontiguousarray(keys, dtype=np.int64)
+        arrays = [np.empty(n, dtype=dt) for _w, dt, _m in outs]
+        ts_out, found = np.empty(n, dtype=np.int64), np.empty(n, dtype=np.uint8)
+        descs = (nat.PitOut * max(len(outs), 1))(*[nat.PitOut(w, np.dtype(dt).itemsize, m, a.ctypes.data)
+                                                   for (w, dt, m), a in zip(outs, arrays)])
+        keep += [keys, descs]
+        c_sets[i] = nat.PitSet(index._h, keys.ctypes.data, int(asof), len(outs), descs, ts_out.ctypes.data, found.ctypes.data)
+        results.append((arrays, ts_out, found))
+    srcs = [np.ascontiguousarray(c) for c in cols]
+    dsts = [np.empty_like(c) for c in srcs]
+    c_cols = (nat.PitCol * max(len(cols), 1))(*[nat.PitCol(s.ctypes.data, d.ctypes.data, s.dtype.itemsize) for s, d in zip(srcs, dsts)])
+    order = np.empty(n, dtype=np.int64)
+    miss = np.zeros(max(len(sets), 1), dtype=np.uint64)
+    stats = nat.Stats()
+    nat.check(lib.b2s_pit_join_host(None if ts is None else ts.ctypes.data, n, c_sets, len(sets), c_cols, len(cols), order.ctypes.data,
+                                    miss.ctypes.data, C.byref(stats)))
+    res = (order, [(a, t, f.view(bool)) for a, t, f in results], dsts, miss[:len(sets)])
+    return res + (stats.as_dict(),) if with_stats else res
+
+
+# ---------------------------------------------------------------------------------------------------------- host encoding
+def _ns(series, what):
+    """datetime64 column -> (int64 nanoseconds, unit), NaT as INT64_MIN; LoweringError for other dtypes"""
+    dt = series.dtype
+    if getattr(dt, "tz", None) is not None or dt.kind != "M":
+        raise LoweringError(f"{what} has dtype {dt}: the as-of join takes tz-naive datetime64 timestamps")
+    unit = np.datetime_data(dt)[0]
+    if unit not in _UNIT_NS:
+        raise LoweringError(f"{what} has unit {unit!r}: the as-of join takes s / ms / us / ns timestamps")
+    raw = series.to_numpy().view(np.int64)
+    f = _UNIT_NS[unit]
+    nat_mask = raw == _NAT
+    if f > 1 and (np.abs(raw[~nat_mask]) > np.iinfo(np.int64).max // f).any():
+        raise LoweringError(f"{what} holds timestamps outside the nanosecond range")
+    return np.where(nat_mask, _NAT, raw * f), unit
+
+
+def _key_kind(frame, names, what):
+    """-> "int" | "pair" | "str" for the key columns `names` of `frame`"""
+    dts = [frame[k].dtype for k in names]
+    if len(names) == 1 and dts[0].kind in "iu" and dts[0] != np.uint64:
+        return "int"
+    if len(names) == 2 and all(str(d) == "int32" for d in dts):
+        return "pair"
+    if len(names) == 1 and (dts[0] == object or str(dts[0]) in ("str", "string")):
+        return "str"
+    raise LoweringError(f"{what}: keys {names} of dtypes {[str(d) for d in dts]} are not lowered (one int32 / int64 column, two "
+                        "int32 columns or one string column)")
+
+
+def _encode_keys(frame, names, kind, what):
+    if kind == "int":
+        return frame[names[0]].to_numpy().astype(np.int64)
+    if kind == "pair":
+        hi, lo = (frame[k].to_numpy().astype(np.int64) for k in names)
+        return (hi << 32) | (lo & 0xFFFFFFFF)
+    col = frame[names[0]]
+    if col.isna().any():
+        raise LoweringError(f"{what}: missing values in the string key {names[0]!r}")
+    return _hash_strings(col.to_numpy())
+
+
+class OfflineSource:
+    """one feature set's offline frame, registered with its device index (built once)"""
+
+    def __init__(self, featureset, frame):
+        self.featureset = featureset
+        self.name = featureset.name
+        self.entities = [e.name for e in featureset.entities]
+        self.timestamp_key = featureset.timestamp_key
+        if frame.index.names[0]:
+            frame = frame.reset_index()
+        missing = [k for k in self.entities + ([self.timestamp_key] if self.timestamp_key else []) if k not in frame.columns]
+        if missing:
+            raise MLRunInvalidArgumentError(f"feature set {self.name}: the offline frame has no column {missing[0]!r}")
+        if not self.entities:
+            raise LoweringError(f"feature set {self.name} has no entities: only keyed feature sets are joined on the device")
+        self.frame = frame
+        self.key_kind = _key_kind(frame, self.entities, f"feature set {self.name}")
+        keys = _encode_keys(frame, self.entities, self.key_kind, f"feature set {self.name}")
+        if self.key_kind == "str":
+            strings = frame[self.entities[0]].to_numpy()
+            if len(np.unique(keys)) != len(set(strings.tolist())):
+                raise MLRunInvalidArgumentError(f"feature set {self.name}: two entity keys share a 64-bit hash")
+        if self.timestamp_key:
+            ts_ns, _unit = _ns(frame[self.timestamp_key], f"feature set {self.name} timestamp {self.timestamp_key!r}")
+            self.has_nat = bool((ts_ns == _NAT).any())
+            # the coarsest unit every timestamp is a whole number of: a query whose timestamps are coarser would round them
+            self.ts_factor = max((f for f in _UNIT_NS.values() if not (ts_ns[ts_ns != _NAT] % f).any()), default=1)
+        else:
+            ts_ns, self.has_nat, self.ts_factor = np.zeros(len(frame), dtype=np.int64), False, 10**9
+        self.features, cols, word = {}, [], 0
+        for name in frame.columns:
+            if name in self.entities or name == self.timestamp_key:
+                continue
+            a = frame[name].to_numpy()
+            s = str(frame[name].dtype)
+            if s == "float32":
+                stored, miss = a, _NAN32
+            elif s in _INT_DTYPES:
+                stored, miss = a.astype(np.int32), 0
+            elif s.startswith("datetime64") and getattr(frame[name].dtype, "tz", None) is None:
+                stored, miss = a.view(np.int64), _NAT
+            else:
+                self.features[name] = (None, s, None)  # refused when a vector selects it
+                continue
+            self.features[name] = (word, s, miss)
+            cols.append(stored)
+            word += stored.dtype.itemsize // 4
+        self.index = PitIndex(keys, ts_ns, cols)
+
+    def close(self):
+        self.index.close()
+
+
+def register_offline_frame(featureset, frame):
+    """hand over a feature set's offline rows (the frame its targets would hold); the device index is built here"""
+    old = _OFFLINE.pop(featureset.name, None)
+    if old is not None:
+        old.close()
+    src = OfflineSource(featureset, frame)
+    _OFFLINE[featureset.name] = src
+    return src
+
+
+class FeatureVector:
+    """mlrun.feature_store.FeatureVector (feature_vector.py): a name and features "set.feature [as alias]" / "set.*\""""
+
+    def __init__(self, name=None, features=None, label_feature=None, description=None, with_indexes=None, join_graph=None,
+                 relations=None):
+        self.name = name
+        self.features = list(features or [])
+        self.label_feature = label_feature
+        self.description = description
+        self.with_indexes = with_indexes
+        self.join_graph = join_graph
+        self.relations = relations
+
+
+class OfflineVectorResponse:
+    """feature_vector.py OfflineVectorResponse: the training set as ordered columns (`columns`, in the frame's row order)"""
+
+    def __init__(self, columns, index_columns):
+        self.columns = columns
+        self._index_columns = index_columns
+
+    @property
+    def status(self):
+        return "completed"
+
+    def to_dataframe(self, to_pandas=True):
+        import pandas as pd
+
+        frame = pd.DataFrame(dict(self.columns), copy=False)
+        if self._index_columns:
+            frame = frame.set_index(self._index_columns)
+        return frame
+
+
+def _parse(vector):
+    """features -> {set: [(feature, alias)]} in vector order"""
+    fields = {}
+    for spec in vector.features:
+        spec, alias = spec.split(" as ", 1) if " as " in spec else (spec, None)
+        if "." not in spec:
+            raise MLRunInvalidArgumentError(f"feature {spec!r} must be named <feature set>.<feature>")
+        name, feat = spec.strip().split(".", 1)
+        if name not in _OFFLINE:
+            raise MLRunInvalidArgumentError(f"feature set {name!r} has no registered offline frame (register_offline_frame)")
+        src = _OFFLINE[name]
+        feats = list(src.features) if feat == "*" else [feat]
+        for f in feats:
+            if f not in src.features:
+                raise MLRunInvalidArgumentError(f"feature {f!r} is not in feature set {name}")
+            if src.features[f][0] is None:
+                raise LoweringError(f"feature {name}.{f} has dtype {src.features[f][1]}: the device joins float32, (u)int8/16/32, "
+                                    "bool and datetime64 features")
+            fields.setdefault(name, []).append((f, alias.strip() if alias else None))
+    if not fields:
+        raise MLRunInvalidArgumentError("No features in vector. Make sure to infer the schema on all the feature sets first")
+    return fields
+
+
+def _restore(values, dtype, found, alive):
+    """a gathered column in the reference's dtype: unchanged when `found` is None or no row in `alive` misses (rows an
+    earlier inner join removed do not count); with a miss, ints become float64 and bool object, with NaN (float32 and
+    datetime64 columns carry NaN / NaT already)"""
+    if dtype.startswith("datetime64"):
+        return values.view(dtype)
+    if dtype == "float32":
+        return values
+    if found is None or found[alive].all():
+        return values.astype(dtype)
+    out = values.astype(bool).astype(object) if dtype == "bool" else values.astype(np.float64)
+    out[~found] = np.nan
+    return out
+
+
+def get_offline_features(feature_vector, entity_rows=None, entity_timestamp_column=None, target=None, run_config=None,
+                         drop_columns=None, start_time=None, end_time=None, with_indexes=False, update_stats=False, engine=None,
+                         engine_args=None, query=None, order_by=None, spark_service=None, timestamp_for_filtering=None,
+                         additional_filters=None):
+    """feature_store/api.py:99 on the local engine: the training frame of `feature_vector` for `entity_rows`, point-in-time
+    correct per feature set.  What the device does not run is refused with LoweringError (there is no pandas fallback)."""
+    vector = feature_vector
+    if engine not in (None, "local"):
+        raise LoweringError(f"engine {engine!r}: only the local engine's merge runs on the device")
+    if start_time is not None or end_time is not None or timestamp_for_filtering is not None:
+        raise LoweringError("start_time / end_time / timestamp_for_filtering are storage filters: not lowered")
+    if query is not None or order_by is not None or additional_filters is not None:
+        raise LoweringError("query / order_by / additional_filters are not lowered")
+    if target is not None:
+        raise LoweringError("targets are storage (out of scope): the training set is returned")
+    if drop_columns is not None or update_stats or run_config is not None or spark_service is not None:
+        raise LoweringError("drop_columns / update_stats / run_config / spark_service are not lowered")
+    if getattr(vector, "join_graph", None) is not None or getattr(vector, "relations", None):
+        raise LoweringError("join graphs and relations between feature sets are not lowered: every set joins the entity frame")
+    if getattr(vector, "label_feature", None):
+        raise LoweringError("label_feature (dropping rows without a label) is not lowered")
+    if entity_rows is None:
+        raise LoweringError("without entity_rows the feature sets are merged among themselves: not lowered")
+    drop_indexes = not (vector.with_indexes or with_indexes)
+    fields = _parse(vector)
+    if entity_rows.index.names[0]:
+        entity_rows = entity_rows.reset_index()
+    n = len(entity_rows)
+    names = [str(c) for c in entity_rows.columns]
+    if len(set(names)) != len(names):
+        raise LoweringError("duplicate column names in the entity frame")
+
+    # the join of each set (base.py:430-460): as-of when it has a timestamp key and an entity timestamp column is known
+    entity_ts = entity_timestamp_column
+    plan, ts_col = [], entity_ts
+    for name in fields:
+        src = _OFFLINE[name]
+        missing = [k for k in src.entities if k not in entity_rows.columns]
+        if missing:
+            raise LoweringError(f"feature set {name}: the entity frame has no key column {missing[0]!r} (relations between "
+                                "differently keyed feature sets are not lowered)")
+        asof = bool(src.timestamp_key and ts_col)
+        if asof and ts_col != entity_ts:
+            raise LoweringError(f"feature set {name} would join as-of on another feature set's timestamp {ts_col!r}: pass "
+                                "entity_timestamp_column")
+        if not asof and src.index.longest_run > 1:
+            raise LoweringError(f"feature set {name} joins on its keys alone and has several rows per key: not lowered")
+        plan.append((name, src, asof))
+        ts_col = ts_col or src.timestamp_key
+    any_asof = any(a for _n, _s, a in plan)
+    ts_ns = unit = None
+    if any_asof:
+        if entity_ts not in entity_rows.columns:
+            raise KeyError(entity_ts)
+        ts_ns, unit = _ns(entity_rows[entity_ts], f"entity timestamp {entity_ts!r}")
+        if (ts_ns == _NAT).any():
+            raise ValueError("Merge keys contain null values on left side")
+        for name, src, asof in plan:
+            if asof and src.has_nat:
+                raise ValueError("Merge keys contain null values on right side")
+            if asof and src.ts_factor < _UNIT_NS[unit]:
+                raise LoweringError(f"feature set {name}: timestamps finer than the entity column's unit {unit!r} would be "
+                                    "rounded by the reference's cast: not lowered")
+
+    # device call: every set's selected words, its timestamps and found flags; numeric entity columns permuted alongside
+    sets = []
+    for name, src, asof in plan:
+        kind = _key_kind(entity_rows, src.entities, f"entity keys of {name}")
+        if kind != src.key_kind:
+            raise LoweringError(f"feature set {name}: entity keys are {kind}, the set's are {src.key_kind}")
+        keys = _encode_keys(entity_rows, src.entities, kind, f"entity keys of {name}")
+        outs = []
+        for f, _a in fields[name]:
+            word, s, miss = src.features[f]
+            outs.append((word, np.int64 if s.startswith("datetime64") else np.float32 if s == "float32" else np.int32, miss))
+        sets.append((src.index, keys, asof, outs))
+    dev_cols = [c for c in entity_rows.columns if entity_rows[c].dtype.kind in "iufMb" and getattr(entity_rows[c].dtype, "tz", None) is None
+                and isinstance(entity_rows[c].dtype, np.dtype)]
+    arrays = [entity_rows[c].to_numpy() for c in dev_cols]
+    order, joined, permuted, _miss = pit_join(ts_ns, sets, arrays) if n else (
+        np.zeros(0, np.int64), [([np.zeros(0, dt) for _w, dt, _m in s[3]], np.zeros(0, np.int64), np.zeros(0, bool)) for s in sets],
+        [a[:0] for a in arrays], None)
+    moved = dict(zip(dev_cols, permuted))
+
+    # the merged frame, set by set (local_merger.py:58-66 / 93-100): right columns after the left ones, the keys and an
+    # equally named timestamp once, colliding names suffixed `_<set>_` (then dropped)
+    cols = {}
+    for c in entity_rows.columns:
+        if c in moved:
+            v = moved[c]
+            cols[c] = v.view(entity_rows[c].dtype) if v.dtype != entity_rows[c].dtype else v
+        else:  # strings, categories, objects: permuted on the host in the device's order
+            cols[c] = entity_rows[c].take(order).reset_index(drop=True).array
+    merge_drop = []
+    alive = np.ones(n, dtype=bool)
+    alias = {}
+    for (name, src, asof), (vals, ts_out, found), (_i, _k, _a, outs) in zip(plan, joined, sets):
+        head = src.entities + ([src.timestamp_key] if src.timestamp_key else [])
+        right = {}
+        if src.timestamp_key and not (asof and src.timestamp_key == entity_ts):
+            # as-of: cast to the entity column's unit (base.py:389-410); exact: the set's own unit
+            tdt = np.dtype(f"datetime64[{unit}]") if asof else src.frame[src.timestamp_key].dtype
+            right[src.timestamp_key] = np.where(ts_out == _NAT, _NAT, ts_out // _UNIT_NS[np.datetime_data(tdt)[0]]).view(tdt)
+        for (f, _a), v in zip(fields[name], vals):
+            right[f"{f}_{name}"] = _restore(v, src.features[f][1], found if asof else None, alive)
+        if not asof:
+            alive &= found
+        for c, v in right.items():
+            out_name = c
+            if c in cols:
+                out_name = f"{c}_{name}_"
+                if out_name not in merge_drop:
+                    merge_drop.append(out_name)
+            cols[out_name] = v
+        new = [(c, c) for c in head] if not drop_indexes else []
+        new += [(f"{f}_{name}", a or f) for f, a in fields[name]]
+        alias.update(dict(new))
+
+    # base.py:113-120, 253-254, 325-341: drop keys / timestamps unless with_indexes, rename to aliases
+    drop = []
+    for c in ([entity_ts] if drop_indexes and entity_ts else []):
+        drop.append(c)
+    index_columns = []
+    for name, src, _asof in plan:
+        if drop_indexes and src.timestamp_key:
+            drop.append(src.timestamp_key)
+        for k in src.entities:
+            if k not in index_columns:
+                index_columns.append(k)
+            if drop_indexes:
+                drop.append(k)
+    drop += merge_drop
+    if not drop_indexes and ts_col and ts_col not in alias.values():
+        alias[ts_col] = ts_col
+    result = {}
+    for c, v in cols.items():
+        new = alias.get(c, c)
+        if new in drop:
+            continue
+        if new in result:
+            raise LoweringError(f"two columns of the training set are named {new!r}")
+        result[new] = v[alive] if not alive.all() else v
+    if drop_indexes or not all(k in result for k in index_columns):
+        index_columns = []
+    return OfflineVectorResponse(result, index_columns)
