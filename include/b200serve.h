@@ -336,11 +336,13 @@ int b2s_cols_destroy(b2s_cols_t plan);
 int b2s_cols_add_copy(b2s_cols_t plan, int32_t src_slot, int32_t kind, int32_t has_fill, float fill, int32_t keep,
                       int32_t check, double cmin, double cmax, int32_t* out_slot, int32_t* check_counter);
 /* MapValues._map_value (steps.py:189-201): first i with lo[i] <= v < hi[i] -> vals[i]; no hit: v passes through
- * and counters[miss_counter] counts the row.  The output slot holds float32. */
+ * and counters[miss_counter] counts the row.  The output slot holds int32 when the source is B2S_COL_I32 and every
+ * vals[i] is an int32 integer, so every int32 value that passes through stays exact; otherwise it holds float32, which
+ * rounds int32 values beyond 2^24 that pass through (mlrun_b200's ingest refuses frames holding such values). */
 int b2s_cols_add_range_map(b2s_cols_t plan, int32_t src_slot, int32_t kind, int32_t has_fill, float fill, const double* lo,
                            const double* hi, const double* vals, int32_t n, int32_t check, double cmin, double cmax,
                            int32_t* out_slot, int32_t* miss_counter, int32_t* check_counter);
-/* MapValues exact-match branch (steps.py:200-201): v == keys[i] -> vals[i]. */
+/* MapValues exact-match branch (steps.py:200-201): v == keys[i] -> vals[i].  Output as for range maps. */
 int b2s_cols_add_value_map(b2s_cols_t plan, int32_t src_slot, int32_t kind, int32_t has_fill, float fill, const double* keys,
                            const double* vals, int32_t n, int32_t check, double cmin, double cmax, int32_t* out_slot,
                            int32_t* miss_counter, int32_t* check_counter);
@@ -353,7 +355,10 @@ int b2s_cols_add_date_part(b2s_cols_t plan, int32_t src_slot, int32_t part, int3
 int b2s_cols_finalize(b2s_cols_t plan);
 int b2s_cols_info(b2s_cols_t plan, int32_t* n_out_slots, int32_t* n_counters);
 /* Device-resident run: slot s of the input starts at d_in + s * in_slot_stride (bytes, multiple of 8, >= 4 * n_rows);
- * d_counters (n_counters uint64, zeroed by the caller) accumulates.  Asynchronous on `stream`. */
+ * d_counters (n_counters uint64, zeroed by the caller) accumulates.  Asynchronous on `stream`.  Returns B2S_ERR_INVALID,
+ * before any launch, when d_in or d_out is NULL (n_rows > 0) or not 4-byte aligned, or not 8-byte aligned while the plan
+ * reads (d_in) or writes (d_out) an 8-byte column, or when d_counters is not 8-byte aligned.  Bases and strides that are
+ * not multiples of 16 bytes are legal; such runs take the kernel's 4- and 8-byte access paths. */
 int b2s_cols_run_device(b2s_cols_t plan, const void* d_in, int64_t in_slot_stride, int64_t n_rows, void* d_out,
                         int64_t out_slot_stride, uint64_t* d_counters, void* stream);
 /* Host run: one pointer per input slot the plan reads (an 8-byte column: pointer at its first slot), one per output

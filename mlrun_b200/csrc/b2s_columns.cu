@@ -4,6 +4,7 @@
 #include <exception>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdint>
 #include <cstdlib>
 #include <cstring>
@@ -31,6 +32,7 @@ struct b2s_cols_s {
   std::vector<uint8_t> out_words;  // per output slot: 1, or 2 for the first slot of an 8-byte column (its second slot holds 0)
   std::vector<uint8_t> in_used;    // per input slot: 0 unused, 1 4-byte, 2 first slot of an 8-byte column
   int32_t n_counters = 0;
+  bool wide_in = false, wide_out = false;  // the plan reads / writes an 8-byte column (set by finalize)
   // device
   ColOp* d_ops = nullptr;
   double* d_tab = nullptr;
@@ -131,6 +133,8 @@ static int add_map(b2s_cols_t c, int kind_op, int32_t src_slot, int32_t kind, in
   c->tab.insert(c->tab.end(), a, a + n);
   if (kind_op == CK_RANGE) c->tab.insert(c->tab.end(), b, b + n);
   c->tab.insert(c->tab.end(), v, v + n);
+  // an int32 column mapped to int32 values stays int32: a value that passes through is exact, where float32 rounds beyond 2^24
+  op.int_out = op.src_int && std::all_of(v, v + n, [](double x) { return x == std::floor(x) && x >= -2147483648.0 && x <= 2147483647.0; });
   op.miss = c->n_counters++;
   if (miss_counter) *miss_counter = op.miss;
   set_check(c, op, check, cmin, cmax, check_counter);
@@ -214,6 +218,8 @@ extern "C" int b2s_cols_finalize(b2s_cols_t c) {
     if (c->finalized) return B2S_OK;
     if (c->ops.empty()) return b2s_int_fail(B2S_ERR_INVALID, "plan has no column ops");
     if (!b2s_int_inited()) return b2s_int_fail(B2S_ERR_STATE, "b2s_init was not called (no CUDA device: there is no CPU fallback)");
+    c->wide_in = std::find(c->in_used.begin(), c->in_used.end(), 2) != c->in_used.end();
+    c->wide_out = std::find(c->out_words.begin(), c->out_words.end(), 2) != c->out_words.end();
     COL_TRY(cudaSetDevice(b2s_int_device()));
     COL_TRY(cudaMalloc(&c->d_ops, c->ops.size() * sizeof(ColOp)));
     COL_TRY(cudaMemcpy(c->d_ops, c->ops.data(), c->ops.size() * sizeof(ColOp), cudaMemcpyHostToDevice));
@@ -240,6 +246,19 @@ extern "C" int b2s_cols_info(b2s_cols_t c, int32_t* n_out_slots, int32_t* n_coun
   } catch (const std::exception& e) {
     return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
   }
+}
+
+// device buffers of a run: 4-byte words, 8-byte words where the plan has an 8-byte column (slot strides are multiples of 8,
+// so the base decides), 8-byte counters.  Bases off 16 bytes are legal: those runs take the kernel's scalar paths.
+static int check_device_buffers(b2s_cols_t c, const void* d_in, const void* d_out, const void* d_counters) {
+  if (!d_in || !d_out) return b2s_int_fail(B2S_ERR_INVALID, "d_in and d_out must not be NULL");
+  const uintptr_t in_align = c->wide_in ? 7 : 3, out_align = c->wide_out ? 7 : 3;
+  if (reinterpret_cast<uintptr_t>(d_in) & in_align)
+    return b2s_int_fail(B2S_ERR_INVALID, "d_in must be %d-byte aligned for this plan", (int)in_align + 1);
+  if (reinterpret_cast<uintptr_t>(d_out) & out_align)
+    return b2s_int_fail(B2S_ERR_INVALID, "d_out must be %d-byte aligned for this plan", (int)out_align + 1);
+  if (c->n_counters && (reinterpret_cast<uintptr_t>(d_counters) & 7)) return b2s_int_fail(B2S_ERR_INVALID, "d_counters must be 8-byte aligned");
+  return B2S_OK;
 }
 
 static int launch_cols(b2s_cols_t c, const void* d_in, int64_t in_stride, int64_t n_rows, void* d_out, int64_t out_stride,
@@ -276,6 +295,7 @@ extern "C" int b2s_cols_run_device(b2s_cols_t c, const void* d_in, int64_t in_sl
       return b2s_int_fail(B2S_ERR_INVALID, "slot strides must hold n_rows words and be multiples of 8 bytes");
     if (n_rows == 0) return B2S_OK;
     if (c->n_counters && !d_counters) return b2s_int_fail(B2S_ERR_INVALID, "the plan has %d counters: pass a device array", c->n_counters);
+    if (int rc = check_device_buffers(c, d_in, d_out, d_counters)) return rc;
     COL_TRY(cudaSetDevice(b2s_int_device()));
     return launch_cols(c, d_in, in_slot_stride, n_rows, d_out, out_slot_stride, (unsigned long long*)d_counters,
                        stream ? (cudaStream_t)stream : b2s_int_stream());
@@ -289,6 +309,11 @@ extern "C" int b2s_cols_time_device(b2s_cols_t c, const void* const* d_in, int32
   try {  // no C++ exception crosses the C boundary
     if (!c || !c->finalized) return b2s_int_fail(B2S_ERR_STATE, "plan not finalized");
     if (!d_in || n_bufs <= 0 || n_iters <= 0 || !total_ms) return b2s_int_fail(B2S_ERR_INVALID, "bad arguments");
+    if (n_rows < 0 || in_slot_stride < n_rows * 4 || out_slot_stride < n_rows * 4 || (in_slot_stride & 7) || (out_slot_stride & 7))
+      return b2s_int_fail(B2S_ERR_INVALID, "slot strides must hold n_rows words and be multiples of 8 bytes");
+    if (c->n_counters && !d_counters) return b2s_int_fail(B2S_ERR_INVALID, "the plan has %d counters: pass a device array", c->n_counters);
+    for (int i = 0; i < n_bufs; ++i)
+      if (int rc = check_device_buffers(c, d_in[i], d_out, d_counters)) return rc;
     COL_TRY(cudaSetDevice(b2s_int_device()));
     cudaStream_t st = b2s_int_stream();
     std::lock_guard<std::mutex> lk(c->mu);

@@ -272,6 +272,7 @@ class IngestPlan:
         self.out = []  # per output column: (name, slot, how, col)
         self.checks = []  # (counter, column name, validator)
         self.miss = []    # (counter, column name, what)
+        self.rounding_maps = []  # (source slot, column name): maps of an int32 column whose float32 output rounds beyond 2^24
         for c in prog.cols:
             chk = None if c.check is None else c.check[:2]
             if c.op is None:
@@ -282,12 +283,12 @@ class IngestPlan:
                 slot, miss, cnt = plan.add_range_map(c.slot, c.kind, [r[:3] for r in c.arg], fill=c.fill, check=chk)
                 self.ops.append(("range", c.slot, c.kind, c.fill, [r[:3] for r in c.arg], chk))
                 self.miss.append((miss, c.name, "matched no range"))
-                how = ("map", miss, all(isinstance(r[3], (int, np.integer)) and not isinstance(r[3], bool) for r in c.arg))
+                how = ("map", miss, _int_labels(r[3] for r in c.arg), _int32_words(c.kind, [r[2] for r in c.arg]))
             elif c.op == "value":
                 slot, miss, cnt = plan.add_value_map(c.slot, c.kind, {k: v for k, v, _ in c.arg}, fill=c.fill, check=chk)
                 self.ops.append(("value", c.slot, c.kind, c.fill, {k: v for k, v, _ in c.arg}, chk))
                 self.miss.append((miss, c.name, "matched no key"))
-                how = ("map", miss, all(isinstance(r[2], (int, np.integer)) and not isinstance(r[2], bool) for r in c.arg))
+                how = ("map", miss, _int_labels(r[2] for r in c.arg), _int32_words(c.kind, [r[1] for r in c.arg]))
             elif c.op == "onehot":
                 g = c.group
                 if g.first_out is None:
@@ -302,6 +303,8 @@ class IngestPlan:
                 cnt, how = -1, ("date", miss, c.arg in nat.DATE_BOOL_PARTS)
             if cnt >= 0:
                 self.checks.append((cnt, c.name, c.check[2]))
+            if isinstance(how, tuple) and how[0] == "map" and c.kind == I32 and not how[3]:
+                self.rounding_maps.append((c.slot, c.name))
             self.out.append((c.name, slot, how))
         for c in prog.checked_dropped:
             chk = c.check[:2]
@@ -376,6 +379,13 @@ class IngestPlan:
         the device run and the dtype rules of the result, with no DataFrame on either side"""
         # result columns live in one pinned block (fast D2H, no second copy); the frame built over them keeps the block
         # alive and it returns to the pool when the frame is collected
+        for slot, name in self.rounding_maps:
+            a = ins[slot]
+            if (a.astype(np.float32).astype(np.int64) != a).any():
+                raise LoweringError(
+                    f"MapValues {name!r}: its values are not all int32 integers, so it writes float32, and the int32 source "
+                    "holds values float32 cannot represent (beyond 2^24): they would be rounded where they pass through. "
+                    "Map to integers, or cast the column to float32 explicitly")
         specs, extra = self._landing()
         layout, off = [], 0
         for dt in [sp[2] for sp in specs] + [np.dtype(np.int32)] * len(extra):
@@ -399,7 +409,9 @@ class IngestPlan:
             if how == "dt":
                 a = a.view("datetime64[ns]")
             elif isinstance(how, tuple) and how[0] == "map":
-                if how[2] and self.counters[how[1]] == 0:
+                if how[3]:  # int32 words: integer labels keep them, integral float labels make the column float
+                    a = a.astype(np.float64) if not how[2] else (a.astype(np.int64) if reference_dtypes else a)
+                elif how[2] and self.counters[how[1]] == 0:
                     a = a.astype(np.int64 if reference_dtypes else np.int32)  # every row got an integer label
             elif isinstance(how, tuple) and how[0] == "date":
                 if self.counters[how[1]]:
@@ -498,12 +510,23 @@ class IngestPlan:
         if cached is None:
             specs = []
             for name, slot, how in self.out:
-                dt = np.int64 if how == "dt" else (np.float32 if (how == "f32" or (isinstance(how, tuple) and how[0] == "map")) else np.int32)
+                is_f32 = how == "f32" or (isinstance(how, tuple) and how[0] == "map" and not how[3])
+                dt = np.int64 if how == "dt" else (np.float32 if is_f32 else np.int32)
                 specs.append((name, slot, np.dtype(dt)))
             taken = {sp[1] for sp in specs} | {slot + 1 for _n, slot, how in self.out if how == "dt"}  # + second halves
             extra = [s for s in range(self.plan.n_out) if s not in taken]
             cached = self._landing_cache = (specs, extra)
         return cached
+
+
+def _int_labels(labels):
+    return all(isinstance(v, (int, np.integer)) and not isinstance(v, bool) for v in labels)
+
+
+def _int32_words(kind, values):
+    """a map writes int32 words when its source is int32 and every value it maps to is an int32 integer (the rule of
+    b2s_cols_add_range_map / _value_map): a value that passes through then stays exact; otherwise it writes float32"""
+    return kind == I32 and all(float(v).is_integer() and -2**31 <= v <= 2**31 - 1 for v in values)
 
 
 def _same_labels_and_dtypes(df, seen):

@@ -103,7 +103,8 @@ def predict(models, E):
 # ------------------------------------------------------------------------------------------ columnar ingest plan
 def run_column_ops(iplan, df):
     """numpy emulation of columns_kernel over the ops an IngestPlan handed to the C-ABI (mlrun_b200/csrc/b2s_columns.cuh):
-    float32 / int32 words, fp64 compares against fp64 tables, outputs in slot order.  -> (outputs, violations, misses)"""
+    float32 / int32 words, fp64 compares against fp64 tables, maps to float32 (int32 when an int32 column maps to int32
+    integers), outputs in slot order.  -> (outputs, violations, misses)"""
     from mlrun_b200 import _native as nat
 
     src = {}
@@ -152,7 +153,9 @@ def run_column_ops_on_slots(iplan, src):
                     hit |= inr
             n_miss = int((~hit).sum())
             x = val
-            outs.append(val.astype(np.float32))
+            labels = [r[2] for r in arg] if kind == "range" else list(arg.values())
+            int_words = skind == nat.COL_I32 and all(float(v).is_integer() and -2**31 <= v <= 2**31 - 1 for v in labels)
+            outs.append(val.astype(np.int32 if int_words else np.float32))  # int32 words keep int32 values exact
         elif kind == "onehot":
             anyhit = np.zeros(len(x), dtype=bool)
             for c in arg:

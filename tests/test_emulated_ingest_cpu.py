@@ -118,3 +118,49 @@ def test_columnar_sources_give_the_frame_path_results_without_pandas():
         fs.ingest({"id": np.arange(5, dtype=np.int32), "x": np.arange(5, dtype=np.float64)})
     with pytest.raises(ValueError, match="Arrow nulls"):
         fs.ingest(pa.table({"id": pa.array([1, 2], type=pa.int32()), "x": pa.array([1.0, None], type=pa.float32())}))
+
+
+
+@pytest.mark.parametrize("kind", ["value", "range"])
+def test_int32_values_beyond_float32_pass_through_maps_exactly(kind):
+    """a MapValues of an int32 column to int32 integers writes int32 words: values that match nothing keep every digit
+    (float32 would round 16 777 217 to 16 777 216 and INT32_MAX to 2^31).  A map to other values writes float32, and a
+    frame whose int32 source holds a value float32 cannot represent is refused instead of rounded"""
+    import contextlib
+    import io
+
+    import numpy as np
+    import pandas as pd
+
+    from mlrun_b200.feature_store import ingest as bi
+    from mlrun_b200.feature_store import steps as bs
+    from mlrun_b200.lowering import LoweringError
+    from oracle import ingest as oi
+    from oracle import transforms as ot
+
+    big = [16_777_217, -16_777_219, 2**31 - 1, -2**31, 16_777_216, 1, 2, 0]
+    df = pd.DataFrame({"k": np.array(big, dtype=np.int32), "x": np.arange(len(big), dtype=np.float32)})
+
+    def steps(api, labels=(10, 20)):
+        fmap = {"ranges": {labels[0]: [1, 2], labels[1]: [2, 3]}} if kind == "range" else {1: labels[0], 2: labels[1]}
+        return [api.MapValues(mapping={"k": fmap}, with_original_features=True),
+                api.FeaturesetValidator(validators={"k_mapped": api.MinMaxValidator(severity="info", min=-2**31, max=2**24)})]
+
+    plan = bi.lower_steps(steps(bs), df)
+    with contextlib.redirect_stdout(io.StringIO()):
+        got = plan.run(df)
+        want, n_viol = oi.ingest_rows(steps(ot), df)
+    assert got["k_mapped"].dtype == np.int32
+    assert got["k_mapped"].tolist() == want["k_mapped"].tolist() == [16_777_217, -16_777_219, 2**31 - 1, -2**31, 16_777_216, 10, 20, 0]
+    assert plan.unmatched == {"k_mapped": 6} and plan.violations == {"k_mapped": 2} and n_viol == 2
+    pd.testing.assert_frame_equal(got, want, check_dtype=False, check_exact=True)
+
+    halves = bi.lower_steps(steps(bs, (0.5, 20)), df)  # float32 output: the frame above would be rounded
+    with pytest.raises(LoweringError, match="float32 cannot represent"):
+        halves.run(df)
+    small = df[df["k"].abs() <= 2**24].reset_index(drop=True)  # every value float32-exact: served
+    with contextlib.redirect_stdout(io.StringIO()):
+        got = halves.run(small)
+        want, _ = oi.ingest_rows(steps(ot, (0.5, 20)), small)
+    assert got["k_mapped"].dtype == np.float32
+    pd.testing.assert_frame_equal(got, want, check_dtype=False, check_exact=True)
