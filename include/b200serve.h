@@ -459,7 +459,8 @@ typedef struct b2s_pit_col {
  * columns in `cols` and order[q] (the input row at sorted position q; may be NULL) are written in that order; miss[s]
  * counts the rows without a match in set s.  _device: every array is device memory, miss accumulates (zero it first),
  * asynchronous on `stream`.  _host: host arrays; the join runs in row ranges whose results are copied back while the next
- * range is joined; miss is written.  B2S_ERR_INVALID before any launch for a misaligned or null array, an output word
+ * range is joined; miss is written; stats->kernels counts every launch: the sort's 24 (with ts) plus, per range, one join
+ * launch per set, with the entity columns 64 to a launch (max(1, n_sets, ceil(n_cols / 64))).  B2S_ERR_INVALID before any launch for a misaligned or null array, an output word
  * outside the index's rows, or an exact-key join on an index with more than one row per key. */
 int b2s_pit_join_device(const int64_t* d_ts, int64_t n, const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols,
                         int32_t n_cols, int64_t* d_order, uint64_t* d_miss, void* stream);

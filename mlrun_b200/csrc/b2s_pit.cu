@@ -28,6 +28,14 @@
       return b2s_int_fail(B2S_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
   } while (0)
 
+// inside a do { ... } while (0) block whose buffers are freed after it: record the failure in rc and leave the block (from
+// a loop nested in the block it leaves the loop only, which is followed by `if (rc) break;`)
+#define PIT_BREAK(expr)                                                                                                  \
+  if (const cudaError_t _e = (expr); _e != cudaSuccess) {                                                              \
+    rc = b2s_int_fail(B2S_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__);       \
+    break;                                                                                                             \
+  }
+
 using namespace b2s_pit;
 using b2s::TableSlot;
 
@@ -328,43 +336,44 @@ static int index_build(b2s_pit_s* ix, const int64_t* keys, const int64_t* ts, in
   int rc = B2S_OK;
   do {
     if ((rc = alloc_sort(sb, n, st))) break;
-    PIT_TRY(cudaMallocAsync(&d_keys, n * 8, st));
-    PIT_TRY(cudaMallocAsync(&d_ts_in, n * 8, st));
-    PIT_TRY(cudaMallocAsync(&d_stat, 16, st));
-    PIT_TRY(cudaMemsetAsync(d_stat, 0, 16, st));
-    PIT_TRY(cudaMemcpyAsync(d_keys, keys, n * 8, cudaMemcpyHostToDevice, st));
-    PIT_TRY(cudaMemcpyAsync(d_ts_in, ts, n * 8, cudaMemcpyHostToDevice, st));
-    PIT_TRY(cudaMemcpyAsync(sb.k[0], ts, n * 8, cudaMemcpyHostToDevice, st));
+    PIT_BREAK(cudaMallocAsync(&d_keys, n * 8, st));
+    PIT_BREAK(cudaMallocAsync(&d_ts_in, n * 8, st));
+    PIT_BREAK(cudaMallocAsync(&d_stat, 16, st));
+    PIT_BREAK(cudaMemsetAsync(d_stat, 0, 16, st));
+    PIT_BREAK(cudaMemcpyAsync(d_keys, keys, n * 8, cudaMemcpyHostToDevice, st));
+    PIT_BREAK(cudaMemcpyAsync(d_ts_in, ts, n * 8, cudaMemcpyHostToDevice, st));
+    PIT_BREAK(cudaMemcpyAsync(sb.k[0], ts, n * 8, cudaMemcpyHostToDevice, st));
     for (int c = 0; c < n_cols; ++c) {
-      PIT_TRY(cudaMallocAsync(&d_cols[c], (size_t)n * col_bytes[c], st));
-      PIT_TRY(cudaMemcpyAsync(d_cols[c], cols[c], (size_t)n * col_bytes[c], cudaMemcpyHostToDevice, st));
+      PIT_BREAK(cudaMallocAsync(&d_cols[c], (size_t)n * col_bytes[c], st));
+      PIT_BREAK(cudaMemcpyAsync(d_cols[c], cols[c], (size_t)n * col_bytes[c], cudaMemcpyHostToDevice, st));
       lp.cols[c] = d_cols[c];
     }
+    if (rc) break;
     // by timestamp, then (stably) by key: rows ordered by (key, timestamp), equal pairs in input order
     if ((rc = radix_sort(sb, false, n, st))) break;
     const int g = grid_for(n, 256);
     gather_keys_kernel<<<g, 256, 0, st>>>(d_keys, sb.v[0], sb.k[0], n);
     if ((rc = radix_sort(sb, true, n, st))) break;
-    PIT_TRY(cudaMalloc(&ix->d_ts, n * 8));
-    PIT_TRY(cudaMalloc(&ix->d_rows, (size_t)n * std::max(lp.row_words, 1) * 4));
+    PIT_BREAK(cudaMalloc(&ix->d_ts, n * 8));
+    PIT_BREAK(cudaMalloc(&ix->d_rows, (size_t)n * std::max(lp.row_words, 1) * 4));
     gather_keys_kernel<<<g, 256, 0, st>>>(d_ts_in, sb.v[0], reinterpret_cast<uint64_t*>(ix->d_ts), n);
     layout_rows_kernel<<<g, 256, 0, st>>>(lp, sb.v[0], ix->d_rows, n);
     count_runs_kernel<<<g, 256, 0, st>>>(sb.k[0], n, d_stat);
     b2s_int_count_launches(4);
     unsigned long long runs = 0;
-    PIT_TRY(cudaMemcpyAsync(&runs, d_stat, 8, cudaMemcpyDeviceToHost, st));
-    PIT_TRY(cudaStreamSynchronize(st));
+    PIT_BREAK(cudaMemcpyAsync(&runs, d_stat, 8, cudaMemcpyDeviceToHost, st));
+    PIT_BREAK(cudaStreamSynchronize(st));
     uint64_t cap = 16;
     while (cap < runs * 2) cap <<= 1;  // load factor <= 0.5: table_find's walk always meets an empty slot
     ix->cap = cap;
     ix->n_keys = (int64_t)runs;
-    PIT_TRY(cudaMalloc(&ix->d_slots, cap * sizeof(TableSlot)));
-    PIT_TRY(cudaMemsetAsync(ix->d_slots, 0xff, cap * sizeof(TableSlot), st));  // row -1: empty
+    PIT_BREAK(cudaMalloc(&ix->d_slots, cap * sizeof(TableSlot)));
+    PIT_BREAK(cudaMemsetAsync(ix->d_slots, 0xff, cap * sizeof(TableSlot), st));  // row -1: empty
     insert_runs_kernel<<<g, 256, 0, st>>>(sb.k[0], n, ix->d_slots, cap - 1, d_stat + 1);
     b2s_int_count_launches(1);
     unsigned long long longest = 0;
-    PIT_TRY(cudaMemcpyAsync(&longest, d_stat + 1, 8, cudaMemcpyDeviceToHost, st));
-    PIT_TRY(cudaStreamSynchronize(st));
+    PIT_BREAK(cudaMemcpyAsync(&longest, d_stat + 1, 8, cudaMemcpyDeviceToHost, st));
+    PIT_BREAK(cudaStreamSynchronize(st));
     ix->longest_run = (int64_t)longest;
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) rc = b2s_int_fail(B2S_ERR_CUDA, "index build failed: %s", cudaGetErrorString(e));
@@ -443,10 +452,10 @@ static int check_sets(const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col
 }
 
 // sort (when ts is given) and launch the join over sorted positions [q0, q1); sets / cols hold device pointers.  Sets and
-// columns beyond one launch's parameter block go to further launches over the same range.
+// columns beyond one launch's parameter block go to further launches over the same range.  *launches grows by the launches made.
 static int launch_join(const int64_t* d_sorted_ts, const uint32_t* d_order, int64_t* d_order_out, int64_t q0, int64_t q1,
                        const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols, int32_t n_cols, unsigned long long* d_miss,
-                       cudaStream_t st) {
+                       cudaStream_t st, int* launches) {
   int s = 0, c = 0;
   bool first = true;
   while (first || s < n_sets || c < n_cols) {
@@ -483,6 +492,7 @@ static int launch_join(const int64_t* d_sorted_ts, const uint32_t* d_order, int6
     if (q1 > q0) {
       pit_join_kernel<<<grid_for(q1 - q0, 256), 256, 0, st>>>(p);
       b2s_int_count_launches(1);
+      ++*launches;
     }
   }
   const cudaError_t e = cudaGetLastError();
@@ -506,11 +516,11 @@ extern "C" int b2s_pit_join_device(const int64_t* d_ts, int64_t n, const b2s_pit
     PIT_TRY(cudaSetDevice(b2s_int_device()));
     cudaStream_t st = stream ? (cudaStream_t)stream : b2s_int_stream();
     SortBufs sb{};
-    int rc = B2S_OK;
+    int rc = B2S_OK, launches = 0;
     if (d_ts) rc = sort_entities(d_ts, n, sb, st);
     if (!rc)
       rc = launch_join(d_ts ? reinterpret_cast<const int64_t*>(sb.k[0]) : nullptr, d_ts ? sb.v[0] : nullptr, d_order, 0, n, sets, n_sets,
-                       cols, n_cols, reinterpret_cast<unsigned long long*>(d_miss), st);
+                       cols, n_cols, reinterpret_cast<unsigned long long*>(d_miss), st, &launches);
     free_sort(sb, st);
     return rc;
   } catch (const std::exception& e) {
@@ -563,12 +573,14 @@ extern "C" int b2s_pit_join_host(const int64_t* ts, int64_t n, const b2s_pit_set
     cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
     std::vector<cudaEvent_t> range_ev;
     do {
-      for (auto& e : ev) PIT_TRY(cudaEventCreate(&e));
-      PIT_TRY(cudaMallocAsync(&d_block, total, st));
-      PIT_TRY(cudaMemsetAsync(d_block + miss_off, 0, 8 * (size_t)std::max(n_sets, 1), st));
-      PIT_TRY(cudaEventRecord(ev[0], st));
-      for (size_t i = 0; i < ins.size(); ++i) PIT_TRY(cudaMemcpyAsync(d_block + in_off[i], ins[i].first, ins[i].second, cudaMemcpyHostToDevice, st));
-      PIT_TRY(cudaEventRecord(ev[1], st));
+      for (auto& e : ev) PIT_BREAK(cudaEventCreate(&e));
+      if (rc) break;
+      PIT_BREAK(cudaMallocAsync(&d_block, total, st));
+      PIT_BREAK(cudaMemsetAsync(d_block + miss_off, 0, 8 * (size_t)std::max(n_sets, 1), st));
+      PIT_BREAK(cudaEventRecord(ev[0], st));
+      for (size_t i = 0; i < ins.size(); ++i) PIT_BREAK(cudaMemcpyAsync(d_block + in_off[i], ins[i].first, ins[i].second, cudaMemcpyHostToDevice, st));
+      if (rc) break;
+      PIT_BREAK(cudaEventRecord(ev[1], st));
       // the same descriptors over the device mirrors
       size_t ii = ts ? 1 : 0, oi = 0;
       for (int s = 0; s < n_sets; ++s) {
@@ -590,35 +602,38 @@ extern "C" int b2s_pit_join_host(const int64_t* ts, int64_t n, const b2s_pit_set
       const int64_t kRange = 1 << 20;
       const int n_ranges = (int)((n + kRange - 1) / kRange);
       range_ev.assign(n_ranges, nullptr);
-      for (auto& e : range_ev) PIT_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+      for (auto& e : range_ev) PIT_BREAK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+      if (rc) break;
       auto* d_miss = reinterpret_cast<unsigned long long*>(d_block + miss_off);
+      int launches = d_ts ? 24 : 0;  // the entity sort's
       for (int k = 0; k < n_ranges && !rc; ++k) {
         const int64_t q0 = (int64_t)k * kRange, q1 = std::min<int64_t>(n, q0 + kRange);
         rc = launch_join(d_ts ? reinterpret_cast<const int64_t*>(sb.k[0]) : nullptr, d_ts ? sb.v[0] : nullptr, d_order, q0, q1, dsets.data(),
-                         n_sets, dcols.data(), n_cols, d_miss, st);
+                         n_sets, dcols.data(), n_cols, d_miss, st, &launches);
         if (rc) break;
-        PIT_TRY(cudaEventRecord(range_ev[k], st));
-        PIT_TRY(cudaStreamWaitEvent(cs, range_ev[k], 0));
+        PIT_BREAK(cudaEventRecord(range_ev[k], st));
+        PIT_BREAK(cudaStreamWaitEvent(cs, range_ev[k], 0));
         for (size_t i = 0; i < outs.size(); ++i) {
           const size_t el = outs[i].second;
-          PIT_TRY(cudaMemcpyAsync(static_cast<char*>(outs[i].first) + q0 * el, d_block + out_off[i] + q0 * el, (size_t)(q1 - q0) * el,
-                                  cudaMemcpyDeviceToHost, cs));
+          PIT_BREAK(cudaMemcpyAsync(static_cast<char*>(outs[i].first) + q0 * el, d_block + out_off[i] + q0 * el, (size_t)(q1 - q0) * el,
+                                    cudaMemcpyDeviceToHost, cs));
         }
       }
       if (rc) break;
-      PIT_TRY(cudaEventRecord(ev[2], st));
-      if (n_sets) PIT_TRY(cudaMemcpyAsync(miss, d_miss, 8 * (size_t)n_sets, cudaMemcpyDeviceToHost, cs));
-      PIT_TRY(cudaStreamSynchronize(cs));
-      PIT_TRY(cudaStreamSynchronize(st));
+      PIT_BREAK(cudaEventRecord(ev[2], st));
+      if (n_sets) PIT_BREAK(cudaMemcpyAsync(miss, d_miss, 8 * (size_t)n_sets, cudaMemcpyDeviceToHost, cs));
+      PIT_BREAK(cudaStreamSynchronize(cs));
+      PIT_BREAK(cudaStreamSynchronize(st));
       if (stats) {
         memset(stats, 0, sizeof(*stats));
         stats->rows = n;
         cudaEventElapsedTime(&stats->h2d_ms, ev[0], ev[1]);
         cudaEventElapsedTime(&stats->kernel_ms, ev[1], ev[2]);  // sort + join (the copies back overlap the join)
-        stats->kernels = n_ranges;
+        stats->kernels = launches;
       }
     } while (0);
     free_sort(sb, st);
+    cudaStreamSynchronize(cs);  // after a failure, copies back queued on cs may still read d_block
     if (d_block) cudaFreeAsync(d_block, st);
     cudaStreamSynchronize(st);
     for (auto& e : ev)

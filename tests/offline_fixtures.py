@@ -40,8 +40,9 @@ def _key_columns(kind, names, chosen):
 
 
 def workload(seed, n_sets=2, n_rows=200, n_keys=16, n_entity=120, key_kind="int64", unit="ns", exact_sets=(), unknown=0.2,
-             before_1970=True, ties=False, n_float=3, ints=True):
-    """-> (featuresets, {name: (entities, ts, frame)}, features, entity frame, entity timestamp column)"""
+             before_1970=True, ties=False, n_float=3, ints=True, dates=()):
+    """-> (featuresets, {name: (entities, ts, frame)}, features, entity frame, entity timestamp column); `dates`: units of
+    datetime64 feature columns to add to every set (values before and after 1970, a tenth of them NaT)"""
     rng = np.random.default_rng(seed)
     span = (-(10**12) if before_1970 else 10**12, 3 * 10**12)
     f = {"s": 10**9, "ms": 10**6, "us": 10**3, "ns": 1}[unit]
@@ -69,11 +70,16 @@ def workload(seed, n_sets=2, n_rows=200, n_keys=16, n_entity=120, key_kind="int6
             cols[f"s{s}count"] = rng.integers(-1000, 1000, size=rows).astype(np.int32)
             cols[f"s{s}small"] = rng.integers(-100, 100, size=rows).astype(np.int8)
             cols[f"s{s}flag"] = rng.random(rows) < 0.5
+        for u in dates:
+            d = rng.integers(-(10**9), 4 * 10**9, size=rows) * (10**9 // {"s": 10**9, "ms": 10**6, "us": 10**3, "ns": 1}[u])
+            d[rng.random(rows) < 0.1] = np.iinfo(np.int64).min
+            cols[f"s{s}d{u}"] = d.view(f"datetime64[{u}]")
         frame = pd.DataFrame(cols)
         fs = bingest.FeatureSet(name, entities=names, timestamp_key=ts)
         fsets.append(fs)
         frames[name] = (names, ts, frame)
         picked = [f"s{s}x{j}" for j in range(1, n_float)] + ([f"s{s}count", f"s{s}small", f"s{s}flag"] if ints else [])
+        picked += [f"s{s}d{u}" for u in dates]
         features += [f"{name}.s{s}x0 as first{s}"] + [f"{name}.{c}" for c in picked] if s % 2 == 0 else [f"{name}.*"]
     # entity rows: known keys, unknown keys, times before / between / after the feature rows
     n_unknown = int(n_entity * unknown)
