@@ -467,6 +467,53 @@ int b2s_pit_join_device(const int64_t* d_ts, int64_t n, const b2s_pit_set* sets,
 int b2s_pit_join_host(const int64_t* ts, int64_t n, const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols,
                       int32_t n_cols, int64_t* order, uint64_t* miss, b2s_stats* stats);
 
+/* ---- windowed aggregations at feature-set ingest ------------------------------------------------------------------
+ * storey.AggregateByKey as FeatureSet.add_aggregation places it in a feature set's graph (feature_store/feature_set.py:
+ * 715-851), emitting every event: row i gains, per (operation, window), the aggregate over the rows j <= i (input order)
+ * of its 64-bit key whose timestamps lie in row i's window.  Windows are aligned to the epoch (floor division, so that
+ * rows before 1970 are right): sliding (period_ns > 0, dividing every window): b(t) = floor(t / period), row j is in
+ * when b(t_j) >= b(t_i) - window / period + 1; fixed (period_ns = 0): floor(t_j / window) == floor(t_i / window).
+ * Sums accumulate in fp64 over the window's rows alone (a range reduce, never a difference of running sums); stdvar is
+ * the sample variance from a pairwise (count, mean, M2) combine, NaN for a window of one row; first is the window's
+ * earliest row in input order, last the row itself.  Every output is [n] float64 in input order. */
+#define B2S_AGG_COUNT 1
+#define B2S_AGG_SUM 2
+#define B2S_AGG_SQR 4      /* sum of squares */
+#define B2S_AGG_MAX 8
+#define B2S_AGG_MIN 16
+#define B2S_AGG_FIRST 32
+#define B2S_AGG_LAST 64
+#define B2S_AGG_AVG 128
+#define B2S_AGG_STDVAR 256
+#define B2S_AGG_STDDEV 512
+typedef struct b2s_agg_spec {
+  const void* src;           /* [n] source column in input order, 4-byte words */
+  int32_t kind;              /* B2S_COL_F32 or B2S_COL_I32 (both widen exactly to fp64) */
+  uint32_t ops;              /* B2S_AGG_* bits */
+  int64_t period_ns;         /* sliding period; 0: fixed windows */
+  int32_t n_windows;         /* 1 .. 16 */
+  const int64_t* windows_ns; /* host array [n_windows] */
+  double* const* outs;       /* host array [popcount(ops) * n_windows]: ops in bit order, windows inner; each [n] float64 */
+} b2s_agg_spec;
+/* n rows: keys and int64 nanosecond timestamps in input order; 1 .. 64 aggregations over at most 16 distinct source
+ * columns.  counters[3] count what the semantics refuse, for the caller to raise on: [0] rows whose timestamp is below the
+ * previous row of their key (late events), [1] NaT (INT64_MIN) rows, [2] NaN source values; the outputs of such a run
+ * are unspecified.  _device: every array is device memory, counters accumulate (zero them first), asynchronous on
+ * `stream`.  _host: host arrays (pinned ones copy at full speed, pageable ones are staged by the driver), counters are
+ * written; stats->h2d_ms is the copy in, kernel_ms the sort plus the aggregation, kernels every launch: the sort's 24,
+ * one prep launch, one per level of each column's range structure (levels with more than 32 elements: about
+ * log32(n) of them; none for a column whose aggregations are only count / first / last) and one per aggregation.
+ * B2S_ERR_INVALID before any launch for a null or misaligned pointer (keys, timestamps, outputs and counters 8 bytes,
+ * sources 4), n >= 2^32 (the sort's 32-bit payload), a period that does not divide a window, a window <= 0, an empty or
+ * unknown op mask, or a kind other than F32 / I32. */
+int b2s_agg_run_device(const int64_t* d_keys, const int64_t* d_ts, int64_t n, const b2s_agg_spec* specs, int32_t n_specs,
+                       uint64_t* d_counters, void* stream);
+int b2s_agg_run_host(const int64_t* keys, const int64_t* ts, int64_t n, const b2s_agg_spec* specs, int32_t n_specs,
+                     uint64_t* counters, b2s_stats* stats);
+/* n_iters device runs on the library stream, CUDA-event timed: the sort alone and the whole run (ms summed over the runs) */
+int b2s_agg_time_device(const int64_t* d_keys, const int64_t* d_ts, int64_t n, const b2s_agg_spec* specs, int32_t n_specs,
+                        uint64_t* d_counters, int32_t n_iters, float* sort_ms, float* total_ms);
+
 #ifdef __cplusplus
 }
 #endif

@@ -70,6 +70,15 @@ class PitSet(C.Structure):
 class PitCol(C.Structure):
     _fields_ = [("src", _vp), ("dst", _vp), ("bytes", _i32)]
 
+
+# B2S_AGG_* operation bits, in the order of the outputs of one aggregation
+AGG_OPS = {"count": 1, "sum": 2, "sqr": 4, "max": 8, "min": 16, "first": 32, "last": 64, "avg": 128, "stdvar": 256, "stddev": 512}
+
+
+class AggSpec(C.Structure):
+    _fields_ = [("src", _vp), ("kind", _i32), ("ops", C.c_uint32), ("period_ns", _i64), ("n_windows", _i32),
+                ("windows_ns", C.POINTER(_i64)), ("outs", C.POINTER(_vp))]
+
 # name -> (restype, argtypes); the single source of truth for the exported surface
 SIGNATURES = {
     "b2s_version": (C.c_int, []),
@@ -156,6 +165,10 @@ SIGNATURES = {
     "b2s_pit_index_info": (C.c_int, [_vp, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_i64), _pi32, C.POINTER(_i64)]),
     "b2s_pit_join_device": (C.c_int, [_vp, _i64, C.POINTER(PitSet), _i32, C.POINTER(PitCol), _i32, _vp, _vp, _vp]),
     "b2s_pit_join_host": (C.c_int, [_vp, _i64, C.POINTER(PitSet), _i32, C.POINTER(PitCol), _i32, _vp, _vp, C.POINTER(Stats)]),
+    # windowed aggregations
+    "b2s_agg_run_device": (C.c_int, [_vp, _vp, _i64, C.POINTER(AggSpec), _i32, _vp, _vp]),
+    "b2s_agg_run_host": (C.c_int, [_vp, _vp, _i64, C.POINTER(AggSpec), _i32, _vp, C.POINTER(Stats)]),
+    "b2s_agg_time_device": (C.c_int, [_vp, _vp, _i64, C.POINTER(AggSpec), _i32, _vp, _i32, _pf32, _pf32]),
     # body codec
     "b2s_json_parse_inputs": (C.c_int, [C.c_char_p, _i64, _pf32, _i64, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_i64),
                                         C.POINTER(_i64)]),

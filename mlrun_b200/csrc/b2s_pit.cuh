@@ -7,20 +7,6 @@
 
 namespace b2s_pit {
 
-// LSD radix sort of 64-bit keys with a 32-bit payload: 8 passes of 8-bit digits, each pass histogram -> scan -> stable scatter.
-// A block sorts a tile of kSortThreads * kSortItems keys; element e of the tile is item e / kSortThreads of thread
-// e % kSortThreads, so ranking items in (item, warp, lane) order is ranking them in input order (stability).
-constexpr int kSortThreads = 256;
-constexpr int kSortItems = 16;
-constexpr int kSortTile = kSortThreads * kSortItems;
-constexpr int kSortWarps = kSortThreads / 32;
-constexpr int kScanThreads = 1024;
-
-// signed order: flipping the sign bit maps INT64_MIN..INT64_MAX onto 0..UINT64_MAX monotonically
-__host__ __device__ inline uint32_t radix_digit(uint64_t key, int shift) {
-  return (uint32_t)(((key ^ 0x8000000000000000ull) >> shift) & 0xffu);
-}
-
 // per launch: feature sets, their output columns, and entity columns permuted into sorted order (more are split over launches).
 // One feature set per launch: on the H100, 4 sets x 32 features over 4 Mi entity rows joined in 7.6 ms as four launches
 // against 9.5 ms as one launch looping over the sets (DESIGN.md §4g).

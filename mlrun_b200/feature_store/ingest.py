@@ -8,11 +8,17 @@ datastore/targets.py:1856-1868).  Here the steps are walked symbolically over th
 (`FrameProgram`, same per-row semantics) and lowered to ONE columnar device plan (`mlrun_b200.columns`); the frame's
 columns go to the GPU as they are (contiguous typed arrays) and the result columns come back the same way.
 
+`FeatureSet.add_aggregation` (storey.AggregateByKey, emitting every event) runs after the columns plan as one more device
+call over the keyed, timestamped result columns (`AggregationPlan`, b2s_agg_run_host): float64 columns land in the same
+result block.
+
 Out of scope (control plane / storage): targets, feature-set metadata / stats inference, sources other than a
 DataFrame.  Steps or dtypes the device cannot hold raise `LoweringError`: there is no per-row Python fallback.
 """
 
+import ctypes as C
 import math
+import re
 
 import numpy as np
 
@@ -319,6 +325,7 @@ class IngestPlan:
         self.violations = {}
         self.unmatched = {}
         self.stats = None
+        self.agg = None  # AggregationPlan of the graph's aggregation step, if it has one
 
     @property
     def out_names(self):
@@ -360,9 +367,10 @@ class IngestPlan:
                 out[name] = block[:, j]
         return out
 
-    def run(self, df, reference_dtypes=False):
+    def run(self, df, reference_dtypes=False, keys=None):
         """transform the frame; returns a new DataFrame with the same index.  `reference_dtypes=True` widens integer
-        results to int64 (what a frame re-assembled from Python ints has) at the price of a host-side copy."""
+        results to int64 (what a frame re-assembled from Python ints has) at the price of a host-side copy.  `keys`: the
+        rows' encoded entity keys (int64), which a plan with an aggregation needs."""
         import pandas as pd
 
         if not _same_labels_and_dtypes(df, getattr(self, "_seen", None)):  # a frame like one already checked skips the walk
@@ -371,12 +379,14 @@ class IngestPlan:
             self._seen = (df.columns, list(df.dtypes))
         n = len(df)
         ins, _keep = self._inputs(df)
-        data, bufs, block, layout = self._run_arrays(ins, n, reference_dtypes)
+        data, bufs, block, layout = self._run_arrays(ins, n, reference_dtypes, keys)
         return self._assemble(data, bufs, block, layout, n, df.index)
 
-    def _run_arrays(self, ins, n, reference_dtypes=False):
+    def _run_arrays(self, ins, n, reference_dtypes=False, keys=None):
         """{input slot: contiguous column array} -> ({result column: array}, landing views, their pinned block, offsets):
         the device run and the dtype rules of the result, with no DataFrame on either side"""
+        if self.agg is not None and (keys is None or len(keys) != n):
+            raise ValueError("a plan with an aggregation needs the encoded entity key of every row")
         # result columns live in one pinned block (fast D2H, no second copy); the frame built over them keeps the block
         # alive and it returns to the pool when the frame is collected
         for slot, name in self.rounding_maps:
@@ -387,8 +397,9 @@ class IngestPlan:
                     "holds values float32 cannot represent (beyond 2^24): they would be rounded where they pass through. "
                     "Map to integers, or cast the column to float32 explicitly")
         specs, extra = self._landing()
+        agg_names = self.agg.out_names if self.agg is not None else []
         layout, off = [], 0
-        for dt in [sp[2] for sp in specs] + [np.dtype(np.int32)] * len(extra):
+        for dt in [sp[2] for sp in specs] + [np.dtype(np.int32)] * len(extra) + [np.dtype(np.float64)] * len(agg_names):
             layout.append(off)
             off += (n * dt.itemsize + 63) // 64 * 64
         block = nat.PINNED.take(off) if n else None
@@ -403,6 +414,10 @@ class IngestPlan:
         for j, s_ in enumerate(extra):
             outs[s_] = column(len(specs) + j, np.dtype(np.int32))
         self.counters, self.stats = self.plan.run_host(ins, n, outs, with_stats=True)
+        if self.agg is not None:  # cross-row: the whole frame in one call, over the result columns just landed
+            for j, name in enumerate(agg_names):
+                bufs[name] = column(len(specs) + len(extra) + j, np.dtype(np.float64))
+            self.agg.run(keys, ins[self.agg.ts_slot], {c: bufs[c] for c in self.agg.sources}, n, bufs)
         data = {}
         for name, _slot, how in self.out:
             a = bufs[name]
@@ -423,6 +438,8 @@ class IngestPlan:
             elif how == "i32" and reference_dtypes:
                 a = a.astype(np.int64)
             data[name] = a
+        for name in agg_names:
+            data[name] = bufs[name]
         self.violations = {name: int(self.counters[cnt]) for cnt, name, _v in self.checks}
         self.unmatched = {name: int(self.counters[cnt]) for cnt, name, _w in self.miss if self.counters[cnt]}
         for cnt, name, v in self.checks:
@@ -433,7 +450,7 @@ class IngestPlan:
                 int(self.counters[cnt]) for cnt, name, v in self.checks if v in step._validators.values())
         return data, bufs, block, layout
 
-    def run_columns(self, columns, reference_dtypes=False):
+    def run_columns(self, columns, reference_dtypes=False, keys=None):
         """columnar twin of `run` (SURVEY 8(f) #1: "Arrow/DLPack in, Arrow/Parquet-ready columns out"): `columns` maps every
         schema column to a contiguous 1-D array of its dtype (numpy, or anything `columnar.as_columns` understands: Arrow
         tables / record batches, DLPack producers); returns a `columnar.ColumnBatch` whose arrays live in one pinned block.
@@ -461,7 +478,7 @@ class IngestPlan:
             elif len(a) != n:
                 raise ValueError("columns of different lengths")
             ins[self.prog.in_slot[name]] = a
-        data, _bufs, block, _layout = self._run_arrays(ins, n or 0, reference_dtypes)
+        data, _bufs, block, _layout = self._run_arrays(ins, n or 0, reference_dtypes, keys)
         return columnar.ColumnBatch(data, n or 0, block)
 
     def _assemble(self, data, bufs, block, layout, n, index):
@@ -535,6 +552,141 @@ def _same_labels_and_dtypes(df, seen):
     return seen is not None and df.columns.equals(seen[0]) and list(df.dtypes) == seen[1]
 
 
+# ------------------------------------------------------------------------------------------ windowed aggregations
+AGGREGATES_STEP = "Aggregates"  # feature_set.py:55 aggregates_step, the default step name
+_DURATION_NS = {"s": 10**9, "m": 60 * 10**9, "h": 3600 * 10**9, "d": 86400 * 10**9}
+_MAX_WINDOWS, _MAX_SPECS, _MAX_SOURCES = 16, 64, 16  # b2s_agg_run_host's limits
+
+
+def _duration_ns(text, what):
+    """'10m' -> nanoseconds; units s / m / h / d"""
+    m = re.fullmatch(r"\s*(\d+)\s*([A-Za-z]+)\s*", str(text))
+    if not m or m.group(2) not in _DURATION_NS:
+        raise LoweringError(f"{what} {text!r}: windows and periods are <count><unit> with unit s, m, h or d")
+    ns = int(m.group(1)) * _DURATION_NS[m.group(2)]
+    if not 0 < ns < 2**63:
+        raise LoweringError(f"{what} {text!r} is empty or beyond the int64 nanosecond range")
+    return ns
+
+
+class AggregateByKey:
+    """storey.AggregateByKey as FeatureSet.add_aggregation places it in the graph: its class arguments only.  It is never
+    run per event; `AggregationPlan` lowers it to one device call over the whole frame."""
+
+    def __init__(self, aggregates=None, table=None, time_field=None, emit_policy=None, key_field=None, **kwargs):
+        self.aggregates = [dict(a) for a in aggregates or []]
+        self.table, self.time_field, self.emit_policy, self.key_field = table, time_field, emit_policy, key_field
+        self.name = kwargs.get("name")
+
+    def do(self, event):
+        raise LoweringError("AggregateByKey runs on the device over a whole frame (FeatureSet.ingest), not per event")
+
+
+class _AggSpec:
+    __slots__ = ("column", "kind", "ops", "period_ns", "windows_ns", "outs")
+
+    def __init__(self, column, kind, ops, period_ns, windows_ns, outs):
+        self.column, self.kind, self.ops, self.period_ns, self.windows_ns = column, kind, ops, period_ns, windows_ns
+        self.outs = outs  # output column names in the C-ABI's order: op bits ascending, windows inner
+
+
+class AggregationPlan:
+    """an AggregateByKey step over the result columns of an IngestPlan (emit every event).  Everything the device does not
+    compute is refused here, before any copy: no timestamp key or entities, sources that are not float32 / int32 result
+    columns, unknown operations or units, a period that does not divide a window, another emit policy."""
+
+    def __init__(self, step, plan, timestamp_key, entities):
+        if not timestamp_key:
+            raise LoweringError("an aggregation needs the feature set's timestamp_key: windows are event-time windows")
+        if not entities:
+            raise LoweringError("an aggregation needs the feature set's entities: it aggregates per key")
+        ep = step.emit_policy
+        if ep is not None and type(ep).__name__ != "EmitEveryEvent" and not (isinstance(ep, dict) and ep.get("mode") == "every_event"):
+            raise LoweringError(f"emit policy {ep!r}: only EmitEveryEvent (the storey default) is lowered")
+        if step.time_field not in (None, timestamp_key):
+            raise LoweringError(f"aggregation time field {step.time_field!r} is not the feature set's timestamp_key")
+        if dict(plan.schema).get(timestamp_key) != I64:
+            raise LoweringError(f"timestamp_key {timestamp_key!r} must be a datetime64 column of the ingested frame")
+        self.ts_slot = plan.prog.in_slot[timestamp_key]
+        landing = {name: dt for name, _slot, dt in plan._landing()[0]}
+        how = {name: h for name, _slot, h in plan.out}
+        self.specs, self.out_names, self.sources = [], [], []
+        for agg in step.aggregates:
+            col = agg.get("column")
+            if col in entities or col == timestamp_key:
+                raise LoweringError(f"aggregation of {col!r}: entities and the timestamp are not aggregated")
+            dt = landing.get(col)
+            if dt is None or isinstance(how[col], tuple) and how[col][0] == "date" or dt not in (np.float32, np.int32):
+                raise LoweringError(f"aggregation of {col!r}: the source must be a float32 or int32 result column of the graph")
+            ops = list(dict.fromkeys(agg.get("operations") or []))
+            bad = [o for o in ops if o not in nat.AGG_OPS]
+            if not ops or bad:
+                raise LoweringError(f"aggregation {agg.get('name')!r}: operations {bad or ops} (have {list(nat.AGG_OPS)})")
+            windows = list(dict.fromkeys(agg.get("windows") or []))
+            if not windows or len(windows) > _MAX_WINDOWS:
+                raise LoweringError(f"aggregation {agg.get('name')!r}: 1 .. {_MAX_WINDOWS} windows")
+            windows_ns = [_duration_ns(w, "window") for w in windows]
+            period_ns = _duration_ns(agg["period"], "period") if agg.get("period") else 0
+            if period_ns and any(w % period_ns for w in windows_ns):
+                raise LoweringError(f"aggregation {agg.get('name')!r}: period {agg['period']} must divide every window {windows}")
+            names = {(o, w): f"{agg['name']}_{o}_{w}" for o in ops for w in windows}
+            self.out_names += [names[o, w] for o in ops for w in windows]  # feature_set.py:847-849
+            by_bit = sorted(ops, key=nat.AGG_OPS.get)
+            self.specs.append(_AggSpec(col, nat.COL_F32 if dt == np.float32 else nat.COL_I32, sum(nat.AGG_OPS[o] for o in ops),
+                                       period_ns, windows_ns, [names[o, w] for o in by_bit for w in windows]))
+            if col not in self.sources:
+                self.sources.append(col)
+        if len(self.specs) > _MAX_SPECS or len(self.sources) > _MAX_SOURCES:
+            raise LoweringError(f"at most {_MAX_SPECS} aggregations over {_MAX_SOURCES} columns per feature set")
+        taken = set(how)
+        for name in self.out_names:
+            if name in taken:
+                raise LoweringError(f"aggregate column {name!r} collides with another column of the result")
+            taken.add(name)
+        self.counters = None
+        self.stats = None
+
+    def run(self, keys, ts, sources, n, outs):
+        """keys / ts: int64 [n]; sources: {column: float32 / int32 [n]}; outs: {aggregate column: float64 [n]} (filled).
+        Raises LoweringError after the run for late events, NaT timestamps or NaN values."""
+        specs = [(sources[sp.column], sp.kind, sp.ops, sp.period_ns, sp.windows_ns, [outs[o] for o in sp.outs]) for sp in self.specs]
+        self.counters, self.stats = aggregate_host(keys, ts, specs, n)
+        late, nat_rows, nans = (int(c) for c in self.counters)
+        if late:
+            raise LoweringError(f"{late} rows have a timestamp below the previous row of their key: late and out-of-order events "
+                                "are not aggregated on the device (sort each key's rows by time)")
+        if nat_rows:
+            raise LoweringError(f"{nat_rows} rows have a NaT timestamp: they belong to no window")
+        if nans:
+            raise LoweringError(f"{nans} aggregated values are NaN: impute them before the aggregation")
+
+
+def aggregate_host(keys, ts, specs, n):
+    """one b2s_agg_run_host call.  specs: [(source [n] float32 / int32, COL_* kind, op bits, period ns, [window ns],
+    [float64 [n] output per (op bit ascending, window)])] -> (counters uint64 [3], stats dict)"""
+    lib = nat.init() if n else nat.load()
+    keys = np.ascontiguousarray(keys, dtype=np.int64)
+    ts = np.ascontiguousarray(ts, dtype=np.int64)
+    c_specs = (nat.AggSpec * len(specs))()
+    keep = []
+    for i, (src, kind, ops, period_ns, windows_ns, arrays) in enumerate(specs):
+        src = np.ascontiguousarray(src)
+        win = np.ascontiguousarray(windows_ns, dtype=np.int64)
+        ptrs = (C.c_void_p * len(arrays))(*[a.ctypes.data for a in arrays])
+        keep += [src, win, ptrs]
+        c_specs[i] = nat.AggSpec(src.ctypes.data, kind, ops, period_ns, len(win), win.ctypes.data_as(C.POINTER(C.c_int64)), ptrs)
+    counters = np.zeros(3, dtype=np.uint64)
+    stats = nat.Stats()
+    nat.check(lib.b2s_agg_run_host(keys.ctypes.data, ts.ctypes.data, n, c_specs, len(specs), counters.ctypes.data, C.byref(stats)))
+    return counters, stats.as_dict()
+
+
+def _aggregation_key(graph):
+    """what of the graph's aggregation steps a cached plan depends on"""
+    return repr([(name, step.class_args) for name, step in graph.steps.items()
+                 if str(getattr(step, "class_name", "") or "") == "storey.AggregateByKey"])
+
+
 def lower_steps(steps, df_or_schema):
     schema = df_or_schema if isinstance(df_or_schema, list) else frame_schema(df_or_schema)
     prog = FrameProgram(schema)
@@ -556,6 +708,7 @@ class Feature:
                  default=None, labels=None):
         self.name, self.value_type, self.description, self.validator = name or "", value_type, description, validator
         self.default, self.labels = default, labels or {}
+        self.aggregate = aggregate
 
 
 class FeatureSet:
@@ -575,6 +728,7 @@ class FeatureSet:
         self.label_column = label_column
         self.passthrough = passthrough
         self.features = {}
+        self._aggregations = {}
         self._graph = RootFlowStep()
         self._graph.engine = "sync"  # steps are only resolved here; the device plan replaces the executor
         self._plan = None
@@ -631,12 +785,111 @@ class FeatureSet:
                 args = {k: getattr(obj, k) for k in ("mapping", "features") if hasattr(obj, k)}
             check(self, **args)
 
+    def _add_aggregation_to_existing(self, new_aggregation):
+        """feature_set.py:689-713"""
+        name = new_aggregation["name"]
+        if name in self._aggregations:
+            current_aggr = self._aggregations[name]
+            if current_aggr["windows"] != new_aggregation["windows"]:
+                raise MLRunInvalidArgumentError(
+                    f"Aggregation with name {name} already exists but with window {current_aggr['windows']}. "
+                    f"Please provide name for the aggregation")
+            if current_aggr["period"] != new_aggregation["period"]:
+                raise MLRunInvalidArgumentError(
+                    f"Aggregation with name {name} already exists but with period {current_aggr['period']}. "
+                    f"Please provide name for the aggregation")
+            if current_aggr["column"] != new_aggregation["column"]:
+                raise MLRunInvalidArgumentError(
+                    f"Aggregation with name {name} already exists but for different column {current_aggr['column']}. "
+                    f"Please provide name for the aggregation")
+            # the reference takes list(set(...)), whose order varies between processes: the same operations, first-seen order
+            current_aggr["operations"] = list(dict.fromkeys(current_aggr["operations"] + new_aggregation["operations"]))
+            return
+        self._aggregations[name] = new_aggregation
+
+    def add_aggregation(self, column, operations, windows, period=None, name=None, step_name=None, after=None, before=None,
+                        emit_policy=None):
+        """feature_set.py:715-851 -- `fset.add_aggregation("ask", ["sum", "max"], "1h", "10m", name="asks")`: a
+        storey.AggregateByKey step whose columns `{name}_{operation}_{window}` are computed on the device at ingest"""
+        if isinstance(operations, str):
+            raise MLRunInvalidArgumentError("Invalid parameters provided - operations must be a list.")
+        name = name or column
+        if isinstance(windows, str):
+            windows = [windows]
+        # FeatureAggregation(...).to_dict(): fields that are None are left out
+        aggregation = {k: v for k, v in (("name", name), ("column", column), ("operations", list(operations)),
+                                         ("windows", windows), ("period", period)) if v is not None}
+
+        def upsert_feature(feature_name):
+            if feature_name in self.features:
+                self.features[feature_name].aggregate = True
+            else:
+                self.add_feature(Feature(name=column, aggregate=True, value_type="float"), feature_name)  # named by its key
+
+        step_name = step_name or AGGREGATES_STEP
+        graph = self._graph
+        if step_name in graph.steps:
+            step = graph.steps[step_name]
+            self._add_aggregation_to_existing(aggregation)
+            step.class_args["aggregates"] = list(self._aggregations.values())
+            if emit_policy is not None:
+                step.class_args["emit_policy"] = emit_policy
+        else:
+            self._aggregations[aggregation["name"]] = aggregation
+            if before is None and after is None:
+                after = "$prev"
+            if self.engine and self.engine != "storey":
+                raise LoweringError(f"aggregations of the {self.engine} engine are not lowered: use the storey engine")
+            # the reference's storey step takes no emit policy (EmitEveryEvent is storey's default); one given here is kept
+            # so that the lowering can refuse any other
+            extra = {"emit_policy": emit_policy} if emit_policy is not None else {}
+            step = graph.add_step(name=step_name, after=after, before=before, class_name="storey.AggregateByKey",
+                                  time_field=self.timestamp_key, aggregates=[aggregation], table=".", **extra)
+        for operation in operations:
+            for window in windows:
+                upsert_feature(f"{name}_{operation}_{window}")
+        return step
+
+    def _split_aggregation(self, objs):
+        """the graph's objects -> (the steps of the columns plan, the AggregateByKey step or None)"""
+        at = [i for i, o in enumerate(objs) if isinstance(o, AggregateByKey)]
+        if not at:
+            return objs, None
+        if len(at) > 1:
+            raise LoweringError("a second aggregation step is not lowered: add every aggregation to one step")
+        if at[0] != len(objs) - 1:
+            raise LoweringError(f"step {type(objs[at[0] + 1]).__name__} after the aggregation step is not lowered: the "
+                                "aggregation must be the graph's last step")
+        return objs[:-1], objs[-1]
+
+    def _lower(self, namespace, df_or_schema):
+        objs, agg = self._split_aggregation(self._step_objects(namespace))
+        plan = lower_steps(objs, df_or_schema)
+        if agg is not None:
+            plan.agg = AggregationPlan(agg, plan, self.timestamp_key, [e.name for e in self.entities])
+        return plan
+
+    def _encoded_keys(self, frame):
+        """the rows' 64-bit entity keys, as the point-in-time join encodes them (keys.py)"""
+        from .keys import _encode_keys, _key_kind
+
+        names = [e.name for e in self.entities]
+        if frame is None or not all(k in frame.columns for k in names):
+            raise LoweringError(f"the aggregation's entity columns {names} must all be in the ingested data")
+        what = f"feature set {self.name}"
+        kind = _key_kind(frame, names, what)
+        keys = _encode_keys(frame, names, kind, what)
+        if kind == "str" and len(np.unique(keys)) != len(set(frame[names[0]].to_numpy().tolist())):
+            raise MLRunInvalidArgumentError(f"feature set {self.name}: two entity keys share a 64-bit hash")
+        return keys
+
     def _step_objects(self, namespace):
         from ..serving.compiler import _chain, _transform_object
         from ..serving.host import create_graph_server
         from . import transforms
 
         ns = {k: getattr(transforms, k) for k in dir(transforms) if not k.startswith("_")}
+        ns["storey.AggregateByKey"] = AggregateByKey
         ns.update(namespace or {})
         server = create_graph_server(graph=self._graph, parameters={})
         server.init_states(context=None, namespace=ns)
@@ -662,24 +915,35 @@ class FeatureSet:
             keys = [e.name for e in self.entities if e.name in cols]
             carried = {k: cols.pop(k) for k in keys}
             schema = columnar.schema_of(cols)
-            if self._plan is None or self._plan_key != ("columns", schema):
+            key = ("columns", schema, _aggregation_key(self._graph))
+            if self._plan is None or not isinstance(self._plan_key[0], str) or self._plan_key != key:
                 self.validate_steps(namespace)
-                self._plan = lower_steps(self._step_objects(namespace), schema)
-                self._plan_key = ("columns", schema)
-            batch = self._plan.run_columns(cols, reference_dtypes=reference_dtypes)
+                self._plan = self._lower(namespace, schema)
+                self._plan_key = key
+            enc = None
+            if self._plan.agg is not None:
+                import pandas as pd
+
+                enc = self._encoded_keys(pd.DataFrame(carried, copy=False) if carried else None)
+            batch = self._plan.run_columns(cols, reference_dtypes=reference_dtypes, keys=enc)
             batch.index = carried
             return batch if return_df else None
         if not (hasattr(source, "columns") and hasattr(source, "index")):
             raise MLRunInvalidArgumentError("illegal source")  # ingestion.py:77-78; only frames are taken here
         df = source
         keys = [e.name for e in self.entities]
+        key_frame = None
         if keys and all(k in df.columns for k in keys):
+            key_frame = df
             df = df.set_index(keys)
-        if self._plan is None or isinstance(self._plan_key[0], str) or not _same_labels_and_dtypes(df, self._plan_key):
+        agg_key = _aggregation_key(self._graph)
+        if (self._plan is None or isinstance(self._plan_key[0], str) or not _same_labels_and_dtypes(df, self._plan_key)
+                or self._plan_key[2] != agg_key):
             self.validate_steps(namespace)
-            self._plan = lower_steps(self._step_objects(namespace), df)
-            self._plan_key = (df.columns, list(df.dtypes))
-        out = self._plan.run(df, reference_dtypes=reference_dtypes)
+            self._plan = self._lower(namespace, df)
+            self._plan_key = (df.columns, list(df.dtypes), agg_key)
+        enc = self._encoded_keys(key_frame) if self._plan.agg is not None else None
+        out = self._plan.run(df, reference_dtypes=reference_dtypes, keys=enc)
         return out if return_df else None
 
     @property
