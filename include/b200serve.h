@@ -185,8 +185,8 @@ const char* b2s_plan_kernel(b2s_plan_t plan);
 #define B2S_KERNEL_DENSE 1             /* dense_head_kernel (wgmma tf32, TMA tensor-map loads)            */
 #define B2S_KERNEL_TREES3_TMAP 2       /* t3_prep_kernel with TMA tensor-map loads + trees3 + vote        */
 #define B2S_KERNEL_TREES3 3            /* the same with plain loads                                       */
-#define B2S_KERNEL_TREES2_TMAP 4       /* trees_model_kernel with TMA tensor-map loads + vote_kernel      */
-#define B2S_KERNEL_TREES2 5            /* the same with plain loads                                       */
+#define B2S_KERNEL_TREES2_TMAP 4       /* retired (trees_model_kernel, TMA loads): no longer returned     */
+#define B2S_KERNEL_TREES2 5            /* retired (trees_model_kernel): no longer returned                */
 #define B2S_KERNEL_ROWTHREAD_TMA 6     /* rowthread kernel, TMA tensor-map loads (swizzled 2-D boxes)     */
 #define B2S_KERNEL_ROWTHREAD_LDGSTS 7  /* rowthread kernel, cp.async loads from device memory             */
 #define B2S_KERNEL_ROWTHREAD_HOST 8    /* rowthread kernel, cp.async loads from mapped host memory        */

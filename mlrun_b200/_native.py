@@ -26,9 +26,9 @@ NAN_ERROR, NAN_DEFAULT_CHILD = 0, 1
 CAT_NONNEG, CAT_TRUNC = 0, 1   # a valid category code is x >= 0 (xgboost) | x > -1, trunc(x) >= 0 (LightGBM)
 COL_F32, COL_I32, COL_I64 = 0, 1, 2
 # B2S_KERNEL_* (b2s_plan_last_kernel) -> name
-KERNELS = {0: None, 1: "dense", 2: "trees3/tma", 3: "trees3", 4: "trees2/tma", 5: "trees2", 6: "rowthread/tma",
-           7: "rowthread/ldgsts", 8: "rowthread/host", 10: "rows", 11: "store", 12: "trees3_cat/tma", 13: "trees3_cat",
-           14: "rows_cat", 15: "rowthread/bulk"}
+KERNELS = {0: None, 1: "dense", 2: "trees3/tma", 3: "trees3", 6: "rowthread/tma", 7: "rowthread/ldgsts",
+           8: "rowthread/host", 10: "rows", 11: "store", 12: "trees3_cat/tma", 13: "trees3_cat", 14: "rows_cat",
+           15: "rowthread/bulk"}
 DATE_PARTS = {"year": 0, "month": 1, "day": 2, "hour": 3, "minute": 4, "second": 5, "day_of_week": 6, "dayofweek": 6,
               "weekday": 6, "day_of_year": 7, "dayofyear": 7, "quarter": 8, "is_leap_year": 9, "days_in_month": 10,
               "daysinmonth": 10, "is_month_start": 11, "is_month_end": 12, "is_quarter_start": 13, "is_quarter_end": 14,

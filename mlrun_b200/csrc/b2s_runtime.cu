@@ -26,7 +26,6 @@
 #include "b2s_internal.h"
 #include "b2s_device.cuh"
 #include "b2s_rowthread.cuh"
-#include "b2s_trees2.cuh"
 #include "b2s_trees3.cuh"
 #include "b2s_dense.cuh"
 #include <nvtx3/nvToolsExt.h>  // header-only: ranges cost nothing unless a profiler is attached
@@ -181,21 +180,6 @@ struct b2s_plan_s {
   std::vector<void*> peers;
   int64_t peer_off = 0;
   struct b2s_comm_s* comm = nullptr;  // attached merge communicator (double-buffered targets + completion flags)
-  // shared-memory-resident tree kernel
-  bool t2_ok = false;
-  int t2_NS = 1, t2_grid = 0, t2_block = 512, t2_smem = 0;
-  T2Params t2{};
-  char* d_t2_blob = nullptr;
-  // per-model predictions between trees_model_kernel and vote_kernel: one scratch per stream the plan is launched on
-  // (launches on one stream are ordered; the ring's stream, the library stream and caller streams may overlap)
-  struct TreeScratch {
-    double* pred = nullptr;
-    int32_t* row_bad = nullptr;
-    uint32_t* xt = nullptr;  // trees3: the batch transposed into tiles (t3_prep_kernel)
-    int64_t rows = 0;
-  };
-  std::map<cudaStream_t, TreeScratch> t2_scratch;
-  std::mutex scratch_mu;
   // dense linear head on the tensor cores (b2s_dense.cu): > 8 scores over <= 128 plain numeric columns
   bool dense_ok = false;
   DenseParams dense{};
@@ -213,6 +197,16 @@ struct b2s_plan_s {
   const int32_t* d_t3_col_score = nullptr;
   const int32_t* d_t3_col_order = nullptr;   // the columns by score (t3_vote_kernel)
   const int32_t* d_t3_model_cols = nullptr;  // [n_models + 1] each model's range of d_t3_col_order
+  // trees3's partial sums, row flags and transposed tiles: one scratch per stream the plan is launched on
+  // (launches on one stream are ordered; the ring's stream, the library stream and caller streams may overlap)
+  struct TreeScratch {
+    double* partial = nullptr;   // per-column partial sums, column-major (trees3_kernel -> t3_vote_kernel)
+    int32_t* row_bad = nullptr;  // per-row non-finite input flags (t3_prep_kernel -> t3_vote_kernel)
+    uint32_t* xt = nullptr;      // the batch transposed into tiles (t3_prep_kernel -> trees3_kernel)
+    int64_t rows = 0;
+  };
+  std::map<cudaStream_t, TreeScratch> tree_scratch;
+  std::mutex scratch_mu;
   // host staging for run_host
   char* h_stage_in = nullptr;
   char* h_stage_out = nullptr;
@@ -847,8 +841,8 @@ static int32_t host_key(float x) {
   return b ^ ((b >> 31) & 0x7fffffff);
 }
 
-// Lower a MODE_TREES plan to parts (b2s_trees3.cuh).  Leaves p->t3_ok false when the plan does not qualify (the caller
-// then falls back to the round-1 kernels); returns an error only for CUDA failures.
+// Lower a MODE_TREES plan to parts (b2s_trees3.cuh).  Leaves p->t3_ok false when the plan does not qualify (the plan
+// then runs on rows_kernel<TREES>); returns an error only for CUDA failures.
 static int t3_build(b2s_plan_s* p, const KParams& k, bool any_fill) {
   const int n_in = p->n_in, M = (int)p->models.size();
   const int sms = G.prop.multiProcessorCount;
@@ -1657,115 +1651,6 @@ extern "C" int b2s_plan_finalize(b2s_plan_t p) {
     if (p->mode == MODE_TREES && identity_schema && !any_map) {
       if (int rc = t3_build(p, k, any_fill)) return rc;
     }
-    // ---- round-1 tree path, for the plans t3_build declines (trees deeper than kT3MaxDepth, or tables too large for it)
-    if (!p->t3_ok && p->mode == MODE_TREES && !need_expand && !p->any_cat) {  // trees_model_kernel has no categorical walk
-      // re-pack every model as complete heap-ordered trees; one model must fit one CTA's shared memory
-      bool ok = true;
-      std::vector<int> depth(M, 0);
-      size_t max_table = 0;
-      for (int mi = 0; mi < M && ok; ++mi) {
-        auto& m = p->models[mi];
-        if (m.kind != MK_TREES) { ok = false; break; }
-        const int nt = (int)m.tree_slot.size();
-        for (int t = 0; t < nt; ++t) {
-          const int base = m.tree_offset[t];
-          std::vector<std::pair<int, int>> stack{{0, 0}};
-          while (!stack.empty()) {
-            auto [node, d] = stack.back();
-            stack.pop_back();
-            depth[mi] = std::max(depth[mi], d);
-            if (m.feature[base + node] >= 0) {
-              stack.push_back({m.left[base + node], d + 1});
-              stack.push_back({m.right[base + node], d + 1});
-            }
-          }
-        }
-        if (depth[mi] > 8) ok = false;
-        const size_t ni = ((size_t)1 << depth[mi]) - 1, nl = (size_t)1 << depth[mi];
-        max_table = std::max(max_table, align_up((size_t)nt * ni * 8, 16) + (size_t)nt * nl * 8 + (size_t)nt * 4);
-      }
-      const int TR2 = kT2TileRows, G2 = kT2Groups, ST2 = 1;  // one row-major landing tile + one transposed tile
-      const int NS2 = p->NS <= 1 ? 1 : (p->NS <= 4 ? 4 : 0);
-      const size_t part_bytes = (size_t)(G2 - 1) * TR2 * std::max(NS2, 1) * 8;
-      const size_t tiles_bytes = (size_t)ST2 * TR2 * pitch * 4 + (size_t)((n_in + 3) / 4 * 4) * TR2 * 4 + (size_t)TR2 * 4 + 16 + 1024;  // + mbarrier + alignment slack
-      const size_t total2 = align_up(max_table, 16) + align_up(part_bytes, 16) + tiles_bytes;
-      if (ok && NS2 > 0 && total2 <= (size_t)smem_cap && M <= sms) {
-        BlobBuilder tb;
-        std::vector<T2Model> t2m(M);
-        std::vector<size_t> o_nodes(M), o_leaves(M), o_slot(M), o_scale(M);
-        for (int mi = 0; mi < M; ++mi) {
-          auto& m = p->models[mi];
-          const int nt = (int)m.tree_slot.size();
-          const int D = depth[mi];
-          const int ni = (1 << D) - 1, nl = 1 << D;
-          std::vector<HeapNode> hn((size_t)nt * std::max(ni, 1), HeapNode{0, std::numeric_limits<float>::infinity()});
-          std::vector<double> hl((size_t)nt * nl, 0.0);
-          for (int t = 0; t < nt; ++t) {
-            const int base = m.tree_offset[t];
-            struct It { int heap, d, src; };
-            std::vector<It> stack{{0, 0, 0}};
-            while (!stack.empty()) {
-              It it = stack.back();
-              stack.pop_back();
-              const bool leaf = m.feature[base + it.src] < 0;
-              if (it.d == D) {
-                hl[(size_t)t * nl + (it.heap - ni)] = m.leaf_value[base + it.src];
-                continue;
-              }
-              if (leaf) {  // pad: a threshold of +inf sends every finite value left; both sides carry the leaf
-                hn[(size_t)t * ni + it.heap] = HeapNode{0, std::numeric_limits<float>::infinity()};
-                stack.push_back({2 * it.heap + 1, it.d + 1, it.src});
-                stack.push_back({2 * it.heap + 2, it.d + 1, it.src});
-              } else {
-                hn[(size_t)t * ni + it.heap] = HeapNode{m.feature[base + it.src], m.threshold[base + it.src]};
-                stack.push_back({2 * it.heap + 1, it.d + 1, m.left[base + it.src]});
-                stack.push_back({2 * it.heap + 2, it.d + 1, m.right[base + it.src]});
-              }
-            }
-          }
-          o_nodes[mi] = tb.add(hn);
-          o_leaves[mi] = tb.add(hl);
-          o_slot[mi] = tb.add(m.tree_slot);
-          o_scale[mi] = tb.add(m.tree_scale);
-          t2m[mi].n_trees = nt;
-          t2m[mi].depth = D;
-          t2m[mi].n_internal = ni;
-          t2m[mi].n_leaves = nl;
-        }
-        const size_t o_models2 = align_up(tb.data.size(), 16);
-        tb.data.resize(o_models2 + sizeof(T2Model) * M);
-        CUDA_TRY(cudaMalloc(&p->d_t2_blob, tb.data.size()));
-        for (int mi = 0; mi < M; ++mi) {
-          t2m[mi].nodes = (const HeapNode*)(p->d_t2_blob + o_nodes[mi]);
-          t2m[mi].leaves = (const double*)(p->d_t2_blob + o_leaves[mi]);
-          t2m[mi].slot = (const int32_t*)(p->d_t2_blob + o_slot[mi]);
-          t2m[mi].scale = (const double*)(p->d_t2_blob + o_scale[mi]);
-        }
-        memcpy(tb.data.data() + o_models2, t2m.data(), sizeof(T2Model) * M);
-        CUDA_TRY(cudaMemcpy(p->d_t2_blob, tb.data.data(), tb.data.size(), cudaMemcpyHostToDevice));
-        T2Params& t = p->t2;
-        memset(&t, 0, sizeof(t));
-        t.n_in = n_in;
-        t.n_models = M;
-        t.tile_rows = TR2;
-        t.pitch = pitch;
-        t.stages = ST2;
-        t.groups = G2;
-        t.t2 = (const T2Model*)(p->d_t2_blob + o_models2);
-        t.models = k.models;
-        t.classes = k.classes;
-        t.bias = k.bias;
-        t.sm_tables = 0;
-        t.sm_part = (int)align_up(max_table, 16);
-        t.sm_tiles = (int)(align_up(max_table, 16) + align_up(part_bytes, 16));
-        p->t2_smem = (int)total2;
-        p->t2_NS = NS2;
-        p->t2_block = TR2 * G2;
-        p->t2_grid = std::max(M, (sms / M) * M);
-        p->t2_ok = true;
-        p->kernels_per_batch = 2;
-      }
-    }
     for (int i = 0; i < 4; ++i) CUDA_TRY(cudaEventCreate(&p->ev[i]));
     p->finalized = true;
     return B2S_OK;
@@ -1781,7 +1666,6 @@ extern "C" const char* b2s_plan_kernel(b2s_plan_t p) {
   const bool tmap = p->rt_NCH >= 8 && p->n_in == p->rt_NCH * 4 && tensor_map_encoder();
   if (p->dense_ok) snprintf(buf, sizeof(buf), "dense_head_kernel<N=%d> (wgmma tf32, %s, register accumulator groups; %d scores over %d columns)", p->dense.n_pad, p->dense.exact ? "exact 3-term input split" : "2-term input split", p->dense.n_scores, p->dense.n_in);
   else if (p->t3_ok) snprintf(buf, sizeof(buf), "t3_prep_kernel + trees3_kernel<D=%d,%s%s> + t3_vote_kernel (%d parts resident in shared memory, %d walking warps)", p->t3_D, p->t3_miss ? "NaN routing" : "floats", p->t3_cat ? ",categorical" : "", p->t3_parts, p->t3.warps);
-  else if (p->t2_ok) snprintf(buf, sizeof(buf), "trees_model_kernel<%d> + vote_kernel (models resident in shared memory)", p->t2_NS);
   else if (p->rt_ok) snprintf(buf, sizeof(buf), "rowthread_kernel<NCH=%d,NS=%d,TPR=%d,%s>", p->rt_NCH, p->rt_NS, rt_tpr(p->rt_NCH), tmap ? "TMA tensor-map loads" : "TMA bulk loads");
   else snprintf(buf, sizeof(buf), "rows_kernel<%s,NS=%d>%s", p->mode == MODE_LINEAR ? "LINEAR" : (p->mode == MODE_TREES ? "TREES" : "STORE"), p->NS, p->any_cat ? " (categorical splits)" : "");
   return buf;
@@ -1811,7 +1695,7 @@ struct NvtxRange {  // one range per plan launch, named after the kernel family 
 static int launch_on(b2s_plan_t p, const void* d_rows, int64_t n_rows, int64_t stride, void* d_out, int32_t* d_status,
                      cudaStream_t st, bool host_rows = false) {
   if (n_rows == 0) return B2S_OK;
-  NvtxRange nvtx(p->dense_ok ? "b2s:dense_head" : p->t3_ok ? "b2s:trees3 (prep+walk+vote)" : p->t2_ok ? "b2s:trees2"
+  NvtxRange nvtx(p->dense_ok ? "b2s:dense_head" : p->t3_ok ? "b2s:trees3 (prep+walk+vote)"
                  : p->rt_ok ? "b2s:rowthread" : p->mode == MODE_STORE ? "b2s:rows_store" : "b2s:rows_kernel");
   KParams k = p->kp;
   k.rows = (const char*)d_rows;
@@ -1857,14 +1741,14 @@ static int launch_on(b2s_plan_t p, const void* d_rows, int64_t n_rows, int64_t s
     b2s_plan_s::TreeScratch sc;
     {
       std::lock_guard<std::mutex> lk(p->scratch_mu);
-      b2s_plan_s::TreeScratch& mine = p->t2_scratch[st];
+      b2s_plan_s::TreeScratch& mine = p->tree_scratch[st];
       if (n_rows > mine.rows) {  // cudaFree waits for the work that still reads the old buffers
-        if (mine.pred) cudaFree(mine.pred);
+        if (mine.partial) cudaFree(mine.partial);
         if (mine.row_bad) cudaFree(mine.row_bad);
         if (mine.xt) cudaFree(mine.xt);
         mine = b2s_plan_s::TreeScratch{};
         const int64_t cap = std::max<int64_t>(align_up((size_t)n_rows, 64), 65536);
-        CUDA_TRY(cudaMalloc(&mine.pred, (size_t)cap * C * 8));
+        CUDA_TRY(cudaMalloc(&mine.partial, (size_t)cap * C * 8));
         CUDA_TRY(cudaMalloc(&mine.row_bad, (size_t)cap * 4));
         CUDA_TRY(cudaMalloc(&mine.xt, (size_t)(cap / kT3TR) * p->t3.xt_words * 4));
         mine.rows = cap;
@@ -1891,59 +1775,13 @@ static int launch_on(b2s_plan_t p, const void* d_rows, int64_t n_rows, int64_t s
     T3Params t = p->t3;
     t.xt = sc.xt;
     t.n_rows = n_rows;
-    t.partial = sc.pred;
+    t.partial = sc.partial;
     t.col_stride = sc.rows;
     e3 = t3_launch_walk(t, p->t3_D, p->t3_miss, p->t3_cat, p->t3_grid, p->t3_block, p->t3_smem, (int)G.prop.sharedMemPerBlockOptin, st);
     if (e3 != cudaSuccess) return fail(B2S_ERR_CUDA, "tree kernel launch failed: %s", cudaGetErrorString(e3));
     const int vgrid = (int)std::max<int64_t>(1, std::min<int64_t>(4 * G.prop.multiProcessorCount, (n_rows + 255) / 256));
-    e3 = t3_launch_vote(k, sc.pred, sc.rows, p->d_t3_col_score, p->d_t3_col_order, p->d_t3_model_cols, sc.row_bad, vgrid, st);
+    e3 = t3_launch_vote(k, sc.partial, sc.rows, p->d_t3_col_score, p->d_t3_col_order, p->d_t3_model_cols, sc.row_bad, vgrid, st);
     if (e3 != cudaSuccess) return fail(B2S_ERR_CUDA, "vote kernel launch failed: %s", cudaGetErrorString(e3));
-    return B2S_OK;
-  }
-  if (p->t2_ok) {
-    b2s_plan_s::TreeScratch sc;
-    {
-      std::lock_guard<std::mutex> lk(p->scratch_mu);
-      b2s_plan_s::TreeScratch& mine = p->t2_scratch[st];
-      if (n_rows > mine.rows) {  // cudaFree waits for the work that still reads the old buffers
-        if (mine.pred) { cudaFree(mine.pred); cudaFree(mine.row_bad); }
-        mine = b2s_plan_s::TreeScratch{};
-        const int64_t cap = std::max<int64_t>(n_rows, 65536);
-        CUDA_TRY(cudaMalloc(&mine.pred, (size_t)cap * p->kp.n_models * 8));
-        CUDA_TRY(cudaMalloc(&mine.row_bad, (size_t)cap * 4));
-        mine.rows = cap;
-      }
-      sc = mine;
-    }
-    T2Params t = p->t2;
-    t.rows = (const char*)d_rows;
-    t.row_stride = stride;
-    t.n_rows = n_rows;
-    t.pred = sc.pred;
-    t.row_bad = sc.row_bad;
-    t.vec_ok = k.vec_ok;
-    static std::atomic<bool> t2_attr{false};
-    if (!t2_attr) {
-      CUDA_TRY(cudaFuncSetAttribute(trees_model_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G.prop.sharedMemPerBlockOptin));
-      CUDA_TRY(cudaFuncSetAttribute(trees_model_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G.prop.sharedMemPerBlockOptin));
-      t2_attr = true;
-    }
-    const int64_t tiles2 = (n_rows + t.tile_rows - 1) / t.tile_rows;
-    const int M2 = p->kp.n_models;
-    const int grid2 = (int)std::max<int64_t>(M2, std::min<int64_t>(p->t2_grid, tiles2 * M2));
-    G.launches.fetch_add(2, std::memory_order_relaxed);
-    alignas(64) CUtensorMap tmap;
-    memset(&tmap, 0, sizeof(tmap));
-    t.use_tmap = (!host_rows && t.vec_ok && (p->n_in % 32) == 0 && encode_rows_map(&tmap, d_rows, n_rows, stride, p->n_in, t.tile_rows)) ? 1 : 0;
-    p->last_kernel.store(t.use_tmap ? B2S_KERNEL_TREES2_TMAP : B2S_KERNEL_TREES2, std::memory_order_relaxed);
-    if (p->t2_NS == 1) trees_model_kernel<1><<<grid2, p->t2_block, p->t2_smem, st>>>(t, tmap);
-    else trees_model_kernel<4><<<grid2, p->t2_block, p->t2_smem, st>>>(t, tmap);
-    cudaError_t e2 = cudaGetLastError();
-    if (e2 != cudaSuccess) return fail(B2S_ERR_CUDA, "tree kernel launch failed: %s", cudaGetErrorString(e2));
-    const int vgrid = (int)std::max<int64_t>(1, std::min<int64_t>(4 * G.prop.multiProcessorCount, (n_rows + 255) / 256));
-    vote_kernel<<<vgrid, 256, 0, st>>>(k, sc.pred, sc.row_bad);
-    e2 = cudaGetLastError();
-    if (e2 != cudaSuccess) return fail(B2S_ERR_CUDA, "vote kernel launch failed: %s", cudaGetErrorString(e2));
     return B2S_OK;
   }
   if (p->dense_ok && !host_rows && k.vec_ok) {
@@ -2003,7 +1841,7 @@ int b2s_int_launch_gathered(b2s_plan_s* p, const B2SGather& g, long long n, void
   static const int fused = getenv("B2S_ENRICH_FUSED") ? atoi(getenv("B2S_ENRICH_FUSED")) : 1;
   // the gather loader lives in the row-thread kernel (linear models, rows of whole 16-byte chunks); with a table impute
   // policy, one-hot sources would need the policy applied before the category search: those plans gather first
-  if (!fused || !p->rt_ok || p->t2_ok || p->t3_ok || (p->n_in % 4) != 0) return fail(B2S_ERR_UNSUPPORTED, "plan is not fusable with the gather");
+  if (!fused || !p->rt_ok || p->t3_ok || (p->n_in % 4) != 0) return fail(B2S_ERR_UNSUPPORTED, "plan is not fusable with the gather");
   if (g.any_impute && p->rt_cat_cols > 0) return fail(B2S_ERR_UNSUPPORTED, "one-hot columns under a table impute policy gather first");
   if (n <= 0) return B2S_OK;
   G.launches.fetch_add(1, std::memory_order_relaxed);
@@ -2659,10 +2497,9 @@ extern "C" int b2s_plan_destroy(b2s_plan_t p) {
       if (p->ev[i]) cudaEventDestroy(p->ev[i]);
     for (cudaEvent_t e : p->chunk_ev) cudaEventDestroy(e);
     if (p->d_blob) cudaFree(p->d_blob);
-    if (p->d_t2_blob) cudaFree(p->d_t2_blob);
     if (p->d_t3_blob) cudaFree(p->d_t3_blob);
-    for (auto& kv : p->t2_scratch)
-      if (kv.second.pred) { cudaFree(kv.second.pred); cudaFree(kv.second.row_bad); if (kv.second.xt) cudaFree(kv.second.xt); }
+    for (auto& kv : p->tree_scratch)
+      if (kv.second.partial) { cudaFree(kv.second.partial); cudaFree(kv.second.row_bad); if (kv.second.xt) cudaFree(kv.second.xt); }
     delete p;
     return B2S_OK;
   } catch (const std::exception& e) {

@@ -1,10 +1,9 @@
 """xgboost and LightGBM models with categorical splits on every kernel that serves them.  Needs an H100: `-m gpu`.
 
-Plans with a categorical node run on trees3 (`trees3_kernel<D,MISS,U,CAT=true>`, depth <= 8) or on `rows_kernel<TREES>`;
-`trees_model_kernel` has no categorical walk, so the plans it would serve land on rows_kernel.  Each case checks the output
-against the float64 walk of the packed model (tests/tree_cat_fixtures.py) with the score bound of
-tests/test_gpu_tree_paths.py, against the libraries' decision functions (the oracle), and asserts `plan.kernel` and
-`plan.last_kernel`.  Labels and status words are compared exactly.
+Plans with a categorical node run on trees3 (`trees3_kernel<D,MISS,U,CAT=true>`, depth <= 8) or on `rows_kernel<TREES>`,
+like numeric ones.  Each case checks the output against the float64 walk of the packed model (tests/tree_cat_fixtures.py)
+with the score bound of tests/test_gpu_tree_paths.py, against the libraries' decision functions (the oracle), and asserts
+`plan.kernel` and `plan.last_kernel`.  Labels and status words are compared exactly.
 """
 
 import ctypes as C
@@ -228,8 +227,8 @@ def test_sets_too_large_for_trees3_fall_back_to_rows_kernel():
     np.testing.assert_allclose(out[ok, 0], fx.xgboost_predict(doc, X[ok]), rtol=1e-5, atol=1e-5)
 
 
-def test_wide_plan_skips_trees_model_kernel():
-    """420 columns leave trees3 no room (a numeric model of this shape runs on trees_model_kernel): rows_kernel<TREES>"""
+def test_wide_plan_on_rows_kernel():
+    """420 columns leave trees3 no room: rows_kernel<TREES> walks the categorical splits"""
     n_in = 420
     doc, m = lgbm_model(6, n_feat=n_in, seed=81, n_trees=10)
     X = inputs(1000, n_feat=n_in, seed=82)

@@ -1,11 +1,10 @@
 """Tree plans on every kernel that can serve them, against plain float64 references.  Needs an H100: `-m gpu`.
 
-A tree plan runs on one of three kernel families, chosen when the plan is finalized (b2s_plan_finalize):
+A tree plan runs on one of two kernel families, chosen when the plan is finalized (b2s_plan_finalize):
   * t3_prep_kernel + trees3_kernel<D,MISS,U> + t3_vote_kernel: identity schema (+ Imputer), depth <= 8, <= 8 linear score
     columns, the part tables fit;
-  * trees_model_kernel<1|4> + vote_kernel: plans trees3 declines (wide rows), all models trees, depth <= 8, <= 4 scores;
   * rows_kernel<TREES,NS>: everything else -- trees deeper than 8 levels (unconstrained scikit-learn forests), trees behind
-    a OneHotEncoder or MapValues, more than 8 linear score columns.
+    a OneHotEncoder or MapValues, more than 8 linear score columns, rows too wide for trees3's transposed tiles.
 Every case asserts `plan.kernel` and, after the run, `plan.last_kernel`, so a plan that moves to another kernel fails.
 
 Scores: every tree path accumulates in fp64 and rounds once to float32 on output.  Per element
@@ -311,7 +310,7 @@ def test_trees3_more_than_32_scores_in_one_plan(sms, shape, vote):
     check_plan_output(out, st, models, X, vote=v)
 
 
-# ------------------------------------------------------------------------------------------ trees_model_kernel (wide rows)
+# ------------------------------------------------------------------------------------------ rows_kernel<TREES,NS>: wide rows
 def wide_rows(n, n_in, seed, models):
     X = on_thresholds(np.random.default_rng(seed).normal(size=(n, n_in)).astype(np.float32), models, seed)
     X[n // 3, 2] = np.nan
@@ -319,29 +318,30 @@ def wide_rows(n, n_in, seed, models):
     return X
 
 
-@pytest.mark.parametrize("case", ["420-cp16", "419-cp4", "416-tma", "408-ns4"])
-def test_trees_model_kernel(case):
+@pytest.mark.parametrize("case", ["420-cp16", "419-cp4", "416-d7", "408-ns4"])
+def test_wide_rows_on_rows_kernel(case):
     """plans trees3 cannot hold (two transposed tiles of rows this wide leave no room for a table) run on
-    trees_model_kernel: 420 columns (16-byte loads), 419 (4-byte), 416 with a device batch (tensor map), and a majority vote
-    of a binary depth-8 classifier and a 3-class one over 408 columns (trees_model_kernel<4>)"""
+    rows_kernel<TREES>: 420 columns (16-byte loads), 419 (4-byte), 416 at depth 7, and a majority vote of a binary depth-8
+    classifier and a 3-class one over 408 columns (NS = 4).  At these widths the kernel's shared-memory budget leaves one
+    tile stage, and a single model's tile shrinks from 256 to 128 rows: code that only wide rows reach"""
     n_in = int(case.split("-")[0])
     vote = None
     if case == "408-ns4":
         models = [pk(gbc(n_in, 8, 1, 2, seed=1)), pk(gbc(n_in, 1, 1, 3, seed=2))]
         assert max_depth(models[0]) == 8
         vote = (nat.VOTE_MAJORITY, [0.6, 0.4])
-        want_kernel, ran = "trees_model_kernel<4>", "trees2"
+        want_kernel = "rows_kernel<TREES,NS=4>"
     else:
         models = [pk(gbr(n_in, 7 if n_in == 416 else 6, 6 if n_in == 416 else 10, seed=n_in))]
         assert max_depth(models[0]) == (7 if n_in == 416 else 6)  # one level less would fit trees3 at 416 columns
-        want_kernel, ran = "trees_model_kernel<1>", ("trees2/tma" if n_in == 416 else "trees2")
+        want_kernel = "rows_kernel<TREES,NS=1>"
     plan = build(ColumnProgram(names(n_in)), models, vote=vote)
     assert_kernel(plan, want_kernel)
     X = wide_rows(1000, n_in, n_in, models)
     rows = Rows(X)
     for n in (1, 65, 777, 1000):
         out, st = run_device(plan, rows, n)
-        assert plan.last_kernel == ran
+        assert plan.last_kernel == "rows"
         check_plan_output(out, st, models, X[:n], vote=vote)
 
 
@@ -473,10 +473,10 @@ def test_many_models_on_rows_kernel(M):
 
 
 # ------------------------------------------------------------------------------------------ the NaN contract of the fallbacks
-def test_nan_routing_models_flag_nan_rows_on_the_fallbacks():
+def test_nan_routing_models_flag_nan_rows_on_rows_kernel():
     """b2s_plan_add_tree_model_ex: NaN routing is honoured on trees3 only; elsewhere a NaN row is flagged, never answered
     differently.  A scikit-learn forest fitted on NaN (rows_kernel: depth > 8) and an xgboost document over 420 columns
-    (trees_model_kernel): NaN rows get status bit 1, Inf rows too, every other row matches the reference"""
+    (rows_kernel: too wide for trees3): NaN rows get status bit 1, Inf rows too, every other row matches the reference"""
     from sklearn.ensemble import RandomForestRegressor
 
     Xf, y = regression_data(12, seed=95, nan_frac=0.1)
@@ -484,7 +484,7 @@ def test_nan_routing_models_flag_nan_rows_on_the_fallbacks():
     assert forest[1].nan_ok and max_depth(forest) > 8
     _, wide = xgb(6, 420, seed=96, n_trees=10)
     for packed, n_in, kernel, ran in ((forest, 12, "rows_kernel<TREES,NS=1>", "rows"),
-                                      (wide, 420, "trees_model_kernel<1>", "trees2")):
+                                      (wide, 420, "rows_kernel<TREES,NS=1>", "rows")):
         plan = build(ColumnProgram(names(n_in)), [packed])
         assert_kernel(plan, kernel)
         X = fx.grid_inputs(3000, n_in, seed=n_in, nan_frac=0.0005 if n_in > 100 else 0.02)
@@ -497,10 +497,11 @@ def test_nan_routing_models_flag_nan_rows_on_the_fallbacks():
         check_plan_output(out, st, [packed], X, ok=ok)
 
 
-# ------------------------------------------------------------------------------------------ one model on every path
-def test_same_model_on_every_path():
-    """the same packed ensemble on trees3 (16 columns), trees_model_kernel (padded with unused zero columns to 420) and
-    rows_kernel (a OneHotEncoder on an unused column): each within the bound of the reference, and of each other"""
+# ------------------------------------------------------------------------------------------ one model on both tree kernels
+def test_same_model_on_trees3_and_rows_kernel():
+    """the same packed ensemble on trees3 (16 columns), rows_kernel over rows too wide for trees3 (padded with unused zero
+    columns to 420) and rows_kernel behind a OneHotEncoder on an unused column: each within the bound of the reference,
+    and of each other"""
     models = [pk(gbr(16, 6, 10, seed=11)), pk(gbr(16, 5, 8, seed=12))]
     X = on_thresholds(np.random.default_rng(13).normal(size=(4000, 16)).astype(np.float32), models, seed=13)
     ref = Ref(models, X)
@@ -511,8 +512,9 @@ def test_same_model_on_every_path():
     Xw = np.zeros((4000, 420), dtype=np.float32)
     Xw[:, :16] = X
     plan = build(ColumnProgram(names(420)), models)
-    assert_kernel(plan, "trees_model_kernel<1>")
-    outs["trees2"] = run_device(plan, Xw)[0]
+    assert_kernel(plan, "rows_kernel<TREES,NS=1>")
+    outs["rows/wide"] = run_device(plan, Xw)[0]
+    assert plan.last_kernel == "rows"
     Xo = np.concatenate([X, np.zeros((4000, 1), dtype=np.float32)], axis=1)
     prog = ColumnProgram(names(17))
     prog.one_hot({"f16": [5.0]})
