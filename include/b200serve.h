@@ -466,6 +466,32 @@ int b2s_pit_join_device(const int64_t* d_ts, int64_t n, const b2s_pit_set* sets,
                         int32_t n_cols, int64_t* d_order, uint64_t* d_miss, void* stream);
 int b2s_pit_join_host(const int64_t* ts, int64_t n, const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols,
                       int32_t n_cols, int64_t* order, uint64_t* miss, b2s_stats* stats);
+/* Training sets: the join above, then only the rows the reference's merged frame keeps after
+ * dropna(subset=[label]) (feature_store/retrieval/base.py:343-346): rows every exact-key (inner) join matched and, with a
+ * label, rows whose label is present.  The label is output `out` of set `set` (then the set must have matched) or, with
+ * set -1, entity column `out`; B2S_PIT_LABEL_NAN also drops NaN values (4- or 8-byte floats), B2S_PIT_LABEL_NAT drops
+ * INT64_MIN (8 bytes).  The kept rows of every output, found flag, ts_out, entity column and order are written first, in
+ * sorted order, and *kept counts them; the arrays still need room for n rows.  miss[s] counts the rows set s misses among
+ * those every earlier exact-key set matched (the frame at the set's place in the merge, before the label filter).  Every
+ * set needs its found array.  _device: device arrays, asynchronous on `stream`; miss and *d_kept are written.  _host:
+ * host arrays; only the kept rows are copied back, in ranges of 1 Mi rows; phase_ms (may be NULL) gets the sort, join and
+ * compaction times; stats->kernels counts every launch: the sort's 24 (with ts), the join's max(1, n_sets,
+ * ceil(n_cols / 64)), 2 to find the kept rows and ceil(arrays / 64) to compact them, where arrays counts each set's outputs,
+ * ts_out and found, the entity columns and order.  B2S_ERR_INVALID before any launch for what b2s_pit_join_* refuses,
+ * more than 64 sets, a set without found flags, a null miss / kept counter, or a label that names no output or does not fit
+ * its kind. */
+enum { B2S_PIT_LABEL_FOUND = 0, B2S_PIT_LABEL_NAN = 1, B2S_PIT_LABEL_NAT = 2 };
+typedef struct b2s_pit_label {
+  int32_t set;   /* index of the label's set, or -1: an entity column */
+  int32_t out;   /* output of that set, or entity column */
+  int32_t kind;  /* B2S_PIT_LABEL_* */
+} b2s_pit_label;
+int b2s_pit_train_device(const int64_t* d_ts, int64_t n, const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols,
+                         int32_t n_cols, const b2s_pit_label* label, int64_t* d_order, uint64_t* d_miss, int64_t* d_kept,
+                         void* stream);
+int b2s_pit_train_host(const int64_t* ts, int64_t n, const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols,
+                       int32_t n_cols, const b2s_pit_label* label, int64_t* order, uint64_t* miss, int64_t* kept,
+                       float* phase_ms, b2s_stats* stats);
 
 /* ---- windowed aggregations at feature-set ingest ------------------------------------------------------------------
  * storey.AggregateByKey as FeatureSet.add_aggregation places it in a feature set's graph (feature_store/feature_set.py:

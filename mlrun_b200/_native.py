@@ -71,6 +71,13 @@ class PitCol(C.Structure):
     _fields_ = [("src", _vp), ("dst", _vp), ("bytes", _i32)]
 
 
+PIT_LABEL_FOUND, PIT_LABEL_NAN, PIT_LABEL_NAT = 0, 1, 2
+
+
+class PitLabel(C.Structure):
+    _fields_ = [("set", _i32), ("out", _i32), ("kind", _i32)]
+
+
 # B2S_AGG_* operation bits, in the order of the outputs of one aggregation
 AGG_OPS = {"count": 1, "sum": 2, "sqr": 4, "max": 8, "min": 16, "first": 32, "last": 64, "avg": 128, "stdvar": 256, "stddev": 512}
 
@@ -165,6 +172,10 @@ SIGNATURES = {
     "b2s_pit_index_info": (C.c_int, [_vp, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_i64), _pi32, C.POINTER(_i64)]),
     "b2s_pit_join_device": (C.c_int, [_vp, _i64, C.POINTER(PitSet), _i32, C.POINTER(PitCol), _i32, _vp, _vp, _vp]),
     "b2s_pit_join_host": (C.c_int, [_vp, _i64, C.POINTER(PitSet), _i32, C.POINTER(PitCol), _i32, _vp, _vp, C.POINTER(Stats)]),
+    "b2s_pit_train_device": (C.c_int, [_vp, _i64, C.POINTER(PitSet), _i32, C.POINTER(PitCol), _i32, C.POINTER(PitLabel), _vp, _vp,
+                                       _vp, _vp]),
+    "b2s_pit_train_host": (C.c_int, [_vp, _i64, C.POINTER(PitSet), _i32, C.POINTER(PitCol), _i32, C.POINTER(PitLabel), _vp, _vp, _vp,
+                                     _pf32, C.POINTER(Stats)]),
     # windowed aggregations
     "b2s_agg_run_device": (C.c_int, [_vp, _vp, _i64, C.POINTER(AggSpec), _i32, _vp, _vp]),
     "b2s_agg_run_host": (C.c_int, [_vp, _vp, _i64, C.POINTER(AggSpec), _i32, _vp, C.POINTER(Stats)]),

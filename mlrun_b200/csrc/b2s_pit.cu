@@ -519,3 +519,372 @@ extern "C" int b2s_pit_join_host(const int64_t* ts, int64_t n, const b2s_pit_set
     return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
   }
 }
+
+// ---- training sets: the join, then the rows the reference's merge and label dropna keep, compacted in order --------------
+namespace {
+
+constexpr int kTrainSets = 64;     // sets one training-set call may join (the keep kernel reads every set's found flags)
+constexpr int kTile = 1024;        // rows per block of the keep and scatter kernels: one row per thread
+constexpr int kScatterCols = 64;   // arrays one scatter launch moves
+
+struct KeepParams {
+  const uint8_t* found[kTrainSets];
+  int32_t exact[kTrainSets];       // 1: an inner (exact-key) join drops the rows this set misses
+  int32_t n_sets;
+  const uint8_t* label_found;      // the label set's found flags; null: the label is an entity column (or there is none)
+  const void* label;               // the label values; null: no value test
+  int32_t label_bytes, label_kind;
+  int64_t n;
+};
+
+// keep[q] = the row survives every inner join and has a label; tile_count[tile] = its kept rows.  miss[s] counts the rows
+// set s misses among those every earlier inner join kept (the rows of the merged frame at the set's place in the merge).
+__global__ void __launch_bounds__(kTile) keep_kernel(const __grid_constant__ KeepParams p, uint8_t* __restrict__ keep,
+                                                     int64_t* __restrict__ tile_count, unsigned long long* __restrict__ miss) {
+  __shared__ unsigned long long s_miss[kTrainSets];
+  if (threadIdx.x < kTrainSets) s_miss[threadIdx.x] = 0;
+  __syncthreads();
+  const int64_t q = (int64_t)blockIdx.x * kTile + threadIdx.x;
+  const bool in = q < p.n;
+  bool alive = in;
+  for (int s = 0; s < p.n_sets; ++s) {
+    const bool f = in && p.found[s][q];
+    const unsigned missed = __ballot_sync(0xffffffffu, alive && !f);
+    if (missed && (threadIdx.x & 31) == 0) atomicAdd(&s_miss[s], (unsigned long long)__popc(missed));
+    if (p.exact[s]) alive = alive && f;
+  }
+  bool k = alive && (!p.label_found || p.label_found[q]);
+  if (k && p.label) {
+    if (p.label_kind == B2S_PIT_LABEL_NAN) {
+      k = p.label_bytes == 4 ? !isnan(static_cast<const float*>(p.label)[q]) : !isnan(static_cast<const double*>(p.label)[q]);
+    } else if (p.label_kind == B2S_PIT_LABEL_NAT) {
+      k = static_cast<const int64_t*>(p.label)[q] != INT64_MIN;
+    }
+  }
+  if (in) keep[q] = k ? 1 : 0;
+  const int kept = __syncthreads_count(k);
+  if (threadIdx.x == 0) tile_count[blockIdx.x] = kept;
+  if (threadIdx.x < p.n_sets && s_miss[threadIdx.x]) atomicAdd(&miss[threadIdx.x], s_miss[threadIdx.x]);
+}
+
+// one block: tile counts -> exclusive offsets (in place), *total = the kept rows
+__global__ void __launch_bounds__(1024) scan_tiles_kernel(int64_t* __restrict__ counts, int64_t n_tiles, int64_t* __restrict__ total) {
+  __shared__ int64_t s_sum[1024];
+  const int64_t per = (n_tiles + 1023) / 1024;
+  const int64_t lo = threadIdx.x * per < n_tiles ? threadIdx.x * per : n_tiles, hi = lo + per < n_tiles ? lo + per : n_tiles;
+  int64_t sum = 0;
+  for (int64_t i = lo; i < hi; ++i) sum += counts[i];
+  s_sum[threadIdx.x] = sum;
+  __syncthreads();
+  for (int off = 1; off < 1024; off <<= 1) {  // inclusive Hillis-Steele scan of the chunk sums
+    const int64_t v = threadIdx.x >= off ? s_sum[threadIdx.x - off] : 0;
+    __syncthreads();
+    s_sum[threadIdx.x] += v;
+    __syncthreads();
+  }
+  int64_t run = s_sum[threadIdx.x] - sum;
+  for (int64_t i = lo; i < hi; ++i) {
+    const int64_t c = counts[i];
+    counts[i] = run;
+    run += c;
+  }
+  if (threadIdx.x == 1023) *total = s_sum[1023];
+}
+
+struct ScatterParams {
+  const void* src[kScatterCols];
+  void* dst[kScatterCols];
+  int32_t bytes[kScatterCols];
+  int32_t n_cols;
+  int64_t n;
+};
+
+// the kept rows of every array, in order: row q goes to tile_off[tile] + its rank among the tile's kept rows
+__global__ void __launch_bounds__(kTile) scatter_kernel(const __grid_constant__ ScatterParams p, const uint8_t* __restrict__ keep,
+                                                        const int64_t* __restrict__ tile_off) {
+  __shared__ int s_warp[kTile / 32];
+  const int64_t q = (int64_t)blockIdx.x * kTile + threadIdx.x;
+  const bool k = q < p.n && keep[q];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned bal = __ballot_sync(0xffffffffu, k);
+  if (lane == 0) s_warp[warp] = __popc(bal);
+  __syncthreads();
+  if (warp == 0) {  // exclusive scan of the 32 warp counts
+    const int c = s_warp[lane];
+    int v = c;
+    for (int off = 1; off < 32; off <<= 1) {
+      const int u = __shfl_up_sync(0xffffffffu, v, off);
+      if (lane >= off) v += u;
+    }
+    s_warp[lane] = v - c;
+  }
+  __syncthreads();
+  if (!k) return;
+  const int64_t d = tile_off[blockIdx.x] + s_warp[warp] + __popc(bal & ((1u << lane) - 1u));
+  for (int c = 0; c < p.n_cols; ++c) {
+    switch (p.bytes[c]) {
+      case 1: static_cast<uint8_t*>(p.dst[c])[d] = static_cast<const uint8_t*>(p.src[c])[q]; break;
+      case 2: static_cast<uint16_t*>(p.dst[c])[d] = static_cast<const uint16_t*>(p.src[c])[q]; break;
+      case 4: static_cast<uint32_t*>(p.dst[c])[d] = static_cast<const uint32_t*>(p.src[c])[q]; break;
+      default: static_cast<uint64_t*>(p.dst[c])[d] = static_cast<const uint64_t*>(p.src[c])[q]; break;
+    }
+  }
+}
+
+int check_train(const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols, int32_t n_cols, const int64_t* ts, int64_t n,
+                const b2s_pit_label* label, const void* miss, const void* kept) {
+  if (int rc = check_sets(sets, n_sets, cols, n_cols, ts, n)) return rc;
+  if (n_sets > kTrainSets) return b2s_int_fail(B2S_ERR_INVALID, "%d feature sets: a training set joins at most %d", n_sets, kTrainSets);
+  if ((n_sets && !miss) || !kept) return b2s_int_fail(B2S_ERR_INVALID, "null miss / kept counters");
+  if (misaligned(miss, 8) || misaligned(kept, 8)) return b2s_int_fail(B2S_ERR_INVALID, "miss / kept must be 8-byte aligned");
+  for (int s = 0; s < n_sets; ++s)
+    if (n && !sets[s].found) return b2s_int_fail(B2S_ERR_INVALID, "set %d: a training set needs every set's found flags", s);
+  if (label) {
+    int bytes = 0;
+    if (label->set >= 0 && label->set < n_sets && label->out >= 0 && label->out < sets[label->set].n_out)
+      bytes = sets[label->set].outs[label->out].bytes;
+    else if (label->set == -1 && label->out >= 0 && label->out < n_cols)
+      bytes = cols[label->out].bytes;
+    if (!bytes) return b2s_int_fail(B2S_ERR_INVALID, "label (set %d, output %d): no such output or entity column", label->set, label->out);
+    const int k = label->kind;
+    if (k != B2S_PIT_LABEL_FOUND && !(k == B2S_PIT_LABEL_NAN && (bytes == 4 || bytes == 8)) && !(k == B2S_PIT_LABEL_NAT && bytes == 8))
+      return b2s_int_fail(B2S_ERR_INVALID, "label kind %d does not fit a %d-byte column", k, bytes);
+  }
+  return B2S_OK;
+}
+
+// The join of n rows into scratch copies of every output, then the kept rows of each into the caller's arrays (device
+// memory: sets[s].outs[j].out, ts_out, found, cols[c].dst, d_order).  d_miss and *d_kept are written.  ev (may be null):
+// four events recorded before the sort, after it, after the join and after the compaction.
+int train_run(const int64_t* d_ts, int64_t n, const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols, int32_t n_cols,
+              const b2s_pit_label* label, int64_t* d_order, unsigned long long* d_miss, int64_t* d_kept, cudaStream_t st,
+              cudaEvent_t* ev, int* launches) {
+  const int64_t n_tiles = (n + kTile - 1) / kTile;
+  // scratch: one n-row copy of every output, the keep flags, the tile counts and the join's own miss counters
+  struct Move { const void* src; void* dst; int32_t bytes; };
+  std::vector<Move> moves;
+  std::vector<b2s_pit_set> dsets(sets, sets + n_sets);
+  std::vector<std::vector<b2s_pit_out>> douts(n_sets);
+  std::vector<b2s_pit_col> dcols(cols, cols + n_cols);
+  size_t total = 0;
+  auto reserve = [&](size_t bytes) {
+    const size_t off = total;
+    total += (bytes + 255) / 256 * 256;
+    return off;
+  };
+  std::vector<size_t> offs;
+  auto add = [&](void* dst, int32_t bytes) { moves.push_back({nullptr, dst, bytes}); offs.push_back(reserve((size_t)n * bytes)); };
+  for (int s = 0; s < n_sets; ++s) {
+    for (int j = 0; j < sets[s].n_out; ++j) add(sets[s].outs[j].out, sets[s].outs[j].bytes);
+    if (sets[s].ts_out) add(sets[s].ts_out, 8);
+    add(sets[s].found, 1);
+  }
+  for (int c = 0; c < n_cols; ++c) add(cols[c].dst, cols[c].bytes);
+  if (d_order) add(d_order, 8);
+  const size_t keep_off = reserve((size_t)n), count_off = reserve((size_t)n_tiles * 8), miss_off = reserve(8 * (size_t)std::max(n_sets, 1));
+  char* d_scratch = nullptr;
+  SortBufs sb{};
+  int rc = B2S_OK;
+  do {
+    PIT_BREAK(cudaMallocAsync(&d_scratch, total, st));
+    PIT_BREAK(cudaMemsetAsync(d_scratch + miss_off, 0, 8 * (size_t)std::max(n_sets, 1), st));
+    if (n_sets) PIT_BREAK(cudaMemsetAsync(d_miss, 0, 8 * (size_t)n_sets, st));
+    size_t m = 0;
+    for (auto& mv : moves) mv.src = d_scratch + offs[m++];
+    m = 0;
+    for (int s = 0; s < n_sets; ++s) {
+      douts[s].assign(sets[s].outs, sets[s].outs + sets[s].n_out);
+      for (auto& o : douts[s]) o.out = const_cast<void*>(moves[m++].src);
+      dsets[s].outs = douts[s].data();
+      if (sets[s].ts_out) dsets[s].ts_out = static_cast<int64_t*>(const_cast<void*>(moves[m++].src));
+      dsets[s].found = static_cast<uint8_t*>(const_cast<void*>(moves[m++].src));
+    }
+    for (int c = 0; c < n_cols; ++c) dcols[c].dst = const_cast<void*>(moves[m++].src);
+    int64_t* d_order_scratch = d_order ? static_cast<int64_t*>(const_cast<void*>(moves[m++].src)) : nullptr;
+    if (ev) PIT_BREAK(cudaEventRecord(ev[0], st));
+    if (d_ts && (rc = sort_entities(d_ts, n, sb, st))) break;
+    if (d_ts) *launches += 24;
+    if (ev) PIT_BREAK(cudaEventRecord(ev[1], st));
+    if ((rc = launch_join(d_ts ? reinterpret_cast<const int64_t*>(sb.k[0]) : nullptr, d_ts ? sb.v[0] : nullptr, d_order_scratch, 0, n,
+                          dsets.data(), n_sets, dcols.data(), n_cols, reinterpret_cast<unsigned long long*>(d_scratch + miss_off), st,
+                          launches)))
+      break;
+    if (ev) PIT_BREAK(cudaEventRecord(ev[2], st));
+    KeepParams kp{};
+    kp.n_sets = n_sets;
+    kp.n = n;
+    for (int s = 0; s < n_sets; ++s) {
+      kp.found[s] = dsets[s].found;
+      kp.exact[s] = sets[s].asof ? 0 : 1;
+    }
+    if (label) {
+      kp.label_kind = label->kind;
+      if (label->set >= 0) {
+        kp.label_found = dsets[label->set].found;
+        kp.label = douts[label->set][label->out].out;
+        kp.label_bytes = douts[label->set][label->out].bytes;
+      } else {
+        kp.label = dcols[label->out].dst;
+        kp.label_bytes = dcols[label->out].bytes;
+      }
+      if (kp.label_kind == B2S_PIT_LABEL_FOUND) kp.label = nullptr;
+    }
+    uint8_t* d_keep = reinterpret_cast<uint8_t*>(d_scratch + keep_off);
+    int64_t* d_count = reinterpret_cast<int64_t*>(d_scratch + count_off);
+    keep_kernel<<<(unsigned)n_tiles, kTile, 0, st>>>(kp, d_keep, d_count, d_miss);
+    scan_tiles_kernel<<<1, 1024, 0, st>>>(d_count, n_tiles, d_kept);
+    b2s_int_count_launches(2);
+    *launches += 2;
+    for (size_t i = 0; i < moves.size(); i += kScatterCols) {
+      ScatterParams sp{};
+      sp.n = n;
+      for (size_t j = i; j < moves.size() && sp.n_cols < kScatterCols; ++j, ++sp.n_cols) {
+        sp.src[sp.n_cols] = moves[j].src;
+        sp.dst[sp.n_cols] = moves[j].dst;
+        sp.bytes[sp.n_cols] = moves[j].bytes;
+      }
+      scatter_kernel<<<(unsigned)n_tiles, kTile, 0, st>>>(sp, d_keep, d_count);
+      b2s_int_count_launches(1);
+      ++*launches;
+    }
+    if (ev) PIT_BREAK(cudaEventRecord(ev[3], st));
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) rc = b2s_int_fail(B2S_ERR_CUDA, "training-set launch failed: %s", cudaGetErrorString(e));
+  } while (0);
+  free_sort(sb, st);
+  if (d_scratch) cudaFreeAsync(d_scratch, st);
+  return rc;
+}
+
+}  // namespace
+
+extern "C" int b2s_pit_train_device(const int64_t* d_ts, int64_t n, const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols,
+                                    int32_t n_cols, const b2s_pit_label* label, int64_t* d_order, uint64_t* d_miss, int64_t* d_kept,
+                                    void* stream) {
+  try {  // no C++ exception crosses the C boundary
+    if (int rc = check_train(sets, n_sets, cols, n_cols, d_ts, n, label, d_miss, d_kept)) return rc;
+    if (misaligned(d_order, 8)) return b2s_int_fail(B2S_ERR_INVALID, "order must be 8-byte aligned");
+    PIT_TRY(cudaSetDevice(b2s_int_device()));
+    cudaStream_t st = stream ? (cudaStream_t)stream : b2s_int_stream();
+    if (n == 0) {
+      PIT_TRY(cudaMemsetAsync(d_kept, 0, 8, st));
+      if (n_sets) PIT_TRY(cudaMemsetAsync(d_miss, 0, 8 * (size_t)n_sets, st));
+      return B2S_OK;
+    }
+    int launches = 0;
+    return train_run(d_ts, n, sets, n_sets, cols, n_cols, label, d_order, reinterpret_cast<unsigned long long*>(d_miss), d_kept, st,
+                     nullptr, &launches);
+  } catch (const std::exception& e) {
+    return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
+  }
+}
+
+extern "C" int b2s_pit_train_host(const int64_t* ts, int64_t n, const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols,
+                                  int32_t n_cols, const b2s_pit_label* label, int64_t* order, uint64_t* miss, int64_t* kept,
+                                  float* phase_ms, b2s_stats* stats) {
+  try {  // no C++ exception crosses the C boundary
+    if (int rc = check_train(sets, n_sets, cols, n_cols, ts, n, label, miss, kept)) return rc;
+    if (n == 0) {
+      *kept = 0;
+      for (int s = 0; s < n_sets; ++s) miss[s] = 0;
+      if (phase_ms) phase_ms[0] = phase_ms[1] = phase_ms[2] = 0.f;
+      if (stats) memset(stats, 0, sizeof(*stats));
+      return B2S_OK;
+    }
+    PIT_TRY(cudaSetDevice(b2s_int_device()));
+    cudaStream_t st = b2s_int_stream();
+    // one device block: every input, then every output's kept rows (n rows reserved), the counters
+    std::vector<std::pair<const void*, size_t>> ins;  // host source, bytes
+    std::vector<std::pair<void*, size_t>> outs;       // host destination, element bytes
+    std::vector<b2s_pit_set> dsets(sets, sets + n_sets);
+    std::vector<std::vector<b2s_pit_out>> douts(n_sets);
+    std::vector<b2s_pit_col> dcols(cols, cols + n_cols);
+    size_t total = 0;
+    auto reserve = [&](size_t bytes) {
+      const size_t off = total;
+      total += (bytes + 255) / 256 * 256;
+      return off;
+    };
+    std::vector<size_t> in_off, out_off;
+    auto add_in = [&](const void* h, size_t bytes) { ins.push_back({h, bytes}); in_off.push_back(reserve(bytes)); };
+    auto add_out = [&](void* h, size_t elem) { outs.push_back({h, elem}); out_off.push_back(reserve((size_t)n * elem)); };
+    if (ts) add_in(ts, (size_t)n * 8);
+    for (int s = 0; s < n_sets; ++s) {
+      add_in(sets[s].keys, (size_t)n * 8);
+      for (int j = 0; j < sets[s].n_out; ++j) add_out(sets[s].outs[j].out, sets[s].outs[j].bytes);
+      if (sets[s].ts_out) add_out(sets[s].ts_out, 8);
+      add_out(sets[s].found, 1);
+    }
+    for (int c = 0; c < n_cols; ++c) {
+      add_in(cols[c].src, (size_t)n * cols[c].bytes);
+      add_out(cols[c].dst, cols[c].bytes);
+    }
+    if (order) add_out(order, 8);
+    const size_t miss_off = reserve(8 * (size_t)std::max(n_sets, 1)), kept_off = reserve(8);
+    char* d_block = nullptr;
+    int rc = B2S_OK, launches = 0;
+    cudaEvent_t ev[6] = {};
+    do {
+      for (auto& e : ev) PIT_BREAK(cudaEventCreate(&e));
+      if (rc) break;
+      PIT_BREAK(cudaMallocAsync(&d_block, total, st));
+      PIT_BREAK(cudaEventRecord(ev[0], st));
+      for (size_t i = 0; i < ins.size(); ++i) PIT_BREAK(cudaMemcpyAsync(d_block + in_off[i], ins[i].first, ins[i].second, cudaMemcpyHostToDevice, st));
+      if (rc) break;
+      size_t ii = ts ? 1 : 0, oi = 0;
+      for (int s = 0; s < n_sets; ++s) {
+        dsets[s].keys = reinterpret_cast<const int64_t*>(d_block + in_off[ii++]);
+        douts[s].assign(sets[s].outs, sets[s].outs + sets[s].n_out);
+        for (auto& o : douts[s]) o.out = d_block + out_off[oi++];
+        dsets[s].outs = douts[s].data();
+        if (sets[s].ts_out) dsets[s].ts_out = reinterpret_cast<int64_t*>(d_block + out_off[oi++]);
+        dsets[s].found = reinterpret_cast<uint8_t*>(d_block + out_off[oi++]);
+      }
+      for (int c = 0; c < n_cols; ++c) {
+        dcols[c].src = d_block + in_off[ii++];
+        dcols[c].dst = d_block + out_off[oi++];
+      }
+      int64_t* d_order = order ? reinterpret_cast<int64_t*>(d_block + out_off[oi++]) : nullptr;
+      const int64_t* d_ts = ts ? reinterpret_cast<const int64_t*>(d_block + in_off[0]) : nullptr;
+      auto* d_miss = reinterpret_cast<unsigned long long*>(d_block + miss_off);
+      auto* d_kept = reinterpret_cast<int64_t*>(d_block + kept_off);
+      if ((rc = train_run(d_ts, n, dsets.data(), n_sets, dcols.data(), n_cols, label, d_order, d_miss, d_kept, st, ev + 1, &launches))) break;
+      PIT_BREAK(cudaMemcpyAsync(kept, d_kept, 8, cudaMemcpyDeviceToHost, st));
+      if (n_sets) PIT_BREAK(cudaMemcpyAsync(miss, d_miss, 8 * (size_t)n_sets, cudaMemcpyDeviceToHost, st));
+      PIT_BREAK(cudaStreamSynchronize(st));
+      // only the kept rows come back, in ranges of 1 Mi rows
+      const int64_t kRange = 1 << 20;
+      for (int64_t q0 = 0; q0 < *kept && !rc; q0 += kRange) {
+        const int64_t q1 = std::min<int64_t>(*kept, q0 + kRange);
+        for (size_t i = 0; i < outs.size(); ++i) {
+          const size_t el = outs[i].second;
+          PIT_BREAK(cudaMemcpyAsync(static_cast<char*>(outs[i].first) + q0 * el, d_block + out_off[i] + q0 * el, (size_t)(q1 - q0) * el,
+                                    cudaMemcpyDeviceToHost, st));
+        }
+      }
+      if (rc) break;
+      PIT_BREAK(cudaEventRecord(ev[5], st));
+      PIT_BREAK(cudaStreamSynchronize(st));
+      if (phase_ms) {
+        cudaEventElapsedTime(&phase_ms[0], ev[1], ev[2]);  // sort
+        cudaEventElapsedTime(&phase_ms[1], ev[2], ev[3]);  // join
+        cudaEventElapsedTime(&phase_ms[2], ev[3], ev[4]);  // compaction
+      }
+      if (stats) {
+        memset(stats, 0, sizeof(*stats));
+        stats->rows = n;
+        cudaEventElapsedTime(&stats->h2d_ms, ev[0], ev[1]);
+        cudaEventElapsedTime(&stats->kernel_ms, ev[1], ev[4]);
+        cudaEventElapsedTime(&stats->d2h_ms, ev[4], ev[5]);
+        stats->kernels = launches;
+      }
+    } while (0);
+    if (d_block) cudaFreeAsync(d_block, st);
+    cudaStreamSynchronize(st);
+    for (auto& e : ev)
+      if (e) cudaEventDestroy(e);
+    return rc;
+  } catch (const std::exception& e) {
+    return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
+  }
+}

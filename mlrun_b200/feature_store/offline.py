@@ -5,7 +5,10 @@ engine, whose BaseMerger.merge (retrieval/base.py:412-468) merges each feature s
 pandas.merge_asof (retrieval/local_merger.py:29-81).  Storage is out of scope, as for the online table: a feature set's offline
 frame is registered beside its `FeatureSet` mirror (`register_offline_frame`), which builds the set's device index once
 (`b2s_pit_index_*`, include/b200serve.h).  A query sorts the entity rows by timestamp and joins every feature set in one
-`b2s_pit_join_host` call; the host only assembles the columns the reference's frame has, with its names and dtypes.
+`b2s_pit_join_host` call; the host only assembles the columns the reference's frame has, with its names and dtypes.  A
+vector with a `label_feature`, or a query without entity rows (the first feature set's own rows are then the frame the
+others join), runs `b2s_pit_train_host` instead: the same join, then the rows the reference's merge and label `dropna`
+keep are compacted on the device, and only those cross back.
 
 Divergences (DESIGN.md §2): entity rows with equal timestamps keep their input order (pandas' quicksort may reorder them), and
 of feature-set rows with equal (key, timestamp) the last in input order is taken.
@@ -23,6 +26,7 @@ from .keys import _NAT, _UNIT_NS, _encode_keys, _key_kind, _ns
 
 _OFFLINE = {}  # feature-set name -> OfflineSource
 _NAN32 = 0x7FC00000
+_NAN64 = 0x7FF8000000000000
 
 
 class PitIndex:
@@ -88,6 +92,43 @@ def pit_join(ts, sets, cols, with_stats=False):
     return res + (stats.as_dict(),) if with_stats else res
 
 
+def pit_train(ts, sets, cols, label, with_stats=False):
+    """pit_join, keeping only the rows of a training set (b2s_pit_train_host): those every exact-key set matched and, with
+    label = (set index, or -1 for an entity column; output or column index; nat.PIT_LABEL_*), those with a label ->
+    (order, [(outputs, ts_out, found)] per set, permuted cols, misses per set among the rows the exact-key sets before it
+    matched), every array holding the kept rows; with_stats adds {sort_ms, join_ms, compact_ms, kept, **stats}"""
+    lib = nat.init()
+    n = len(ts) if ts is not None else len(cols[0]) if cols else len(sets[0][1]) if sets else 0
+    ts = None if ts is None else np.ascontiguousarray(ts, dtype=np.int64)
+    keep = []  # arrays the descriptors point into
+    c_sets = (nat.PitSet * max(len(sets), 1))()
+    results = []
+    for i, (index, keys, asof, outs) in enumerate(sets):
+        keys = np.ascontiguousarray(keys, dtype=np.int64)
+        arrays = [np.empty(n, dtype=dt) for _w, dt, _m in outs]
+        ts_out, found = np.empty(n, dtype=np.int64), np.empty(n, dtype=np.uint8)
+        descs = (nat.PitOut * max(len(outs), 1))(*[nat.PitOut(w, np.dtype(dt).itemsize, m, a.ctypes.data)
+                                                   for (w, dt, m), a in zip(outs, arrays)])
+        keep += [keys, descs]
+        c_sets[i] = nat.PitSet(index._h, keys.ctypes.data, int(asof), len(outs), descs, ts_out.ctypes.data, found.ctypes.data)
+        results.append((arrays, ts_out, found))
+    srcs = [np.ascontiguousarray(c) for c in cols]
+    dsts = [np.empty_like(c) for c in srcs]
+    c_cols = (nat.PitCol * max(len(cols), 1))(*[nat.PitCol(s.ctypes.data, d.ctypes.data, s.dtype.itemsize) for s, d in zip(srcs, dsts)])
+    c_label = None if label is None else C.byref(nat.PitLabel(*label))
+    order = np.empty(n, dtype=np.int64)
+    miss = np.zeros(max(len(sets), 1), dtype=np.uint64)
+    kept = C.c_int64()
+    phase = (C.c_float * 3)()
+    stats = nat.Stats()
+    nat.check(lib.b2s_pit_train_host(None if ts is None else ts.ctypes.data, n, c_sets, len(sets), c_cols, len(cols), c_label,
+                                     order.ctypes.data, miss.ctypes.data, C.byref(kept), phase, C.byref(stats)))
+    k = kept.value
+    res = (order[:k], [([a[:k] for a in arr], t[:k], f[:k].view(bool)) for arr, t, f in results], [d[:k] for d in dsts],
+           miss[:len(sets)])
+    return res + (dict(sort_ms=phase[0], join_ms=phase[1], compact_ms=phase[2], kept=k, **stats.as_dict()),) if with_stats else res
+
+
 class OfflineSource:
     """one feature set's offline frame, registered with its device index (built once)"""
 
@@ -125,6 +166,8 @@ class OfflineSource:
             s = str(frame[name].dtype)
             if s == "float32":
                 stored, miss = a, _NAN32
+            elif s == "float64":
+                stored, miss = a, _NAN64
             elif s in _INT_DTYPES:
                 stored, miss = a.astype(np.int32), 0
             elif s.startswith("datetime64") and getattr(frame[name].dtype, "tz", None) is None:
@@ -185,10 +228,11 @@ class OfflineVectorResponse:
         return frame
 
 
-def _parse(vector):
-    """features -> {set: [(feature, alias)]} in vector order"""
+def _parse(vector, label=None):
+    """features, then the label feature (set, feature) -> {set: [(feature, alias)]} in vector order; a set's "*" skips its
+    label (feature_vector.py:645-681)"""
     fields = {}
-    for spec in vector.features:
+    for spec in vector.features + ([f"{label[0]}.{label[1]}"] if label else []):
         spec, alias = spec.split(" as ", 1) if " as " in spec else (spec, None)
         if "." not in spec:
             raise MLRunInvalidArgumentError(f"feature {spec!r} must be named <feature set>.<feature>")
@@ -196,12 +240,12 @@ def _parse(vector):
         if name not in _OFFLINE:
             raise MLRunInvalidArgumentError(f"feature set {name!r} has no registered offline frame (register_offline_frame)")
         src = _OFFLINE[name]
-        feats = list(src.features) if feat == "*" else [feat]
+        feats = [f for f in src.features if not (label and (name, f) == label)] if feat == "*" else [feat]
         for f in feats:
             if f not in src.features:
                 raise MLRunInvalidArgumentError(f"feature {f!r} is not in feature set {name}")
             if src.features[f][0] is None:
-                raise LoweringError(f"feature {name}.{f} has dtype {src.features[f][1]}: the device joins float32, (u)int8/16/32, "
+                raise LoweringError(f"feature {name}.{f} has dtype {src.features[f][1]}: the device joins float32, float64, (u)int8/16/32, "
                                     "bool and datetime64 features")
             fields.setdefault(name, []).append((f, alias.strip() if alias else None))
     if not fields:
@@ -209,15 +253,15 @@ def _parse(vector):
     return fields
 
 
-def _restore(values, dtype, found, alive):
-    """a gathered column in the reference's dtype: unchanged when `found` is None or no row in `alive` misses (rows an
-    earlier inner join removed do not count); with a miss, ints become float64 and bool object, with NaN (float32 and
-    datetime64 columns carry NaN / NaT already)"""
+def _restore(values, dtype, found, missed):
+    """a gathered column in the reference's dtype: unchanged when `found` is None or the set missed no row of the merged
+    frame (`missed` False: rows an earlier inner join removed do not count); with a miss, ints become float64 and bool
+    object, with NaN where `found` is False (float32, float64 and datetime64 columns carry NaN / NaT already)"""
     if dtype.startswith("datetime64"):
         return values.view(dtype)
-    if dtype == "float32":
+    if dtype in ("float32", "float64"):
         return values
-    if found is None or found[alive].all():
+    if found is None or not missed:
         return values.astype(dtype)
     out = values.astype(bool).astype(object) if dtype == "bool" else values.astype(np.float64)
     out[~found] = np.nan
@@ -231,6 +275,8 @@ def get_offline_features(feature_vector, entity_rows=None, entity_timestamp_colu
     """feature_store/api.py:99 on the local engine: the training frame of `feature_vector` for `entity_rows`, point-in-time
     correct per feature set.  What the device does not run is refused with LoweringError (there is no pandas fallback)."""
     vector = feature_vector
+    if entity_rows is None and entity_timestamp_column is not None:  # api.py:228-232
+        raise MLRunInvalidArgumentError("entity_timestamp_column param can not be specified without entity_rows param")
     if engine not in (None, "local"):
         raise LoweringError(f"engine {engine!r}: only the local engine's merge runs on the device")
     if start_time is not None or end_time is not None or timestamp_for_filtering is not None:
@@ -243,14 +289,37 @@ def get_offline_features(feature_vector, entity_rows=None, entity_timestamp_colu
         raise LoweringError("drop_columns / update_stats / run_config / spark_service are not lowered")
     if getattr(vector, "join_graph", None) is not None or getattr(vector, "relations", None):
         raise LoweringError("join graphs and relations between feature sets are not lowered: every set joins the entity frame")
+    label = None
     if getattr(vector, "label_feature", None):
-        raise LoweringError("label_feature (dropping rows without a label) is not lowered")
-    if entity_rows is None:
-        raise LoweringError("without entity_rows the feature sets are merged among themselves: not lowered")
+        spec = vector.label_feature.split(" as ", 1)[0].strip()
+        if "." not in spec:
+            raise MLRunInvalidArgumentError(f"label feature {spec!r} must be named <feature set>.<feature>")
+        label = tuple(spec.split(".", 1))
     drop_indexes = not (vector.with_indexes or with_indexes)
-    fields = _parse(vector)
-    if entity_rows.index.names[0]:
-        entity_rows = entity_rows.reset_index()
+    fields = _parse(vector, label)
+    spine_alias = {}
+    entity_less = entity_rows is None
+    if entity_less:
+        # the first set's own rows are the frame the others join (base.py:202-216, 268-285, 427-428): its entities, its
+        # timestamp key and its selected features renamed <feature>_<set>
+        spine_name = next(iter(fields))
+        spine = _OFFLINE[spine_name]
+        for name in fields:
+            if set(_OFFLINE[name].entities) != set(spine.entities):
+                raise LoweringError(f"feature set {name} is keyed by {_OFFLINE[name].entities}, the first set by {spine.entities}: "
+                                    "relations between differently keyed feature sets are not lowered")
+        head = spine.entities + ([spine.timestamp_key] if spine.timestamp_key else [])
+        entity_rows = spine.frame[head + [f for f, _a in fields[spine_name]]].copy(deep=False)
+        entity_rows.columns = head + [f"{f}_{spine_name}" for f, _a in fields[spine_name]]
+        entity_rows = entity_rows.reset_index(drop=True)
+        entity_timestamp_column = spine.timestamp_key
+        spine_alias = dict(([(c, c) for c in head] if not drop_indexes else []) +
+                           [(f"{f}_{spine_name}", a or f) for f, a in fields.pop(spine_name)])
+        index_columns = list(spine.entities)
+    else:
+        index_columns = []
+        if entity_rows.index.names[0]:
+            entity_rows = entity_rows.reset_index()
     n = len(entity_rows)
     names = [str(c) for c in entity_rows.columns]
     if len(set(names)) != len(names):
@@ -298,14 +367,32 @@ def get_offline_features(feature_vector, entity_rows=None, entity_timestamp_colu
         outs = []
         for f, _a in fields[name]:
             word, s, miss = src.features[f]
-            outs.append((word, np.int64 if s.startswith("datetime64") else np.float32 if s == "float32" else np.int32, miss))
+            outs.append((word, np.int64 if s.startswith("datetime64") else np.float64 if s == "float64" else np.float32 if s == "float32"
+                         else np.int32, miss))
         sets.append((src.index, keys, asof, outs))
     dev_cols = [c for c in entity_rows.columns if entity_rows[c].dtype.kind in "iufMb" and getattr(entity_rows[c].dtype, "tz", None) is None
                 and isinstance(entity_rows[c].dtype, np.dtype)]
     arrays = [entity_rows[c].to_numpy() for c in dev_cols]
-    order, joined, permuted, _miss = pit_join(ts_ns, sets, arrays) if n else (
-        np.zeros(0, np.int64), [([np.zeros(0, dt) for _w, dt, _m in s[3]], np.zeros(0, np.int64), np.zeros(0, bool)) for s in sets],
-        [a[:0] for a in arrays], None)
+    train = label is not None or entity_less
+    dev_label = None
+    if label is not None:  # the label's place on the device: an output of its set, or the spine's own column
+        lname, lfeat = label
+        ldtype = _OFFLINE[lname].features[lfeat][1]
+        kind = nat.PIT_LABEL_NAN if ldtype.startswith("float") else nat.PIT_LABEL_NAT if ldtype.startswith("datetime64") else \
+            nat.PIT_LABEL_FOUND
+        if lname in fields:
+            s_i = [name for name, _s, _a in plan].index(lname)
+            dev_label = (s_i, max(j for j, (f, _a) in enumerate(fields[lname]) if f == lfeat), kind)
+        else:
+            dev_label = (-1, dev_cols.index(f"{lfeat}_{lname}"), kind)
+    if not n:
+        order, joined, permuted, miss = (
+            np.zeros(0, np.int64), [([np.zeros(0, dt) for _w, dt, _m in s[3]], np.zeros(0, np.int64), np.zeros(0, bool)) for s in sets],
+            [a[:0] for a in arrays], np.zeros(len(sets), np.uint64))
+    elif train:
+        order, joined, permuted, miss = pit_train(ts_ns, sets, arrays, dev_label)
+    else:
+        order, joined, permuted, _miss = pit_join(ts_ns, sets, arrays)
     moved = dict(zip(dev_cols, permuted))
 
     # the merged frame, set by set (local_merger.py:58-66 / 93-100): right columns after the left ones, the keys and an
@@ -318,9 +405,9 @@ def get_offline_features(feature_vector, entity_rows=None, entity_timestamp_colu
         else:  # strings, categories, objects: permuted on the host in the device's order
             cols[c] = entity_rows[c].take(order).reset_index(drop=True).array
     merge_drop = []
-    alive = np.ones(n, dtype=bool)
-    alias = {}
-    for (name, src, asof), (vals, ts_out, found), (_i, _k, _a, outs) in zip(plan, joined, sets):
+    alive = np.ones(len(order), dtype=bool)
+    alias = dict(spine_alias)
+    for s_i, ((name, src, asof), (vals, ts_out, found), (_i, _k, _a, outs)) in enumerate(zip(plan, joined, sets)):
         head = src.entities + ([src.timestamp_key] if src.timestamp_key else [])
         right = {}
         if src.timestamp_key and not (asof and src.timestamp_key == entity_ts):
@@ -328,7 +415,8 @@ def get_offline_features(feature_vector, entity_rows=None, entity_timestamp_colu
             tdt = np.dtype(f"datetime64[{unit}]") if asof else src.frame[src.timestamp_key].dtype
             right[src.timestamp_key] = np.where(ts_out == _NAT, _NAT, ts_out // _UNIT_NS[np.datetime_data(tdt)[0]]).view(tdt)
         for (f, _a), v in zip(fields[name], vals):
-            right[f"{f}_{name}"] = _restore(v, src.features[f][1], found if asof else None, alive)
+            missed = miss[s_i] > 0 if train else not found[alive].all()
+            right[f"{f}_{name}"] = _restore(v, src.features[f][1], found if asof else None, missed)
         if not asof:
             alive &= found
         for c, v in right.items():
@@ -346,7 +434,8 @@ def get_offline_features(feature_vector, entity_rows=None, entity_timestamp_colu
     drop = []
     for c in ([entity_ts] if drop_indexes and entity_ts else []):
         drop.append(c)
-    index_columns = []
+    if entity_less and drop_indexes:
+        drop += index_columns
     for name, src, _asof in plan:
         if drop_indexes and src.timestamp_key:
             drop.append(src.timestamp_key)
