@@ -22,12 +22,7 @@
 #include "../../include/b200serve.h"
 #include "b2s_internal.h"
 #include "b2s_sort.cuh"
-
-#define AGG_BREAK(expr)                                                                                                  \
-  if (const cudaError_t _e = (expr); _e != cudaSuccess) {                                                              \
-    rc = b2s_int_fail(B2S_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__);       \
-    break;                                                                                                             \
-  }
+#include "b2s_stage.h"
 
 namespace {
 
@@ -289,12 +284,6 @@ __global__ void __launch_bounds__(kThreads) reduce_kernel(const __grid_constant_
   }
 }
 
-int grid_for(int64_t n, int threads) {
-  return (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)b2s_int_sm_count() * 8, (n + threads - 1) / threads));
-}
-
-bool misaligned(const void* ptr, uintptr_t bytes) { return ((uintptr_t)ptr & (bytes - 1)) != 0; }
-
 int n_ops(uint32_t ops) { return __builtin_popcount(ops); }
 
 // levels of the range structure that hold more than one 32-wide block
@@ -342,105 +331,83 @@ int check_specs(const void* keys, const void* ts, int64_t n, const b2s_agg_spec*
   return B2S_OK;
 }
 
-// everything after the checks, over device arrays; *launches grows by the launches made
+// everything after the checks, over device arrays
 int run(const int64_t* d_keys, const int64_t* d_ts, int64_t n, const b2s_agg_spec* specs, int32_t n_specs,
-        const std::vector<const void*>& sources, unsigned long long* d_counters, cudaStream_t st, int* launches, cudaEvent_t sorted) {
-  SortBufs sb{};
-  std::vector<void*> allocs;
-  int rc = B2S_OK;
-  auto alloc = [&](size_t bytes) -> void* {
-    void* p = nullptr;
-    if (cudaMallocAsync(&p, std::max<size_t>(bytes, 8), st) != cudaSuccess) return nullptr;
-    allocs.push_back(p);
-    return p;
-  };
-  do {
-    if ((rc = alloc_sort(sb, n, st))) break;
-    AGG_BREAK(cudaMemcpyAsync(sb.k[0], d_keys, n * 8, cudaMemcpyDeviceToDevice, st));
-    if ((rc = radix_sort(sb, false, n, st))) break;
-    *launches += 24;
-    if (sorted) AGG_BREAK(cudaEventRecord(sorted, st));
-    const int ns = (int)sources.size();
-    std::vector<int> fields(ns, 0);
-    for (int s = 0; s < n_specs; ++s) {
-      const int c = (int)(std::find(sources.begin(), sources.end(), specs[s].src) - sources.begin());
-      fields[c] |= fields_of(specs[s].ops);
-    }
-    PrepParams pp{};
-    pp.keys = sb.k[0];
-    pp.order = sb.v[0];
-    pp.ts = d_ts;
-    pp.n = n;
-    pp.n_src = ns;
-    pp.counters = d_counters;
-    pp.ts_sorted = static_cast<int64_t*>(alloc((size_t)n * 8));
-    pp.run_start = static_cast<int64_t*>(alloc((size_t)n * 8));
-    if (!pp.ts_sorted || !pp.run_start) {
-      rc = b2s_int_fail(B2S_ERR_CUDA, "out of device memory for %lld rows", (long long)n);
-      break;
-    }
-    std::vector<Tree> trees(ns);
-    for (int c = 0; c < ns && !rc; ++c) {
-      Tree& t = trees[c];
-      t = Tree{};
-      t.n = n;
-      t.fields = fields[c];
-      t.n_levels = levels_of(n, t.m);
-      for (const b2s_agg_spec* d = specs; d < specs + n_specs; ++d)
-        if (d->src == sources[c]) pp.kind[c] = d->kind;
-      pp.src[c] = sources[c];
-      pp.x[c] = static_cast<double*>(alloc((size_t)n * 8));
-      t.x = pp.x[c];
-      if (!t.x) rc = b2s_int_fail(B2S_ERR_CUDA, "out of device memory for %lld rows", (long long)n);
-      for (int L = 0; L < t.n_levels && !rc; ++L)
-        for (int f = 0; f < kFields; ++f) {
-          if (!(t.fields & (1 << f))) continue;
-          t.pre[L][f] = static_cast<double*>(alloc((size_t)t.m[L] * 8));
-          t.suf[L][f] = static_cast<double*>(alloc((size_t)t.m[L] * 8));
-          if (!t.pre[L][f] || !t.suf[L][f]) rc = b2s_int_fail(B2S_ERR_CUDA, "out of device memory for the range structure");
-        }
-    }
-    if (rc) break;
-    prep_kernel<<<grid_for(n, kThreads), kThreads, 0, st>>>(pp);
-    b2s_int_count_launches(1);
-    ++*launches;
-    for (int c = 0; c < ns; ++c) {
-      if (!trees[c].fields) continue;  // count / first / last only: no reduce
-      for (int L = 0; L < trees[c].n_levels; ++L) {
-        build_level_kernel<<<grid_for((trees[c].m[L] + 31) / 32 * 32, kThreads), kThreads, 0, st>>>(trees[c], L);
-        b2s_int_count_launches(1);
-        ++*launches;
+        const std::vector<const void*>& sources, unsigned long long* d_counters, cudaStream_t st, Launches& launches, cudaEvent_t sorted) {
+  const int ns = (int)sources.size();
+  std::vector<int> fields(ns, 0);
+  for (int s = 0; s < n_specs; ++s) {
+    const int c = (int)(std::find(sources.begin(), sources.end(), specs[s].src) - sources.begin());
+    fields[c] |= fields_of(specs[s].ops);
+  }
+  // the intermediates in one block: sorted timestamps, run starts, and per source its widened rows and range structure
+  DeviceBlock blk(st);
+  PrepParams pp{};
+  pp.ts = d_ts;
+  pp.n = n;
+  pp.n_src = ns;
+  pp.counters = d_counters;
+  blk.scratch(pp.ts_sorted, (size_t)n * 8);
+  blk.scratch(pp.run_start, (size_t)n * 8);
+  std::vector<Tree> trees(ns);
+  for (int c = 0; c < ns; ++c) {
+    Tree& t = trees[c];
+    t = Tree{};
+    t.n = n;
+    t.fields = fields[c];
+    t.n_levels = levels_of(n, t.m);
+    for (const b2s_agg_spec* d = specs; d < specs + n_specs; ++d)
+      if (d->src == sources[c]) pp.kind[c] = d->kind;
+    pp.src[c] = sources[c];
+    blk.scratch(pp.x[c], (size_t)n * 8);
+    for (int L = 0; L < t.n_levels; ++L)
+      for (int f = 0; f < kFields; ++f) {
+        if (!(t.fields & (1 << f))) continue;
+        blk.scratch(t.pre[L][f], (size_t)t.m[L] * 8);
+        blk.scratch(t.suf[L][f], (size_t)t.m[L] * 8);
       }
+  }
+  SortBufs sb(st);
+  if (int rc = sort_keys(sb, d_keys, n, launches)) return rc;
+  if (sorted) B2S_CUDA_TRY(cudaEventRecord(sorted, st));
+  if (int rc = blk.alloc()) return rc;  // while the sort runs
+  for (int c = 0; c < ns; ++c) trees[c].x = pp.x[c];
+  pp.keys = sb.k[0];
+  pp.order = sb.v[0];
+  prep_kernel<<<grid_for(n, kThreads), kThreads, 0, st>>>(pp);
+  launches.add(1);
+  for (int c = 0; c < ns; ++c) {
+    if (!trees[c].fields) continue;  // count / first / last only: no reduce
+    for (int L = 0; L < trees[c].n_levels; ++L) {
+      build_level_kernel<<<grid_for((trees[c].m[L] + 31) / 32 * 32, kThreads), kThreads, 0, st>>>(trees[c], L);
+      launches.add(1);
     }
-    for (int s = 0; s < n_specs; ++s) {
-      const b2s_agg_spec& d = specs[s];
-      const int c = (int)(std::find(sources.begin(), sources.end(), d.src) - sources.begin());
-      ReduceParams rp{};
-      rp.t = trees[c];
-      rp.t.fields = fields_of(d.ops);  // this aggregation's fields only (the column's structure may hold more)
-      rp.ts = pp.ts_sorted;
-      rp.run_start = pp.run_start;
-      rp.order = sb.v[0];
-      rp.ops = d.ops;
-      rp.n_windows = d.n_windows;
-      rp.period = d.period_ns;
-      for (int w = 0; w < d.n_windows; ++w) rp.window[w] = d.windows_ns[w];
-      int j = 0;
-      for (int bit = 0; bit < 10; ++bit) {
-        if (!(d.ops & (1u << bit))) continue;
-        for (int w = 0; w < d.n_windows; ++w) rp.out[bit][w] = d.outs[j * d.n_windows + w];
-        ++j;
-      }
-      reduce_kernel<<<grid_for(n, kThreads), kThreads, 0, st>>>(rp);
-      b2s_int_count_launches(1);
-      ++*launches;
+  }
+  for (int s = 0; s < n_specs; ++s) {
+    const b2s_agg_spec& d = specs[s];
+    const int c = (int)(std::find(sources.begin(), sources.end(), d.src) - sources.begin());
+    ReduceParams rp{};
+    rp.t = trees[c];
+    rp.t.fields = fields_of(d.ops);  // this aggregation's fields only (the column's structure may hold more)
+    rp.ts = pp.ts_sorted;
+    rp.run_start = pp.run_start;
+    rp.order = sb.v[0];
+    rp.ops = d.ops;
+    rp.n_windows = d.n_windows;
+    rp.period = d.period_ns;
+    for (int w = 0; w < d.n_windows; ++w) rp.window[w] = d.windows_ns[w];
+    int j = 0;
+    for (int bit = 0; bit < 10; ++bit) {
+      if (!(d.ops & (1u << bit))) continue;
+      for (int w = 0; w < d.n_windows; ++w) rp.out[bit][w] = d.outs[j * d.n_windows + w];
+      ++j;
     }
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) rc = b2s_int_fail(B2S_ERR_CUDA, "aggregation launch failed: %s", cudaGetErrorString(e));
-  } while (0);
-  free_sort(sb, st);
-  for (void* p : allocs) cudaFreeAsync(p, st);
-  return rc;
+    reduce_kernel<<<grid_for(n, kThreads), kThreads, 0, st>>>(rp);
+    launches.add(1);
+  }
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return b2s_int_fail(B2S_ERR_CUDA, "aggregation launch failed: %s", cudaGetErrorString(e));
+  return B2S_OK;
 }
 
 }  // namespace
@@ -452,10 +419,10 @@ extern "C" int b2s_agg_run_device(const int64_t* d_keys, const int64_t* d_ts, in
     if (int rc = check_specs(d_keys, d_ts, n, specs, n_specs, d_counters, &sources)) return rc;
     if (n == 0) return B2S_OK;
     if (!b2s_int_inited()) return b2s_int_fail(B2S_ERR_STATE, "b2s_init was not called (no CUDA device: there is no CPU fallback)");
-    SORT_TRY(cudaSetDevice(b2s_int_device()));
+    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
     cudaStream_t st = stream ? (cudaStream_t)stream : b2s_int_stream();
-    int launches = 0;
-    return run(d_keys, d_ts, n, specs, n_specs, sources, reinterpret_cast<unsigned long long*>(d_counters), st, &launches, nullptr);
+    Launches launches;
+    return run(d_keys, d_ts, n, specs, n_specs, sources, reinterpret_cast<unsigned long long*>(d_counters), st, launches, nullptr);
   } catch (const std::exception& e) {
     return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
   }
@@ -475,75 +442,50 @@ extern "C" int b2s_agg_run_host(const int64_t* keys, const int64_t* ts, int64_t 
       return B2S_OK;
     }
     if (!b2s_int_inited()) return b2s_int_fail(B2S_ERR_STATE, "b2s_init was not called (no CUDA device: there is no CPU fallback)");
-    SORT_TRY(cudaSetDevice(b2s_int_device()));
+    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
     cudaStream_t st = b2s_int_stream();
-    // device mirrors: keys, timestamps, each distinct source, each output; one block, each array 256-byte aligned
-    size_t total = 0;
-    auto reserve = [&](size_t bytes) {
-      const size_t off = total;
-      total += (bytes + 255) / 256 * 256;
-      return off;
-    };
-    const size_t cnt_off = reserve(24), keys_off = reserve((size_t)n * 8), ts_off = reserve((size_t)n * 8);
-    std::vector<size_t> src_off;
-    for (const void* s : sources) {
-      (void)s;
-      src_off.push_back(reserve((size_t)n * 4));
-    }
+    Events ev;
+    if (int rc = ev.create(4)) return rc;
+    // device mirrors: the counters, keys, timestamps, each distinct source, each output; one block
+    SyncOnExit done{st};
+    DeviceBlock blk(st);
+    unsigned long long* d_cnt = nullptr;
+    const int64_t* d_keys = nullptr;
+    const int64_t* d_ts = nullptr;
+    blk.scratch(d_cnt, 24);
+    blk.input(d_keys, keys, (size_t)n * 8);
+    blk.input(d_ts, ts, (size_t)n * 8);
+    std::vector<const void*> dsources(sources);
+    for (const void*& src : dsources) blk.input(src, src, (size_t)n * 4);
     std::vector<b2s_agg_spec> dspecs(specs, specs + n_specs);
     std::vector<std::vector<double*>> douts(n_specs);
-    std::vector<std::pair<double*, size_t>> outs;  // host destination, device offset
     for (int s = 0; s < n_specs; ++s) {
-      const int k = n_ops(specs[s].ops) * specs[s].n_windows;
-      for (int j = 0; j < k; ++j) outs.push_back({specs[s].outs[j], reserve((size_t)n * 8)});
+      douts[s].assign(specs[s].outs, specs[s].outs + n_ops(specs[s].ops) * specs[s].n_windows);
+      for (double*& o : douts[s]) blk.output(o, o, 8, n);
+      dspecs[s].outs = douts[s].data();
     }
-    char* d_block = nullptr;
-    int rc = B2S_OK, launches = 0;
-    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
-    do {
-      for (auto& e : ev) AGG_BREAK(cudaEventCreate(&e));
-      if (rc) break;
-      AGG_BREAK(cudaMallocAsync(&d_block, total, st));
-      AGG_BREAK(cudaMemsetAsync(d_block + cnt_off, 0, 24, st));
-      AGG_BREAK(cudaEventRecord(ev[0], st));
-      AGG_BREAK(cudaMemcpyAsync(d_block + keys_off, keys, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-      AGG_BREAK(cudaMemcpyAsync(d_block + ts_off, ts, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-      for (size_t c = 0; c < sources.size(); ++c)
-        AGG_BREAK(cudaMemcpyAsync(d_block + src_off[c], sources[c], (size_t)n * 4, cudaMemcpyHostToDevice, st));
-      if (rc) break;
-      AGG_BREAK(cudaEventRecord(ev[1], st));
-      size_t oi = 0;
-      for (int s = 0; s < n_specs; ++s) {
-        const int c = (int)(std::find(sources.begin(), sources.end(), specs[s].src) - sources.begin());
-        dspecs[s].src = d_block + src_off[c];
-        const int k = n_ops(specs[s].ops) * specs[s].n_windows;
-        for (int j = 0; j < k; ++j) douts[s].push_back(reinterpret_cast<double*>(d_block + outs[oi++].second));
-        dspecs[s].outs = douts[s].data();
-      }
-      std::vector<const void*> dsources;
-      for (size_t c = 0; c < sources.size(); ++c) dsources.push_back(d_block + src_off[c]);
-      rc = run(reinterpret_cast<const int64_t*>(d_block + keys_off), reinterpret_cast<const int64_t*>(d_block + ts_off), n, dspecs.data(),
-               n_specs, dsources, reinterpret_cast<unsigned long long*>(d_block + cnt_off), st, &launches, ev[2]);
-      if (rc) break;
-      AGG_BREAK(cudaEventRecord(ev[3], st));
-      for (const auto& o : outs) AGG_BREAK(cudaMemcpyAsync(o.first, d_block + o.second, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
-      if (rc) break;
-      AGG_BREAK(cudaMemcpyAsync(counters, d_block + cnt_off, 24, cudaMemcpyDeviceToHost, st));
-      AGG_BREAK(cudaStreamSynchronize(st));
-      if (stats) {
-        float sort_ms = 0.f, agg_ms = 0.f;
-        cudaEventElapsedTime(&stats->h2d_ms, ev[0], ev[1]);
-        cudaEventElapsedTime(&sort_ms, ev[1], ev[2]);
-        cudaEventElapsedTime(&agg_ms, ev[2], ev[3]);
-        stats->kernel_ms = sort_ms + agg_ms;
-        stats->kernels = launches;
-      }
-    } while (0);
-    if (d_block) cudaFreeAsync(d_block, st);
-    cudaStreamSynchronize(st);
-    for (auto& e : ev)
-      if (e) cudaEventDestroy(e);
-    return rc;
+    if (int rc = blk.alloc()) return rc;
+    for (int s = 0; s < n_specs; ++s)
+      dspecs[s].src = dsources[std::find(sources.begin(), sources.end(), specs[s].src) - sources.begin()];
+    B2S_CUDA_TRY(cudaMemsetAsync(d_cnt, 0, 24, st));
+    B2S_CUDA_TRY(cudaEventRecord(ev[0], st));
+    if (int rc = blk.upload()) return rc;
+    B2S_CUDA_TRY(cudaEventRecord(ev[1], st));
+    Launches launches;
+    if (int rc = run(d_keys, d_ts, n, dspecs.data(), n_specs, dsources, d_cnt, st, launches, ev[2])) return rc;
+    B2S_CUDA_TRY(cudaEventRecord(ev[3], st));
+    if (int rc = blk.download(0, n, st)) return rc;
+    B2S_CUDA_TRY(cudaMemcpyAsync(counters, d_cnt, 24, cudaMemcpyDeviceToHost, st));
+    B2S_CUDA_TRY(cudaStreamSynchronize(st));
+    if (stats) {
+      float sort_ms = 0.f, agg_ms = 0.f;
+      cudaEventElapsedTime(&stats->h2d_ms, ev[0], ev[1]);
+      cudaEventElapsedTime(&sort_ms, ev[1], ev[2]);
+      cudaEventElapsedTime(&agg_ms, ev[2], ev[3]);
+      stats->kernel_ms = sort_ms + agg_ms;
+      stats->kernels = launches.n;
+    }
+    return B2S_OK;
   } catch (const std::exception& e) {
     return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
   }
@@ -556,30 +498,25 @@ extern "C" int b2s_agg_time_device(const int64_t* d_keys, const int64_t* d_ts, i
     if (int rc = check_specs(d_keys, d_ts, n, specs, n_specs, d_counters, &sources)) return rc;
     if (n_iters < 1 || !sort_ms || !total_ms) return b2s_int_fail(B2S_ERR_INVALID, "n_iters >= 1 and both times are required");
     if (!b2s_int_inited()) return b2s_int_fail(B2S_ERR_STATE, "b2s_init was not called (no CUDA device: there is no CPU fallback)");
-    SORT_TRY(cudaSetDevice(b2s_int_device()));
+    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
     cudaStream_t st = b2s_int_stream();
-    cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
-    int rc = B2S_OK;
     *sort_ms = *total_ms = 0.f;
-    do {
-      for (auto& e : ev) AGG_BREAK(cudaEventCreate(&e));
-      for (int it = 0; it < n_iters && !rc && n; ++it) {
-        int launches = 0;
-        AGG_BREAK(cudaEventRecord(ev[0], st));
-        if ((rc = run(d_keys, d_ts, n, specs, n_specs, sources, reinterpret_cast<unsigned long long*>(d_counters), st, &launches, ev[1]))) break;
-        AGG_BREAK(cudaEventRecord(ev[2], st));
-        AGG_BREAK(cudaEventSynchronize(ev[2]));
-        float a = 0.f, b = 0.f;
-        cudaEventElapsedTime(&a, ev[0], ev[1]);
-        cudaEventElapsedTime(&b, ev[0], ev[2]);
-        *sort_ms += a;
-        *total_ms += b;
-      }
-    } while (0);
-    cudaStreamSynchronize(st);
-    for (auto& e : ev)
-      if (e) cudaEventDestroy(e);
-    return rc;
+    Events ev;
+    if (int rc = ev.create(3)) return rc;
+    SyncOnExit done{st};
+    for (int it = 0; it < n_iters && n; ++it) {
+      Launches launches;
+      B2S_CUDA_TRY(cudaEventRecord(ev[0], st));
+      if (int rc = run(d_keys, d_ts, n, specs, n_specs, sources, reinterpret_cast<unsigned long long*>(d_counters), st, launches, ev[1])) return rc;
+      B2S_CUDA_TRY(cudaEventRecord(ev[2], st));
+      B2S_CUDA_TRY(cudaEventSynchronize(ev[2]));
+      float a = 0.f, b = 0.f;
+      cudaEventElapsedTime(&a, ev[0], ev[1]);
+      cudaEventElapsedTime(&b, ev[0], ev[2]);
+      *sort_ms += a;
+      *total_ms += b;
+    }
+    return B2S_OK;
   } catch (const std::exception& e) {
     return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
   }

@@ -17,13 +17,6 @@
 
 using namespace b2s;
 
-#define COL_TRY(expr)                                                                                       \
-  do {                                                                                                      \
-    cudaError_t _e = (expr);                                                                                \
-    if (_e != cudaSuccess)                                                                                  \
-      return b2s_int_fail(B2S_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
-  } while (0)
-
 struct b2s_cols_s {
   int32_t n_in = 0;
   bool finalized = false;
@@ -220,16 +213,16 @@ extern "C" int b2s_cols_finalize(b2s_cols_t c) {
     if (!b2s_int_inited()) return b2s_int_fail(B2S_ERR_STATE, "b2s_init was not called (no CUDA device: there is no CPU fallback)");
     c->wide_in = std::find(c->in_used.begin(), c->in_used.end(), 2) != c->in_used.end();
     c->wide_out = std::find(c->out_words.begin(), c->out_words.end(), 2) != c->out_words.end();
-    COL_TRY(cudaSetDevice(b2s_int_device()));
-    COL_TRY(cudaMalloc(&c->d_ops, c->ops.size() * sizeof(ColOp)));
-    COL_TRY(cudaMemcpy(c->d_ops, c->ops.data(), c->ops.size() * sizeof(ColOp), cudaMemcpyHostToDevice));
-    COL_TRY(cudaMalloc(&c->d_tab, std::max<size_t>(c->tab.size(), 1) * sizeof(double)));
-    if (!c->tab.empty()) COL_TRY(cudaMemcpy(c->d_tab, c->tab.data(), c->tab.size() * sizeof(double), cudaMemcpyHostToDevice));
-    COL_TRY(cudaMalloc(&c->d_cnt, std::max(c->n_counters, 1) * sizeof(unsigned long long)));
+    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
+    B2S_CUDA_TRY(cudaMalloc(&c->d_ops, c->ops.size() * sizeof(ColOp)));
+    B2S_CUDA_TRY(cudaMemcpy(c->d_ops, c->ops.data(), c->ops.size() * sizeof(ColOp), cudaMemcpyHostToDevice));
+    B2S_CUDA_TRY(cudaMalloc(&c->d_tab, std::max<size_t>(c->tab.size(), 1) * sizeof(double)));
+    if (!c->tab.empty()) B2S_CUDA_TRY(cudaMemcpy(c->d_tab, c->tab.data(), c->tab.size() * sizeof(double), cudaMemcpyHostToDevice));
+    B2S_CUDA_TRY(cudaMalloc(&c->d_cnt, std::max(c->n_counters, 1) * sizeof(unsigned long long)));
     int occ = 0;
-    COL_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, columns_kernel, kColThreads, 0));
+    B2S_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, columns_kernel, kColThreads, 0));
     c->grid = b2s_int_sm_count() * std::max(occ, 1);
-    for (int i = 0; i < 4; ++i) COL_TRY(cudaEventCreate(&c->ev[i]));
+    for (int i = 0; i < 4; ++i) B2S_CUDA_TRY(cudaEventCreate(&c->ev[i]));
     c->finalized = true;
     return B2S_OK;
   } catch (const std::exception& e) {
@@ -296,7 +289,7 @@ extern "C" int b2s_cols_run_device(b2s_cols_t c, const void* d_in, int64_t in_sl
     if (n_rows == 0) return B2S_OK;
     if (c->n_counters && !d_counters) return b2s_int_fail(B2S_ERR_INVALID, "the plan has %d counters: pass a device array", c->n_counters);
     if (int rc = check_device_buffers(c, d_in, d_out, d_counters)) return rc;
-    COL_TRY(cudaSetDevice(b2s_int_device()));
+    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
     return launch_cols(c, d_in, in_slot_stride, n_rows, d_out, out_slot_stride, (unsigned long long*)d_counters,
                        stream ? (cudaStream_t)stream : b2s_int_stream());
   } catch (const std::exception& e) {
@@ -314,15 +307,15 @@ extern "C" int b2s_cols_time_device(b2s_cols_t c, const void* const* d_in, int32
     if (c->n_counters && !d_counters) return b2s_int_fail(B2S_ERR_INVALID, "the plan has %d counters: pass a device array", c->n_counters);
     for (int i = 0; i < n_bufs; ++i)
       if (int rc = check_device_buffers(c, d_in[i], d_out, d_counters)) return rc;
-    COL_TRY(cudaSetDevice(b2s_int_device()));
+    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
     cudaStream_t st = b2s_int_stream();
     std::lock_guard<std::mutex> lk(c->mu);
-    COL_TRY(cudaEventRecord(c->ev[0], st));
+    B2S_CUDA_TRY(cudaEventRecord(c->ev[0], st));
     for (int i = 0; i < n_iters; ++i)
       if (int rc = launch_cols(c, d_in[i % n_bufs], in_slot_stride, n_rows, d_out, out_slot_stride, (unsigned long long*)d_counters, st)) return rc;
-    COL_TRY(cudaEventRecord(c->ev[1], st));
-    COL_TRY(cudaStreamSynchronize(st));
-    COL_TRY(cudaEventElapsedTime(total_ms, c->ev[0], c->ev[1]));
+    B2S_CUDA_TRY(cudaEventRecord(c->ev[1], st));
+    B2S_CUDA_TRY(cudaStreamSynchronize(st));
+    B2S_CUDA_TRY(cudaEventElapsedTime(total_ms, c->ev[0], c->ev[1]));
     return B2S_OK;
   } catch (const std::exception& e) {
     return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
@@ -338,14 +331,14 @@ extern "C" int b2s_cols_run_host(b2s_cols_t c, const void* const* h_in_slots, in
     for (int i = 0; i < c->n_counters; ++i) counters[i] = 0;
     if (n_rows == 0) return B2S_OK;
     std::lock_guard<std::mutex> lk(c->mu);
-    COL_TRY(cudaSetDevice(b2s_int_device()));
+    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
     const int64_t stride = ((n_rows * 4 + 255) / 256) * 256;
     const size_t n_out = c->out_words.size();
     if (n_rows > c->cap_rows) {
       if (c->d_in) { cudaFree(c->d_in); cudaFree(c->d_out); c->d_in = c->d_out = nullptr; }
       c->cap_rows = 0;
-      COL_TRY(cudaMalloc(&c->d_in, (size_t)stride * c->n_in));
-      COL_TRY(cudaMalloc(&c->d_out, (size_t)stride * n_out));
+      B2S_CUDA_TRY(cudaMalloc(&c->d_in, (size_t)stride * c->n_in));
+      B2S_CUDA_TRY(cudaMalloc(&c->d_out, (size_t)stride * n_out));
       c->cap_rows = n_rows;
     }
     cudaStream_t st = b2s_int_stream();
@@ -360,16 +353,16 @@ extern "C" int b2s_cols_run_host(b2s_cols_t c, const void* const* h_in_slots, in
       cudaStream_t cs = b2s_int_copy_stream();
       while ((int)c->chunk_ev.size() < n_chunks) {
         cudaEvent_t e;
-        COL_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        B2S_CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
         c->chunk_ev.push_back(e);
       }
       for (int s = 0; s < c->n_in; ++s)
         if (c->in_used[s] && !h_in_slots[s]) return b2s_int_fail(B2S_ERR_INVALID, "input slot %d is read by the plan but its pointer is NULL", s);
       for (size_t s = 0; s < n_out; ++s)
         if (c->out_words[s] && !h_out_slots[s]) return b2s_int_fail(B2S_ERR_INVALID, "output slot %zu has no destination", s);
-      if (c->n_counters) COL_TRY(cudaMemsetAsync(c->d_cnt, 0, c->n_counters * sizeof(unsigned long long), st));
-      COL_TRY(cudaEventRecord(c->ev[0], st));
-      COL_TRY(cudaStreamWaitEvent(cs, c->ev[0], 0));  // whatever ran on the library stream before is done with d_in
+      if (c->n_counters) B2S_CUDA_TRY(cudaMemsetAsync(c->d_cnt, 0, c->n_counters * sizeof(unsigned long long), st));
+      B2S_CUDA_TRY(cudaEventRecord(c->ev[0], st));
+      B2S_CUDA_TRY(cudaStreamWaitEvent(cs, c->ev[0], 0));  // whatever ran on the library stream before is done with d_in
       // Columns that sit at a constant pitch in host memory (views of one pinned block: columnar.pinned_columns, the
       // ColumnBatch of the results) cross PCIe as ONE 2-D copy per row range and run of columns instead of one copy per
       // column: ~570 copies of 256 KB per range become a handful (copy-engine set-up and driver calls were 2/3 of the time).
@@ -406,11 +399,11 @@ extern "C" int b2s_cols_run_host(b2s_cols_t c, const void* const* h_in_slots, in
         for (const Run& r : in_runs) {
           char* dst = c->d_in + (size_t)r.s0 * stride + (size_t)r0 * r.w;
           const char* src = (const char*)h_in_slots[r.s0] + (size_t)r0 * r.w;
-          if (r.count == 1) COL_TRY(cudaMemcpyAsync(dst, src, (size_t)nr * r.w, cudaMemcpyHostToDevice, cs));
-          else COL_TRY(cudaMemcpy2DAsync(dst, r.dpitch, src, r.hpitch, (size_t)nr * r.w, (size_t)r.count, cudaMemcpyHostToDevice, cs));
+          if (r.count == 1) B2S_CUDA_TRY(cudaMemcpyAsync(dst, src, (size_t)nr * r.w, cudaMemcpyHostToDevice, cs));
+          else B2S_CUDA_TRY(cudaMemcpy2DAsync(dst, r.dpitch, src, r.hpitch, (size_t)nr * r.w, (size_t)r.count, cudaMemcpyHostToDevice, cs));
         }
-        COL_TRY(cudaEventRecord(c->chunk_ev[k], cs));
-        COL_TRY(cudaStreamWaitEvent(st, c->chunk_ev[k], 0));
+        B2S_CUDA_TRY(cudaEventRecord(c->chunk_ev[k], cs));
+        B2S_CUDA_TRY(cudaStreamWaitEvent(st, c->chunk_ev[k], 0));
         if (int rc = launch_cols(c, c->d_in, stride, nr, c->d_out, stride, c->d_cnt, st, r0)) {
           cudaStreamSynchronize(cs);
           cudaStreamSynchronize(st);
@@ -419,14 +412,14 @@ extern "C" int b2s_cols_run_host(b2s_cols_t c, const void* const* h_in_slots, in
         for (const Run& r : out_runs) {
           char* dst = (char*)h_out_slots[r.s0] + (size_t)r0 * r.w;
           const char* src = c->d_out + (size_t)r.s0 * stride + (size_t)r0 * r.w;
-          if (r.count == 1) COL_TRY(cudaMemcpyAsync(dst, src, (size_t)nr * r.w, cudaMemcpyDeviceToHost, st));
-          else COL_TRY(cudaMemcpy2DAsync(dst, r.hpitch, src, r.dpitch, (size_t)nr * r.w, (size_t)r.count, cudaMemcpyDeviceToHost, st));
+          if (r.count == 1) B2S_CUDA_TRY(cudaMemcpyAsync(dst, src, (size_t)nr * r.w, cudaMemcpyDeviceToHost, st));
+          else B2S_CUDA_TRY(cudaMemcpy2DAsync(dst, r.hpitch, src, r.dpitch, (size_t)nr * r.w, (size_t)r.count, cudaMemcpyDeviceToHost, st));
         }
       }
-      if (c->n_counters) COL_TRY(cudaMemcpyAsync(counters, c->d_cnt, c->n_counters * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-      COL_TRY(cudaEventRecord(c->ev[3], st));
-      COL_TRY(cudaStreamSynchronize(st));
-      COL_TRY(cudaStreamSynchronize(cs));
+      if (c->n_counters) B2S_CUDA_TRY(cudaMemcpyAsync(counters, c->d_cnt, c->n_counters * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+      B2S_CUDA_TRY(cudaEventRecord(c->ev[3], st));
+      B2S_CUDA_TRY(cudaStreamSynchronize(st));
+      B2S_CUDA_TRY(cudaStreamSynchronize(cs));
       if (stats) {
         memset(stats, 0, sizeof(*stats));
         stats->rows = n_rows;
@@ -435,24 +428,24 @@ extern "C" int b2s_cols_run_host(b2s_cols_t c, const void* const* h_in_slots, in
       }
       return B2S_OK;
     }
-    COL_TRY(cudaEventRecord(c->ev[0], st));
+    B2S_CUDA_TRY(cudaEventRecord(c->ev[0], st));
     for (int s = 0; s < c->n_in; ++s) {
       if (!c->in_used[s]) continue;
       if (!h_in_slots[s]) return b2s_int_fail(B2S_ERR_INVALID, "input slot %d is read by the plan but its pointer is NULL", s);
-      COL_TRY(cudaMemcpyAsync(c->d_in + (size_t)s * stride, h_in_slots[s], (size_t)n_rows * 4 * c->in_used[s], cudaMemcpyHostToDevice, st));
+      B2S_CUDA_TRY(cudaMemcpyAsync(c->d_in + (size_t)s * stride, h_in_slots[s], (size_t)n_rows * 4 * c->in_used[s], cudaMemcpyHostToDevice, st));
     }
-    if (c->n_counters) COL_TRY(cudaMemsetAsync(c->d_cnt, 0, c->n_counters * sizeof(unsigned long long), st));
-    COL_TRY(cudaEventRecord(c->ev[1], st));
+    if (c->n_counters) B2S_CUDA_TRY(cudaMemsetAsync(c->d_cnt, 0, c->n_counters * sizeof(unsigned long long), st));
+    B2S_CUDA_TRY(cudaEventRecord(c->ev[1], st));
     if (int rc = launch_cols(c, c->d_in, stride, n_rows, c->d_out, stride, c->d_cnt, st)) return rc;
-    COL_TRY(cudaEventRecord(c->ev[2], st));
+    B2S_CUDA_TRY(cudaEventRecord(c->ev[2], st));
     for (size_t s = 0; s < n_out; ++s) {
       if (!c->out_words[s]) continue;  // second half of an 8-byte column
       if (!h_out_slots[s]) return b2s_int_fail(B2S_ERR_INVALID, "output slot %zu has no destination", s);
-      COL_TRY(cudaMemcpyAsync(h_out_slots[s], c->d_out + s * (size_t)stride, (size_t)n_rows * 4 * c->out_words[s], cudaMemcpyDeviceToHost, st));
+      B2S_CUDA_TRY(cudaMemcpyAsync(h_out_slots[s], c->d_out + s * (size_t)stride, (size_t)n_rows * 4 * c->out_words[s], cudaMemcpyDeviceToHost, st));
     }
-    if (c->n_counters) COL_TRY(cudaMemcpyAsync(counters, c->d_cnt, c->n_counters * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-    COL_TRY(cudaEventRecord(c->ev[3], st));
-    COL_TRY(cudaStreamSynchronize(st));
+    if (c->n_counters) B2S_CUDA_TRY(cudaMemcpyAsync(counters, c->d_cnt, c->n_counters * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    B2S_CUDA_TRY(cudaEventRecord(c->ev[3], st));
+    B2S_CUDA_TRY(cudaStreamSynchronize(st));
     if (stats) {
       memset(stats, 0, sizeof(*stats));
       stats->rows = n_rows;

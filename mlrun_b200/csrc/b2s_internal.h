@@ -2,6 +2,9 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
+#include <cstdint>
+
 #define B2S_HIDDEN __attribute__((visibility("hidden")))
 
 B2S_HIDDEN int b2s_int_fail(int code, const char* fmt, ...);  // sets b2s_last_error(), returns code
@@ -11,6 +14,22 @@ B2S_HIDDEN int b2s_int_sm_count();
 B2S_HIDDEN cudaStream_t b2s_int_stream();                      // the library stream
 B2S_HIDDEN cudaStream_t b2s_int_copy_stream();                 // the library's copy stream (pipelined host runs)
 B2S_HIDDEN void b2s_int_count_launches(int n);
+
+// return B2S_ERR_CUDA (with the failed call, the CUDA error and the source line in b2s_last_error()) when expr fails
+#define B2S_CUDA_TRY(expr)                                                                                             \
+  do {                                                                                                                 \
+    cudaError_t _e = (expr);                                                                                           \
+    if (_e != cudaSuccess)                                                                                             \
+      return b2s_int_fail(B2S_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
+  } while (0)
+
+static inline bool misaligned(const void* ptr, uintptr_t bytes) { return ((uintptr_t)ptr & (bytes - 1)) != 0; }
+
+// blocks of a grid-stride launch over n items: enough to fill the device (8 per SM), no more than the items need
+static inline int grid_for(int64_t n, int threads) {
+  return (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)b2s_int_sm_count() * 8, (n + threads - 1) / threads));
+}
+
 struct b2s_plan_s;
 B2S_HIDDEN int b2s_int_plan_shape(b2s_plan_s* plan, int* n_in, int* out_cols);  // B2S_ERR_STATE unless finalized
 

@@ -21,21 +21,7 @@
 #include "b2s_internal.h"
 #include "b2s_pit.cuh"
 #include "b2s_sort.cuh"
-
-#define PIT_TRY(expr)                                                                                                  \
-  do {                                                                                                                 \
-    cudaError_t _e = (expr);                                                                                           \
-    if (_e != cudaSuccess)                                                                                             \
-      return b2s_int_fail(B2S_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
-  } while (0)
-
-// inside a do { ... } while (0) block whose buffers are freed after it: record the failure in rc and leave the block (from
-// a loop nested in the block it leaves the loop only, which is followed by `if (rc) break;`)
-#define PIT_BREAK(expr)                                                                                                  \
-  if (const cudaError_t _e = (expr); _e != cudaSuccess) {                                                              \
-    rc = b2s_int_fail(B2S_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__);       \
-    break;                                                                                                             \
-  }
+#include "b2s_stage.h"
 
 using namespace b2s_pit;
 using b2s::TableSlot;
@@ -161,12 +147,6 @@ __global__ void __launch_bounds__(256) pit_join_kernel(const __grid_constant__ J
   if (threadIdx.x < p.n_sets && s_miss[threadIdx.x]) atomicAdd(&p.miss[threadIdx.x], s_miss[threadIdx.x]);
 }
 
-int grid_for(int64_t n, int threads) {
-  return (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)b2s_int_sm_count() * 8, (n + threads - 1) / threads));
-}
-
-bool misaligned(const void* ptr, uintptr_t bytes) { return ((uintptr_t)ptr & (bytes - 1)) != 0; }
-
 }  // namespace
 
 struct b2s_pit_s {
@@ -202,64 +182,52 @@ static int index_build(b2s_pit_s* ix, const int64_t* keys, const int64_t* ts, in
     lp.row_words += lp.words[c];
   }
   ix->row_words = lp.row_words;
-  SortBufs sb{};
-  int64_t* d_keys = nullptr;
-  int64_t* d_ts_in = nullptr;
-  std::vector<void*> d_cols(n_cols, nullptr);
+  // the temporaries in one block: keys and timestamps in input order, the columns, the counters
+  SyncOnExit done{st};
+  DeviceBlock blk(st);
+  const int64_t* d_keys = nullptr;
+  const int64_t* d_ts_in = nullptr;
   unsigned long long* d_stat = nullptr;  // [0] runs, [1] longest run
-  int rc = B2S_OK;
-  do {
-    if ((rc = alloc_sort(sb, n, st))) break;
-    PIT_BREAK(cudaMallocAsync(&d_keys, n * 8, st));
-    PIT_BREAK(cudaMallocAsync(&d_ts_in, n * 8, st));
-    PIT_BREAK(cudaMallocAsync(&d_stat, 16, st));
-    PIT_BREAK(cudaMemsetAsync(d_stat, 0, 16, st));
-    PIT_BREAK(cudaMemcpyAsync(d_keys, keys, n * 8, cudaMemcpyHostToDevice, st));
-    PIT_BREAK(cudaMemcpyAsync(d_ts_in, ts, n * 8, cudaMemcpyHostToDevice, st));
-    PIT_BREAK(cudaMemcpyAsync(sb.k[0], ts, n * 8, cudaMemcpyHostToDevice, st));
-    for (int c = 0; c < n_cols; ++c) {
-      PIT_BREAK(cudaMallocAsync(&d_cols[c], (size_t)n * col_bytes[c], st));
-      PIT_BREAK(cudaMemcpyAsync(d_cols[c], cols[c], (size_t)n * col_bytes[c], cudaMemcpyHostToDevice, st));
-      lp.cols[c] = d_cols[c];
-    }
-    if (rc) break;
-    // by timestamp, then (stably) by key: rows ordered by (key, timestamp), equal pairs in input order
-    if ((rc = radix_sort(sb, false, n, st))) break;
-    const int g = grid_for(n, 256);
-    gather_keys_kernel<<<g, 256, 0, st>>>(d_keys, sb.v[0], sb.k[0], n);
-    if ((rc = radix_sort(sb, true, n, st))) break;
-    PIT_BREAK(cudaMalloc(&ix->d_ts, n * 8));
-    PIT_BREAK(cudaMalloc(&ix->d_rows, (size_t)n * std::max(lp.row_words, 1) * 4));
-    gather_keys_kernel<<<g, 256, 0, st>>>(d_ts_in, sb.v[0], reinterpret_cast<uint64_t*>(ix->d_ts), n);
-    layout_rows_kernel<<<g, 256, 0, st>>>(lp, sb.v[0], ix->d_rows, n);
-    count_runs_kernel<<<g, 256, 0, st>>>(sb.k[0], n, d_stat);
-    b2s_int_count_launches(4);
-    unsigned long long runs = 0;
-    PIT_BREAK(cudaMemcpyAsync(&runs, d_stat, 8, cudaMemcpyDeviceToHost, st));
-    PIT_BREAK(cudaStreamSynchronize(st));
-    uint64_t cap = 16;
-    while (cap < runs * 2) cap <<= 1;  // load factor <= 0.5: table_find's walk always meets an empty slot
-    ix->cap = cap;
-    ix->n_keys = (int64_t)runs;
-    PIT_BREAK(cudaMalloc(&ix->d_slots, cap * sizeof(TableSlot)));
-    PIT_BREAK(cudaMemsetAsync(ix->d_slots, 0xff, cap * sizeof(TableSlot), st));  // row -1: empty
-    insert_runs_kernel<<<g, 256, 0, st>>>(sb.k[0], n, ix->d_slots, cap - 1, d_stat + 1);
-    b2s_int_count_launches(1);
-    unsigned long long longest = 0;
-    PIT_BREAK(cudaMemcpyAsync(&longest, d_stat + 1, 8, cudaMemcpyDeviceToHost, st));
-    PIT_BREAK(cudaStreamSynchronize(st));
-    ix->longest_run = (int64_t)longest;
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) rc = b2s_int_fail(B2S_ERR_CUDA, "index build failed: %s", cudaGetErrorString(e));
-  } while (0);
-  free_sort(sb, st);
-  if (d_keys) cudaFreeAsync(d_keys, st);
-  if (d_ts_in) cudaFreeAsync(d_ts_in, st);
-  if (d_stat) cudaFreeAsync(d_stat, st);
-  for (void* p : d_cols)
-    if (p) cudaFreeAsync(p, st);
-  cudaStreamSynchronize(st);
-  return rc;
+  blk.input(d_keys, keys, (size_t)n * 8);
+  blk.input(d_ts_in, ts, (size_t)n * 8);
+  blk.scratch(d_stat, 16);
+  for (int c = 0; c < n_cols; ++c) blk.input(lp.cols[c], cols[c], (size_t)n * col_bytes[c]);
+  SortBufs sb(st);
+  if (int rc = sb.alloc(n)) return rc;
+  if (int rc = blk.alloc()) return rc;
+  B2S_CUDA_TRY(cudaMemsetAsync(d_stat, 0, 16, st));
+  if (int rc = blk.upload()) return rc;
+  B2S_CUDA_TRY(cudaMemcpyAsync(sb.k[0], ts, n * 8, cudaMemcpyHostToDevice, st));
+  // by timestamp, then (stably) by key: rows ordered by (key, timestamp), equal pairs in input order
+  Launches launches;
+  if (int rc = radix_sort(sb, false, n, launches)) return rc;
+  const int g = grid_for(n, 256);
+  gather_keys_kernel<<<g, 256, 0, st>>>(d_keys, sb.v[0], sb.k[0], n);
+  if (int rc = radix_sort(sb, true, n, launches)) return rc;
+  B2S_CUDA_TRY(cudaMalloc(&ix->d_ts, n * 8));
+  B2S_CUDA_TRY(cudaMalloc(&ix->d_rows, (size_t)n * std::max(lp.row_words, 1) * 4));
+  gather_keys_kernel<<<g, 256, 0, st>>>(d_ts_in, sb.v[0], reinterpret_cast<uint64_t*>(ix->d_ts), n);
+  layout_rows_kernel<<<g, 256, 0, st>>>(lp, sb.v[0], ix->d_rows, n);
+  count_runs_kernel<<<g, 256, 0, st>>>(sb.k[0], n, d_stat);
+  launches.add(4);
+  unsigned long long runs = 0;
+  B2S_CUDA_TRY(cudaMemcpyAsync(&runs, d_stat, 8, cudaMemcpyDeviceToHost, st));
+  B2S_CUDA_TRY(cudaStreamSynchronize(st));
+  uint64_t cap = 16;
+  while (cap < runs * 2) cap <<= 1;  // load factor <= 0.5: table_find's walk always meets an empty slot
+  ix->cap = cap;
+  ix->n_keys = (int64_t)runs;
+  B2S_CUDA_TRY(cudaMalloc(&ix->d_slots, cap * sizeof(TableSlot)));
+  B2S_CUDA_TRY(cudaMemsetAsync(ix->d_slots, 0xff, cap * sizeof(TableSlot), st));  // row -1: empty
+  insert_runs_kernel<<<g, 256, 0, st>>>(sb.k[0], n, ix->d_slots, cap - 1, d_stat + 1);
+  launches.add(1);
+  unsigned long long longest = 0;
+  B2S_CUDA_TRY(cudaMemcpyAsync(&longest, d_stat + 1, 8, cudaMemcpyDeviceToHost, st));
+  B2S_CUDA_TRY(cudaStreamSynchronize(st));
+  ix->longest_run = (int64_t)longest;
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return b2s_int_fail(B2S_ERR_CUDA, "index build failed: %s", cudaGetErrorString(e));
+  return B2S_OK;
 }
 
 extern "C" int b2s_pit_index_create(const int64_t* keys, const int64_t* ts_ns, int64_t n_rows, const void* const* cols,
@@ -270,7 +238,7 @@ extern "C" int b2s_pit_index_create(const int64_t* keys, const int64_t* ts_ns, i
     for (int c = 0; c < n_cols; ++c)
       if (!cols[c] || (col_bytes[c] != 4 && col_bytes[c] != 8)) return b2s_int_fail(B2S_ERR_INVALID, "column %d: null or not 4 / 8 bytes wide", c);
     if (!b2s_int_inited()) return b2s_int_fail(B2S_ERR_STATE, "b2s_init was not called (no CUDA device: there is no CPU fallback)");
-    PIT_TRY(cudaSetDevice(b2s_int_device()));
+    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
     auto* ix = new b2s_pit_s();
     ix->n_rows = n_rows;
     if (int rc = index_build(ix, keys, ts_ns, n_rows, cols, col_bytes, n_cols, b2s_int_stream())) {
@@ -326,10 +294,10 @@ static int check_sets(const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col
 }
 
 // sort (when ts is given) and launch the join over sorted positions [q0, q1); sets / cols hold device pointers.  Sets and
-// columns beyond one launch's parameter block go to further launches over the same range.  *launches grows by the launches made.
+// columns beyond one launch's parameter block go to further launches over the same range.
 static int launch_join(const int64_t* d_sorted_ts, const uint32_t* d_order, int64_t* d_order_out, int64_t q0, int64_t q1,
                        const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols, int32_t n_cols, unsigned long long* d_miss,
-                       cudaStream_t st, int* launches) {
+                       cudaStream_t st, Launches& launches) {
   int s = 0, c = 0;
   bool first = true;
   while (first || s < n_sets || c < n_cols) {
@@ -365,8 +333,7 @@ static int launch_join(const int64_t* d_sorted_ts, const uint32_t* d_order, int6
     first = false;
     if (q1 > q0) {
       pit_join_kernel<<<grid_for(q1 - q0, 256), 256, 0, st>>>(p);
-      b2s_int_count_launches(1);
-      ++*launches;
+      launches.add(1);
     }
   }
   const cudaError_t e = cudaGetLastError();
@@ -374,11 +341,43 @@ static int launch_join(const int64_t* d_sorted_ts, const uint32_t* d_order, int6
   return B2S_OK;
 }
 
-static int sort_entities(const int64_t* d_ts, int64_t n, SortBufs& sb, cudaStream_t st) {
-  if (int rc = alloc_sort(sb, n, st)) return rc;
-  PIT_TRY(cudaMemcpyAsync(sb.k[0], d_ts, n * 8, cudaMemcpyDeviceToDevice, st));
-  return radix_sort(sb, false, n, st);
-}
+// Device copies of a call's descriptors over n entity rows.  Every output (each set's outputs, ts_out and found, each
+// entity column's destination, the order) and, when `inputs`, every input (the timestamps, each set's keys, each entity
+// column's source) gets a region of blk; blk.outputs() lists the outputs with the pointers their regions replace as
+// destinations.  So do the join's miss counters.  The copies point at the regions once blk is allocated.
+namespace {
+struct DeviceDescs {
+  DeviceDescs(DeviceBlock& blk, int64_t n, bool inputs, const int64_t* ts, const b2s_pit_set* sets, int32_t n_sets,
+              const b2s_pit_col* cols, int32_t n_cols, int64_t* order)
+      : ts(ts), sets(sets, sets + n_sets), outs(n_sets), cols(cols, cols + n_cols), order(order) {
+    if (inputs && ts) blk.input(this->ts, ts, (size_t)n * 8);
+    for (int s = 0; s < n_sets; ++s) {
+      b2s_pit_set& d = this->sets[s];
+      if (inputs) blk.input(d.keys, d.keys, (size_t)n * 8);
+      outs[s].assign(d.outs, d.outs + d.n_out);
+      d.outs = outs[s].data();
+      for (b2s_pit_out& o : outs[s]) blk.output(o.out, o.out, o.bytes, n);
+      if (d.ts_out) blk.output(d.ts_out, d.ts_out, 8, n);
+      if (d.found) blk.output(d.found, d.found, 1, n);
+    }
+    for (b2s_pit_col& c : this->cols) {
+      if (inputs) blk.input(c.src, c.src, (size_t)n * c.bytes);
+      blk.output(c.dst, c.dst, c.bytes, n);
+    }
+    if (order) blk.output(this->order, order, 8, n);
+    blk.scratch(miss, 8 * (size_t)std::max(n_sets, 1));
+  }
+  DeviceDescs(const DeviceDescs&) = delete;
+  DeviceDescs& operator=(const DeviceDescs&) = delete;
+
+  const int64_t* ts;
+  std::vector<b2s_pit_set> sets;
+  std::vector<std::vector<b2s_pit_out>> outs;
+  std::vector<b2s_pit_col> cols;
+  int64_t* order;
+  unsigned long long* miss = nullptr;  // [max(n_sets, 1)]
+};
+}  // namespace
 
 extern "C" int b2s_pit_join_device(const int64_t* d_ts, int64_t n, const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols,
                                    int32_t n_cols, int64_t* d_order, uint64_t* d_miss, void* stream) {
@@ -387,16 +386,13 @@ extern "C" int b2s_pit_join_device(const int64_t* d_ts, int64_t n, const b2s_pit
     if (n_sets && !d_miss) return b2s_int_fail(B2S_ERR_INVALID, "null miss counters");
     if (misaligned(d_order, 8) || misaligned(d_miss, 8)) return b2s_int_fail(B2S_ERR_INVALID, "order / miss must be 8-byte aligned");
     if (n == 0) return B2S_OK;
-    PIT_TRY(cudaSetDevice(b2s_int_device()));
+    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
     cudaStream_t st = stream ? (cudaStream_t)stream : b2s_int_stream();
-    SortBufs sb{};
-    int rc = B2S_OK, launches = 0;
-    if (d_ts) rc = sort_entities(d_ts, n, sb, st);
-    if (!rc)
-      rc = launch_join(d_ts ? reinterpret_cast<const int64_t*>(sb.k[0]) : nullptr, d_ts ? sb.v[0] : nullptr, d_order, 0, n, sets, n_sets,
-                       cols, n_cols, reinterpret_cast<unsigned long long*>(d_miss), st, &launches);
-    free_sort(sb, st);
-    return rc;
+    SortBufs sb(st);  // stays empty without timestamps: the join then reads no sorted order
+    Launches launches;
+    if (int rc = d_ts ? sort_keys(sb, d_ts, n, launches) : B2S_OK) return rc;
+    return launch_join(reinterpret_cast<const int64_t*>(sb.k[0]), sb.v[0], d_order, 0, n, sets, n_sets, cols, n_cols,
+                       reinterpret_cast<unsigned long long*>(d_miss), st, launches);
   } catch (const std::exception& e) {
     return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
   }
@@ -411,110 +407,48 @@ extern "C" int b2s_pit_join_host(const int64_t* ts, int64_t n, const b2s_pit_set
       for (int s = 0; s < n_sets; ++s) miss[s] = 0;
       return B2S_OK;
     }
-    PIT_TRY(cudaSetDevice(b2s_int_device()));
+    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
     cudaStream_t st = b2s_int_stream(), cs = b2s_int_copy_stream();
-    // device mirrors of every input and output: one block, each array 256-byte aligned
-    std::vector<std::pair<const void*, size_t>> ins;   // host source, bytes
-    std::vector<std::pair<void*, size_t>> outs;        // host destination, element bytes (copied back per row range)
-    std::vector<b2s_pit_set> dsets(sets, sets + n_sets);
-    std::vector<std::vector<b2s_pit_out>> douts(n_sets);
-    std::vector<b2s_pit_col> dcols(cols, cols + n_cols);
-    size_t total = 0;
-    auto reserve = [&](size_t bytes) {
-      const size_t off = total;
-      total += (bytes + 255) / 256 * 256;
-      return off;
-    };
-    std::vector<size_t> in_off, out_off;
-    auto add_in = [&](const void* h, size_t bytes) { ins.push_back({h, bytes}); in_off.push_back(reserve(bytes)); };
-    auto add_out = [&](void* h, size_t elem) { outs.push_back({h, elem}); out_off.push_back(reserve((size_t)n * elem)); };
-    if (ts) add_in(ts, (size_t)n * 8);
-    for (int s = 0; s < n_sets; ++s) {
-      add_in(sets[s].keys, (size_t)n * 8);
-      for (int j = 0; j < sets[s].n_out; ++j) add_out(sets[s].outs[j].out, sets[s].outs[j].bytes);
-      if (sets[s].ts_out) add_out(sets[s].ts_out, 8);
-      if (sets[s].found) add_out(sets[s].found, 1);
+    // row ranges of sorted positions: range k's results go back on the copy stream while range k + 1 is joined
+    const int64_t kRange = 1 << 20;
+    const int n_ranges = (int)((n + kRange - 1) / kRange);
+    Events ev, range_ev;
+    if (int rc = ev.create(3)) return rc;
+    if (int rc = range_ev.create(n_ranges, cudaEventDisableTiming)) return rc;
+    // device mirrors of every input and output in one block, freed after the copy stream is synchronised
+    SyncOnExit st_done{st};
+    DeviceBlock blk(st);
+    SyncOnExit cs_done{cs};  // after a failure, copies back queued on cs may still read the block
+    DeviceDescs d(blk, n, true, ts, sets, n_sets, cols, n_cols, order);
+    if (int rc = blk.alloc()) return rc;
+    B2S_CUDA_TRY(cudaMemsetAsync(d.miss, 0, 8 * (size_t)std::max(n_sets, 1), st));
+    B2S_CUDA_TRY(cudaEventRecord(ev[0], st));
+    if (int rc = blk.upload()) return rc;
+    B2S_CUDA_TRY(cudaEventRecord(ev[1], st));
+    SortBufs sb(st);
+    Launches launches;
+    if (int rc = d.ts ? sort_keys(sb, d.ts, n, launches) : B2S_OK) return rc;
+    for (int k = 0; k < n_ranges; ++k) {
+      const int64_t q0 = (int64_t)k * kRange, q1 = std::min<int64_t>(n, q0 + kRange);
+      if (int rc = launch_join(reinterpret_cast<const int64_t*>(sb.k[0]), sb.v[0], d.order, q0, q1, d.sets.data(), n_sets, d.cols.data(),
+                               n_cols, d.miss, st, launches))
+        return rc;
+      B2S_CUDA_TRY(cudaEventRecord(range_ev[k], st));
+      B2S_CUDA_TRY(cudaStreamWaitEvent(cs, range_ev[k], 0));
+      if (int rc = blk.download(q0, q1, cs)) return rc;
     }
-    for (int c = 0; c < n_cols; ++c) {
-      add_in(cols[c].src, (size_t)n * cols[c].bytes);
-      add_out(cols[c].dst, cols[c].bytes);
+    B2S_CUDA_TRY(cudaEventRecord(ev[2], st));
+    if (n_sets) B2S_CUDA_TRY(cudaMemcpyAsync(miss, d.miss, 8 * (size_t)n_sets, cudaMemcpyDeviceToHost, cs));
+    B2S_CUDA_TRY(cudaStreamSynchronize(cs));
+    B2S_CUDA_TRY(cudaStreamSynchronize(st));
+    if (stats) {
+      memset(stats, 0, sizeof(*stats));
+      stats->rows = n;
+      cudaEventElapsedTime(&stats->h2d_ms, ev[0], ev[1]);
+      cudaEventElapsedTime(&stats->kernel_ms, ev[1], ev[2]);  // sort + join (the copies back overlap the join)
+      stats->kernels = launches.n;
     }
-    if (order) add_out(order, 8);
-    const size_t miss_off = reserve(8 * (size_t)std::max(n_sets, 1));
-    char* d_block = nullptr;
-    SortBufs sb{};
-    int rc = B2S_OK;
-    cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
-    std::vector<cudaEvent_t> range_ev;
-    do {
-      for (auto& e : ev) PIT_BREAK(cudaEventCreate(&e));
-      if (rc) break;
-      PIT_BREAK(cudaMallocAsync(&d_block, total, st));
-      PIT_BREAK(cudaMemsetAsync(d_block + miss_off, 0, 8 * (size_t)std::max(n_sets, 1), st));
-      PIT_BREAK(cudaEventRecord(ev[0], st));
-      for (size_t i = 0; i < ins.size(); ++i) PIT_BREAK(cudaMemcpyAsync(d_block + in_off[i], ins[i].first, ins[i].second, cudaMemcpyHostToDevice, st));
-      if (rc) break;
-      PIT_BREAK(cudaEventRecord(ev[1], st));
-      // the same descriptors over the device mirrors
-      size_t ii = ts ? 1 : 0, oi = 0;
-      for (int s = 0; s < n_sets; ++s) {
-        dsets[s].keys = reinterpret_cast<const int64_t*>(d_block + in_off[ii++]);
-        douts[s].assign(sets[s].outs, sets[s].outs + sets[s].n_out);
-        for (auto& o : douts[s]) o.out = d_block + out_off[oi++];
-        dsets[s].outs = douts[s].data();
-        if (sets[s].ts_out) dsets[s].ts_out = reinterpret_cast<int64_t*>(d_block + out_off[oi++]);
-        if (sets[s].found) dsets[s].found = reinterpret_cast<uint8_t*>(d_block + out_off[oi++]);
-      }
-      for (int c = 0; c < n_cols; ++c) {
-        dcols[c].src = d_block + in_off[ii++];
-        dcols[c].dst = d_block + out_off[oi++];
-      }
-      int64_t* d_order = order ? reinterpret_cast<int64_t*>(d_block + out_off[oi++]) : nullptr;
-      const int64_t* d_ts = ts ? reinterpret_cast<const int64_t*>(d_block + in_off[0]) : nullptr;
-      if (d_ts && (rc = sort_entities(d_ts, n, sb, st))) break;
-      // row ranges of sorted positions: range k's results go back on the copy stream while range k + 1 is joined
-      const int64_t kRange = 1 << 20;
-      const int n_ranges = (int)((n + kRange - 1) / kRange);
-      range_ev.assign(n_ranges, nullptr);
-      for (auto& e : range_ev) PIT_BREAK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-      if (rc) break;
-      auto* d_miss = reinterpret_cast<unsigned long long*>(d_block + miss_off);
-      int launches = d_ts ? 24 : 0;  // the entity sort's
-      for (int k = 0; k < n_ranges && !rc; ++k) {
-        const int64_t q0 = (int64_t)k * kRange, q1 = std::min<int64_t>(n, q0 + kRange);
-        rc = launch_join(d_ts ? reinterpret_cast<const int64_t*>(sb.k[0]) : nullptr, d_ts ? sb.v[0] : nullptr, d_order, q0, q1, dsets.data(),
-                         n_sets, dcols.data(), n_cols, d_miss, st, &launches);
-        if (rc) break;
-        PIT_BREAK(cudaEventRecord(range_ev[k], st));
-        PIT_BREAK(cudaStreamWaitEvent(cs, range_ev[k], 0));
-        for (size_t i = 0; i < outs.size(); ++i) {
-          const size_t el = outs[i].second;
-          PIT_BREAK(cudaMemcpyAsync(static_cast<char*>(outs[i].first) + q0 * el, d_block + out_off[i] + q0 * el, (size_t)(q1 - q0) * el,
-                                    cudaMemcpyDeviceToHost, cs));
-        }
-      }
-      if (rc) break;
-      PIT_BREAK(cudaEventRecord(ev[2], st));
-      if (n_sets) PIT_BREAK(cudaMemcpyAsync(miss, d_miss, 8 * (size_t)n_sets, cudaMemcpyDeviceToHost, cs));
-      PIT_BREAK(cudaStreamSynchronize(cs));
-      PIT_BREAK(cudaStreamSynchronize(st));
-      if (stats) {
-        memset(stats, 0, sizeof(*stats));
-        stats->rows = n;
-        cudaEventElapsedTime(&stats->h2d_ms, ev[0], ev[1]);
-        cudaEventElapsedTime(&stats->kernel_ms, ev[1], ev[2]);  // sort + join (the copies back overlap the join)
-        stats->kernels = launches;
-      }
-    } while (0);
-    free_sort(sb, st);
-    cudaStreamSynchronize(cs);  // after a failure, copies back queued on cs may still read d_block
-    if (d_block) cudaFreeAsync(d_block, st);
-    cudaStreamSynchronize(st);
-    for (auto& e : ev)
-      if (e) cudaEventDestroy(e);
-    for (auto& e : range_ev)
-      if (e) cudaEventDestroy(e);
-    return rc;
+    return B2S_OK;
   } catch (const std::exception& e) {
     return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
   }
@@ -658,102 +592,65 @@ int check_train(const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols
 // four events recorded before the sort, after it, after the join and after the compaction.
 int train_run(const int64_t* d_ts, int64_t n, const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols, int32_t n_cols,
               const b2s_pit_label* label, int64_t* d_order, unsigned long long* d_miss, int64_t* d_kept, cudaStream_t st,
-              cudaEvent_t* ev, int* launches) {
+              const cudaEvent_t* ev, Launches& launches) {
   const int64_t n_tiles = (n + kTile - 1) / kTile;
-  // scratch: one n-row copy of every output, the keep flags, the tile counts and the join's own miss counters
-  struct Move { const void* src; void* dst; int32_t bytes; };
-  std::vector<Move> moves;
-  std::vector<b2s_pit_set> dsets(sets, sets + n_sets);
-  std::vector<std::vector<b2s_pit_out>> douts(n_sets);
-  std::vector<b2s_pit_col> dcols(cols, cols + n_cols);
-  size_t total = 0;
-  auto reserve = [&](size_t bytes) {
-    const size_t off = total;
-    total += (bytes + 255) / 256 * 256;
-    return off;
-  };
-  std::vector<size_t> offs;
-  auto add = [&](void* dst, int32_t bytes) { moves.push_back({nullptr, dst, bytes}); offs.push_back(reserve((size_t)n * bytes)); };
+  // scratch: one n-row copy of every output, the join's own miss counters, the keep flags and the tile counts
+  DeviceBlock blk(st);
+  DeviceDescs d(blk, n, false, d_ts, sets, n_sets, cols, n_cols, d_order);
+  uint8_t* d_keep = nullptr;
+  int64_t* d_count = nullptr;
+  blk.scratch(d_keep, (size_t)n);
+  blk.scratch(d_count, (size_t)n_tiles * 8);
+  if (int rc = blk.alloc()) return rc;
+  B2S_CUDA_TRY(cudaMemsetAsync(d.miss, 0, 8 * (size_t)std::max(n_sets, 1), st));
+  if (n_sets) B2S_CUDA_TRY(cudaMemsetAsync(d_miss, 0, 8 * (size_t)n_sets, st));
+  if (ev) B2S_CUDA_TRY(cudaEventRecord(ev[0], st));
+  SortBufs sb(st);
+  if (int rc = d_ts ? sort_keys(sb, d_ts, n, launches) : B2S_OK) return rc;
+  if (ev) B2S_CUDA_TRY(cudaEventRecord(ev[1], st));
+  if (int rc = launch_join(reinterpret_cast<const int64_t*>(sb.k[0]), sb.v[0], d.order, 0, n, d.sets.data(), n_sets, d.cols.data(), n_cols,
+                           d.miss, st, launches))
+    return rc;
+  if (ev) B2S_CUDA_TRY(cudaEventRecord(ev[2], st));
+  KeepParams kp{};
+  kp.n_sets = n_sets;
+  kp.n = n;
   for (int s = 0; s < n_sets; ++s) {
-    for (int j = 0; j < sets[s].n_out; ++j) add(sets[s].outs[j].out, sets[s].outs[j].bytes);
-    if (sets[s].ts_out) add(sets[s].ts_out, 8);
-    add(sets[s].found, 1);
+    kp.found[s] = d.sets[s].found;
+    kp.exact[s] = sets[s].asof ? 0 : 1;
   }
-  for (int c = 0; c < n_cols; ++c) add(cols[c].dst, cols[c].bytes);
-  if (d_order) add(d_order, 8);
-  const size_t keep_off = reserve((size_t)n), count_off = reserve((size_t)n_tiles * 8), miss_off = reserve(8 * (size_t)std::max(n_sets, 1));
-  char* d_scratch = nullptr;
-  SortBufs sb{};
-  int rc = B2S_OK;
-  do {
-    PIT_BREAK(cudaMallocAsync(&d_scratch, total, st));
-    PIT_BREAK(cudaMemsetAsync(d_scratch + miss_off, 0, 8 * (size_t)std::max(n_sets, 1), st));
-    if (n_sets) PIT_BREAK(cudaMemsetAsync(d_miss, 0, 8 * (size_t)n_sets, st));
-    size_t m = 0;
-    for (auto& mv : moves) mv.src = d_scratch + offs[m++];
-    m = 0;
-    for (int s = 0; s < n_sets; ++s) {
-      douts[s].assign(sets[s].outs, sets[s].outs + sets[s].n_out);
-      for (auto& o : douts[s]) o.out = const_cast<void*>(moves[m++].src);
-      dsets[s].outs = douts[s].data();
-      if (sets[s].ts_out) dsets[s].ts_out = static_cast<int64_t*>(const_cast<void*>(moves[m++].src));
-      dsets[s].found = static_cast<uint8_t*>(const_cast<void*>(moves[m++].src));
+  if (label) {
+    kp.label_kind = label->kind;
+    if (label->set >= 0) {
+      kp.label_found = d.sets[label->set].found;
+      kp.label = d.outs[label->set][label->out].out;
+      kp.label_bytes = d.outs[label->set][label->out].bytes;
+    } else {
+      kp.label = d.cols[label->out].dst;
+      kp.label_bytes = d.cols[label->out].bytes;
     }
-    for (int c = 0; c < n_cols; ++c) dcols[c].dst = const_cast<void*>(moves[m++].src);
-    int64_t* d_order_scratch = d_order ? static_cast<int64_t*>(const_cast<void*>(moves[m++].src)) : nullptr;
-    if (ev) PIT_BREAK(cudaEventRecord(ev[0], st));
-    if (d_ts && (rc = sort_entities(d_ts, n, sb, st))) break;
-    if (d_ts) *launches += 24;
-    if (ev) PIT_BREAK(cudaEventRecord(ev[1], st));
-    if ((rc = launch_join(d_ts ? reinterpret_cast<const int64_t*>(sb.k[0]) : nullptr, d_ts ? sb.v[0] : nullptr, d_order_scratch, 0, n,
-                          dsets.data(), n_sets, dcols.data(), n_cols, reinterpret_cast<unsigned long long*>(d_scratch + miss_off), st,
-                          launches)))
-      break;
-    if (ev) PIT_BREAK(cudaEventRecord(ev[2], st));
-    KeepParams kp{};
-    kp.n_sets = n_sets;
-    kp.n = n;
-    for (int s = 0; s < n_sets; ++s) {
-      kp.found[s] = dsets[s].found;
-      kp.exact[s] = sets[s].asof ? 0 : 1;
+    if (kp.label_kind == B2S_PIT_LABEL_FOUND) kp.label = nullptr;
+  }
+  keep_kernel<<<(unsigned)n_tiles, kTile, 0, st>>>(kp, d_keep, d_count, d_miss);
+  scan_tiles_kernel<<<1, 1024, 0, st>>>(d_count, n_tiles, d_kept);
+  launches.add(2);
+  // each scratch copy's kept rows go to the array it stands for
+  const std::vector<DeviceBlock::Out>& moves = blk.outputs();
+  for (size_t i = 0; i < moves.size(); i += kScatterCols) {
+    ScatterParams sp{};
+    sp.n = n;
+    for (size_t j = i; j < moves.size() && sp.n_cols < kScatterCols; ++j, ++sp.n_cols) {
+      sp.src[sp.n_cols] = blk.at(moves[j].off);
+      sp.dst[sp.n_cols] = moves[j].dst;
+      sp.bytes[sp.n_cols] = (int32_t)moves[j].elem;
     }
-    if (label) {
-      kp.label_kind = label->kind;
-      if (label->set >= 0) {
-        kp.label_found = dsets[label->set].found;
-        kp.label = douts[label->set][label->out].out;
-        kp.label_bytes = douts[label->set][label->out].bytes;
-      } else {
-        kp.label = dcols[label->out].dst;
-        kp.label_bytes = dcols[label->out].bytes;
-      }
-      if (kp.label_kind == B2S_PIT_LABEL_FOUND) kp.label = nullptr;
-    }
-    uint8_t* d_keep = reinterpret_cast<uint8_t*>(d_scratch + keep_off);
-    int64_t* d_count = reinterpret_cast<int64_t*>(d_scratch + count_off);
-    keep_kernel<<<(unsigned)n_tiles, kTile, 0, st>>>(kp, d_keep, d_count, d_miss);
-    scan_tiles_kernel<<<1, 1024, 0, st>>>(d_count, n_tiles, d_kept);
-    b2s_int_count_launches(2);
-    *launches += 2;
-    for (size_t i = 0; i < moves.size(); i += kScatterCols) {
-      ScatterParams sp{};
-      sp.n = n;
-      for (size_t j = i; j < moves.size() && sp.n_cols < kScatterCols; ++j, ++sp.n_cols) {
-        sp.src[sp.n_cols] = moves[j].src;
-        sp.dst[sp.n_cols] = moves[j].dst;
-        sp.bytes[sp.n_cols] = moves[j].bytes;
-      }
-      scatter_kernel<<<(unsigned)n_tiles, kTile, 0, st>>>(sp, d_keep, d_count);
-      b2s_int_count_launches(1);
-      ++*launches;
-    }
-    if (ev) PIT_BREAK(cudaEventRecord(ev[3], st));
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) rc = b2s_int_fail(B2S_ERR_CUDA, "training-set launch failed: %s", cudaGetErrorString(e));
-  } while (0);
-  free_sort(sb, st);
-  if (d_scratch) cudaFreeAsync(d_scratch, st);
-  return rc;
+    scatter_kernel<<<(unsigned)n_tiles, kTile, 0, st>>>(sp, d_keep, d_count);
+    launches.add(1);
+  }
+  if (ev) B2S_CUDA_TRY(cudaEventRecord(ev[3], st));
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return b2s_int_fail(B2S_ERR_CUDA, "training-set launch failed: %s", cudaGetErrorString(e));
+  return B2S_OK;
 }
 
 }  // namespace
@@ -764,16 +661,16 @@ extern "C" int b2s_pit_train_device(const int64_t* d_ts, int64_t n, const b2s_pi
   try {  // no C++ exception crosses the C boundary
     if (int rc = check_train(sets, n_sets, cols, n_cols, d_ts, n, label, d_miss, d_kept)) return rc;
     if (misaligned(d_order, 8)) return b2s_int_fail(B2S_ERR_INVALID, "order must be 8-byte aligned");
-    PIT_TRY(cudaSetDevice(b2s_int_device()));
+    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
     cudaStream_t st = stream ? (cudaStream_t)stream : b2s_int_stream();
     if (n == 0) {
-      PIT_TRY(cudaMemsetAsync(d_kept, 0, 8, st));
-      if (n_sets) PIT_TRY(cudaMemsetAsync(d_miss, 0, 8 * (size_t)n_sets, st));
+      B2S_CUDA_TRY(cudaMemsetAsync(d_kept, 0, 8, st));
+      if (n_sets) B2S_CUDA_TRY(cudaMemsetAsync(d_miss, 0, 8 * (size_t)n_sets, st));
       return B2S_OK;
     }
-    int launches = 0;
+    Launches launches;
     return train_run(d_ts, n, sets, n_sets, cols, n_cols, label, d_order, reinterpret_cast<unsigned long long*>(d_miss), d_kept, st,
-                     nullptr, &launches);
+                     nullptr, launches);
   } catch (const std::exception& e) {
     return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
   }
@@ -791,99 +688,45 @@ extern "C" int b2s_pit_train_host(const int64_t* ts, int64_t n, const b2s_pit_se
       if (stats) memset(stats, 0, sizeof(*stats));
       return B2S_OK;
     }
-    PIT_TRY(cudaSetDevice(b2s_int_device()));
+    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
     cudaStream_t st = b2s_int_stream();
+    Events ev;
+    if (int rc = ev.create(6)) return rc;
     // one device block: every input, then every output's kept rows (n rows reserved), the counters
-    std::vector<std::pair<const void*, size_t>> ins;  // host source, bytes
-    std::vector<std::pair<void*, size_t>> outs;       // host destination, element bytes
-    std::vector<b2s_pit_set> dsets(sets, sets + n_sets);
-    std::vector<std::vector<b2s_pit_out>> douts(n_sets);
-    std::vector<b2s_pit_col> dcols(cols, cols + n_cols);
-    size_t total = 0;
-    auto reserve = [&](size_t bytes) {
-      const size_t off = total;
-      total += (bytes + 255) / 256 * 256;
-      return off;
-    };
-    std::vector<size_t> in_off, out_off;
-    auto add_in = [&](const void* h, size_t bytes) { ins.push_back({h, bytes}); in_off.push_back(reserve(bytes)); };
-    auto add_out = [&](void* h, size_t elem) { outs.push_back({h, elem}); out_off.push_back(reserve((size_t)n * elem)); };
-    if (ts) add_in(ts, (size_t)n * 8);
-    for (int s = 0; s < n_sets; ++s) {
-      add_in(sets[s].keys, (size_t)n * 8);
-      for (int j = 0; j < sets[s].n_out; ++j) add_out(sets[s].outs[j].out, sets[s].outs[j].bytes);
-      if (sets[s].ts_out) add_out(sets[s].ts_out, 8);
-      add_out(sets[s].found, 1);
+    SyncOnExit done{st};
+    DeviceBlock blk(st);
+    DeviceDescs d(blk, n, true, ts, sets, n_sets, cols, n_cols, order);
+    int64_t* d_kept = nullptr;
+    blk.scratch(d_kept, 8);
+    if (int rc = blk.alloc()) return rc;
+    B2S_CUDA_TRY(cudaEventRecord(ev[0], st));
+    if (int rc = blk.upload()) return rc;
+    Launches launches;
+    if (int rc = train_run(d.ts, n, d.sets.data(), n_sets, d.cols.data(), n_cols, label, d.order, d.miss, d_kept, st, ev.data() + 1, launches))
+      return rc;
+    B2S_CUDA_TRY(cudaMemcpyAsync(kept, d_kept, 8, cudaMemcpyDeviceToHost, st));
+    if (n_sets) B2S_CUDA_TRY(cudaMemcpyAsync(miss, d.miss, 8 * (size_t)n_sets, cudaMemcpyDeviceToHost, st));
+    B2S_CUDA_TRY(cudaStreamSynchronize(st));
+    // only the kept rows come back, in ranges of 1 Mi rows
+    const int64_t kRange = 1 << 20;
+    for (int64_t q0 = 0; q0 < *kept; q0 += kRange)
+      if (int rc = blk.download(q0, std::min<int64_t>(*kept, q0 + kRange), st)) return rc;
+    B2S_CUDA_TRY(cudaEventRecord(ev[5], st));
+    B2S_CUDA_TRY(cudaStreamSynchronize(st));
+    if (phase_ms) {
+      cudaEventElapsedTime(&phase_ms[0], ev[1], ev[2]);  // sort
+      cudaEventElapsedTime(&phase_ms[1], ev[2], ev[3]);  // join
+      cudaEventElapsedTime(&phase_ms[2], ev[3], ev[4]);  // compaction
     }
-    for (int c = 0; c < n_cols; ++c) {
-      add_in(cols[c].src, (size_t)n * cols[c].bytes);
-      add_out(cols[c].dst, cols[c].bytes);
+    if (stats) {
+      memset(stats, 0, sizeof(*stats));
+      stats->rows = n;
+      cudaEventElapsedTime(&stats->h2d_ms, ev[0], ev[1]);
+      cudaEventElapsedTime(&stats->kernel_ms, ev[1], ev[4]);
+      cudaEventElapsedTime(&stats->d2h_ms, ev[4], ev[5]);
+      stats->kernels = launches.n;
     }
-    if (order) add_out(order, 8);
-    const size_t miss_off = reserve(8 * (size_t)std::max(n_sets, 1)), kept_off = reserve(8);
-    char* d_block = nullptr;
-    int rc = B2S_OK, launches = 0;
-    cudaEvent_t ev[6] = {};
-    do {
-      for (auto& e : ev) PIT_BREAK(cudaEventCreate(&e));
-      if (rc) break;
-      PIT_BREAK(cudaMallocAsync(&d_block, total, st));
-      PIT_BREAK(cudaEventRecord(ev[0], st));
-      for (size_t i = 0; i < ins.size(); ++i) PIT_BREAK(cudaMemcpyAsync(d_block + in_off[i], ins[i].first, ins[i].second, cudaMemcpyHostToDevice, st));
-      if (rc) break;
-      size_t ii = ts ? 1 : 0, oi = 0;
-      for (int s = 0; s < n_sets; ++s) {
-        dsets[s].keys = reinterpret_cast<const int64_t*>(d_block + in_off[ii++]);
-        douts[s].assign(sets[s].outs, sets[s].outs + sets[s].n_out);
-        for (auto& o : douts[s]) o.out = d_block + out_off[oi++];
-        dsets[s].outs = douts[s].data();
-        if (sets[s].ts_out) dsets[s].ts_out = reinterpret_cast<int64_t*>(d_block + out_off[oi++]);
-        dsets[s].found = reinterpret_cast<uint8_t*>(d_block + out_off[oi++]);
-      }
-      for (int c = 0; c < n_cols; ++c) {
-        dcols[c].src = d_block + in_off[ii++];
-        dcols[c].dst = d_block + out_off[oi++];
-      }
-      int64_t* d_order = order ? reinterpret_cast<int64_t*>(d_block + out_off[oi++]) : nullptr;
-      const int64_t* d_ts = ts ? reinterpret_cast<const int64_t*>(d_block + in_off[0]) : nullptr;
-      auto* d_miss = reinterpret_cast<unsigned long long*>(d_block + miss_off);
-      auto* d_kept = reinterpret_cast<int64_t*>(d_block + kept_off);
-      if ((rc = train_run(d_ts, n, dsets.data(), n_sets, dcols.data(), n_cols, label, d_order, d_miss, d_kept, st, ev + 1, &launches))) break;
-      PIT_BREAK(cudaMemcpyAsync(kept, d_kept, 8, cudaMemcpyDeviceToHost, st));
-      if (n_sets) PIT_BREAK(cudaMemcpyAsync(miss, d_miss, 8 * (size_t)n_sets, cudaMemcpyDeviceToHost, st));
-      PIT_BREAK(cudaStreamSynchronize(st));
-      // only the kept rows come back, in ranges of 1 Mi rows
-      const int64_t kRange = 1 << 20;
-      for (int64_t q0 = 0; q0 < *kept && !rc; q0 += kRange) {
-        const int64_t q1 = std::min<int64_t>(*kept, q0 + kRange);
-        for (size_t i = 0; i < outs.size(); ++i) {
-          const size_t el = outs[i].second;
-          PIT_BREAK(cudaMemcpyAsync(static_cast<char*>(outs[i].first) + q0 * el, d_block + out_off[i] + q0 * el, (size_t)(q1 - q0) * el,
-                                    cudaMemcpyDeviceToHost, st));
-        }
-      }
-      if (rc) break;
-      PIT_BREAK(cudaEventRecord(ev[5], st));
-      PIT_BREAK(cudaStreamSynchronize(st));
-      if (phase_ms) {
-        cudaEventElapsedTime(&phase_ms[0], ev[1], ev[2]);  // sort
-        cudaEventElapsedTime(&phase_ms[1], ev[2], ev[3]);  // join
-        cudaEventElapsedTime(&phase_ms[2], ev[3], ev[4]);  // compaction
-      }
-      if (stats) {
-        memset(stats, 0, sizeof(*stats));
-        stats->rows = n;
-        cudaEventElapsedTime(&stats->h2d_ms, ev[0], ev[1]);
-        cudaEventElapsedTime(&stats->kernel_ms, ev[1], ev[4]);
-        cudaEventElapsedTime(&stats->d2h_ms, ev[4], ev[5]);
-        stats->kernels = launches;
-      }
-    } while (0);
-    if (d_block) cudaFreeAsync(d_block, st);
-    cudaStreamSynchronize(st);
-    for (auto& e : ev)
-      if (e) cudaEventDestroy(e);
-    return rc;
+    return B2S_OK;
   } catch (const std::exception& e) {
     return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
   }

@@ -52,13 +52,6 @@ int b2s_int_fail(int code, const char* fmt, ...) {
   g_err = buf;
   return code;
 }
-#define CUDA_TRY(expr)                                                                           \
-  do {                                                                                           \
-    cudaError_t _e = (expr);                                                                     \
-    if (_e != cudaSuccess)                                                                       \
-      return fail(B2S_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
-  } while (0)
-
 // ------------------------------------------------------------------------------------------ globals
 struct Global {
   bool inited = false;
@@ -540,10 +533,10 @@ extern "C" int b2s_init(int device_ordinal, const char* cfg) {
       return fail(B2S_ERR_NO_DEVICE, "no CUDA device (%s); this engine has no CPU fallback",
                   e == cudaSuccess ? "device count 0" : cudaGetErrorString(e));
     if (device_ordinal < 0 || device_ordinal >= n) return fail(B2S_ERR_INVALID, "device ordinal %d out of range", device_ordinal);
-    CUDA_TRY(cudaSetDevice(device_ordinal));
-    CUDA_TRY(cudaGetDeviceProperties(&G.prop, device_ordinal));
-    CUDA_TRY(cudaStreamCreateWithFlags(&G.stream, cudaStreamNonBlocking));
-    CUDA_TRY(cudaStreamCreateWithFlags(&G.copy_stream, cudaStreamNonBlocking));
+    B2S_CUDA_TRY(cudaSetDevice(device_ordinal));
+    B2S_CUDA_TRY(cudaGetDeviceProperties(&G.prop, device_ordinal));
+    B2S_CUDA_TRY(cudaStreamCreateWithFlags(&G.stream, cudaStreamNonBlocking));
+    B2S_CUDA_TRY(cudaStreamCreateWithFlags(&G.copy_stream, cudaStreamNonBlocking));
     G.device = device_ordinal;
     std::string c = cfg ? cfg : "";
     G.ring_slots = (int)cfg_get(c, "ring_slots", 4);
@@ -1102,7 +1095,7 @@ static int t3_build(b2s_plan_s* p, const KParams& k, bool any_fill) {
   const size_t o_cols = tb.add(col_score), o_order = tb.add(col_order), o_mcols = tb.add(model_cols);
   const size_t o_parts = align_up(tb.data.size(), 16);
   tb.data.resize(o_parts + sizeof(T3Part) * P);
-  CUDA_TRY(cudaMalloc(&p->d_t3_blob, tb.data.size()));
+  B2S_CUDA_TRY(cudaMalloc(&p->d_t3_blob, tb.data.size()));
   std::vector<T3Part> dev(P);
   int cta0 = 0;
   for (int i = 0; i < P; ++i) {
@@ -1118,7 +1111,7 @@ static int t3_build(b2s_plan_s* p, const KParams& k, bool any_fill) {
     cta0 += n_ctas[i];
   }
   memcpy(tb.data.data() + o_parts, dev.data(), sizeof(T3Part) * P);
-  CUDA_TRY(cudaMemcpy(p->d_t3_blob, tb.data.data(), tb.data.size(), cudaMemcpyHostToDevice));
+  B2S_CUDA_TRY(cudaMemcpy(p->d_t3_blob, tb.data.data(), tb.data.size(), cudaMemcpyHostToDevice));
   p->d_t3_col_score = (const int32_t*)(p->d_t3_blob + o_cols);
   p->d_t3_col_order = (const int32_t*)(p->d_t3_blob + o_order);
   p->d_t3_model_cols = (const int32_t*)(p->d_t3_blob + o_mcols);
@@ -1443,9 +1436,9 @@ extern "C" int b2s_plan_finalize(b2s_plan_t p) {
                  o_votew = bb.add(p->vote_w), o_wgen = bb.add(wgen), o_nodes = bb.add(nodes), o_leaf = bb.add(leaf),
                  o_troot = bb.add(tree_root), o_tslot = bb.add(tree_slot), o_tscale = bb.add(tree_scale),
                  o_chunk = bb.add(chunk_kind);
-    CUDA_TRY(cudaSetDevice(G.device));
-    CUDA_TRY(cudaMalloc(&p->d_blob, bb.data.size()));
-    CUDA_TRY(cudaMemcpy(p->d_blob, bb.data.data(), bb.data.size(), cudaMemcpyHostToDevice));
+    B2S_CUDA_TRY(cudaSetDevice(G.device));
+    B2S_CUDA_TRY(cudaMalloc(&p->d_blob, bb.data.size()));
+    B2S_CUDA_TRY(cudaMemcpy(p->d_blob, bb.data.data(), bb.data.size(), cudaMemcpyHostToDevice));
     p->blob_bytes = bb.data.size();
     char* B = p->d_blob;
 
@@ -1651,7 +1644,7 @@ extern "C" int b2s_plan_finalize(b2s_plan_t p) {
     if (p->mode == MODE_TREES && identity_schema && !any_map) {
       if (int rc = t3_build(p, k, any_fill)) return rc;
     }
-    for (int i = 0; i < 4; ++i) CUDA_TRY(cudaEventCreate(&p->ev[i]));
+    for (int i = 0; i < 4; ++i) B2S_CUDA_TRY(cudaEventCreate(&p->ev[i]));
     p->finalized = true;
     return B2S_OK;
   } catch (const std::exception& e) {
@@ -1748,9 +1741,9 @@ static int launch_on(b2s_plan_t p, const void* d_rows, int64_t n_rows, int64_t s
         if (mine.xt) cudaFree(mine.xt);
         mine = b2s_plan_s::TreeScratch{};
         const int64_t cap = std::max<int64_t>(align_up((size_t)n_rows, 64), 65536);
-        CUDA_TRY(cudaMalloc(&mine.partial, (size_t)cap * C * 8));
-        CUDA_TRY(cudaMalloc(&mine.row_bad, (size_t)cap * 4));
-        CUDA_TRY(cudaMalloc(&mine.xt, (size_t)(cap / kT3TR) * p->t3.xt_words * 4));
+        B2S_CUDA_TRY(cudaMalloc(&mine.partial, (size_t)cap * C * 8));
+        B2S_CUDA_TRY(cudaMalloc(&mine.row_bad, (size_t)cap * 4));
+        B2S_CUDA_TRY(cudaMalloc(&mine.xt, (size_t)(cap / kT3TR) * p->t3.xt_words * 4));
         mine.rows = cap;
       }
       sc = mine;
@@ -1866,11 +1859,11 @@ static int ensure_stage(b2s_plan_t p, int64_t n_rows) {
   p->d_stage_status = nullptr;
   p->stage_rows = 0;
   const int64_t cap = std::max<int64_t>(n_rows, 4096);
-  CUDA_TRY(cudaMallocHost(&p->h_stage_in, (size_t)cap * p->n_in * 4));
-  CUDA_TRY(cudaMallocHost(&p->h_stage_out, (size_t)cap * (p->out_cols + 1) * 4));
-  CUDA_TRY(cudaMalloc(&p->d_stage_in, (size_t)cap * p->n_in * 4));
-  CUDA_TRY(cudaMalloc(&p->d_stage_out, (size_t)cap * p->out_cols * 4));
-  CUDA_TRY(cudaMalloc(&p->d_stage_status, (size_t)cap * 4));
+  B2S_CUDA_TRY(cudaMallocHost(&p->h_stage_in, (size_t)cap * p->n_in * 4));
+  B2S_CUDA_TRY(cudaMallocHost(&p->h_stage_out, (size_t)cap * (p->out_cols + 1) * 4));
+  B2S_CUDA_TRY(cudaMalloc(&p->d_stage_in, (size_t)cap * p->n_in * 4));
+  B2S_CUDA_TRY(cudaMalloc(&p->d_stage_out, (size_t)cap * p->out_cols * 4));
+  B2S_CUDA_TRY(cudaMalloc(&p->d_stage_status, (size_t)cap * 4));
   p->stage_rows = cap;
   return B2S_OK;
 }
@@ -1893,7 +1886,7 @@ extern "C" int b2s_run_host(b2s_plan_t p, const void* rows, int64_t n_rows, int6
     if (out_bytes < n_rows * p->out_cols * 4) return fail(B2S_ERR_INVALID, "out buffer too small");
     if (n_rows == 0) return B2S_OK;
     std::lock_guard<std::mutex> lk(p->host_mu);
-    CUDA_TRY(cudaSetDevice(G.device));
+    B2S_CUDA_TRY(cudaSetDevice(G.device));
     if (int rc = ensure_stage(p, n_rows)) return rc;
     cudaStream_t st = G.stream;
     cudaPointerAttributes attr{};
@@ -1916,42 +1909,42 @@ extern "C" int b2s_run_host(b2s_plan_t p, const void* rows, int64_t n_rows, int6
       const int n_chunks = (int)((n_rows + chunk - 1) / chunk);
       while ((int)p->chunk_ev.size() < 4 * n_chunks) {
         cudaEvent_t e;
-        CUDA_TRY(cudaEventCreate(&e));
+        B2S_CUDA_TRY(cudaEventCreate(&e));
         p->chunk_ev.push_back(e);
       }
       cudaStream_t cs = G.copy_stream;
       int32_t* h_status = (int32_t*)(p->h_stage_out + out_sz);
       const size_t out_row = (size_t)p->out_cols * 4;
-      CUDA_TRY(cudaEventRecord(p->ev[0], cs));
+      B2S_CUDA_TRY(cudaEventRecord(p->ev[0], cs));
       for (int c = 0; c < n_chunks; ++c) {
         const int64_t r0 = (int64_t)c * chunk, nr = std::min<int64_t>(chunk, n_rows - r0);
         cudaEvent_t* ce = &p->chunk_ev[4 * c];
-        CUDA_TRY(cudaMemcpyAsync(p->d_stage_in + r0 * row_bytes, (const char*)src + r0 * row_bytes, (size_t)nr * row_bytes,
+        B2S_CUDA_TRY(cudaMemcpyAsync(p->d_stage_in + r0 * row_bytes, (const char*)src + r0 * row_bytes, (size_t)nr * row_bytes,
                                  cudaMemcpyHostToDevice, cs));
-        CUDA_TRY(cudaEventRecord(ce[0], cs));
-        CUDA_TRY(cudaStreamWaitEvent(st, ce[0], 0));
-        CUDA_TRY(cudaEventRecord(ce[1], st));
+        B2S_CUDA_TRY(cudaEventRecord(ce[0], cs));
+        B2S_CUDA_TRY(cudaStreamWaitEvent(st, ce[0], 0));
+        B2S_CUDA_TRY(cudaEventRecord(ce[1], st));
         if (int rc = launch_on(p, p->d_stage_in + r0 * row_bytes, nr, row_bytes, p->d_stage_out + r0 * out_row,
                                p->d_stage_status + r0, st)) {
           cudaStreamSynchronize(cs);
           cudaStreamSynchronize(st);
           return rc;
         }
-        CUDA_TRY(cudaEventRecord(ce[2], st));
-        CUDA_TRY(cudaMemcpyAsync(p->h_stage_out + r0 * out_row, p->d_stage_out + r0 * out_row, (size_t)nr * out_row,
+        B2S_CUDA_TRY(cudaEventRecord(ce[2], st));
+        B2S_CUDA_TRY(cudaMemcpyAsync(p->h_stage_out + r0 * out_row, p->d_stage_out + r0 * out_row, (size_t)nr * out_row,
                                  cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaMemcpyAsync(h_status + r0, p->d_stage_status + r0, (size_t)nr * 4, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaEventRecord(ce[3], st));
+        B2S_CUDA_TRY(cudaMemcpyAsync(h_status + r0, p->d_stage_status + r0, (size_t)nr * 4, cudaMemcpyDeviceToHost, st));
+        B2S_CUDA_TRY(cudaEventRecord(ce[3], st));
       }
       int bad = 0;
       for (int c = 0; c < n_chunks; ++c) {  // hand each chunk to the caller as it lands
         const int64_t r0 = (int64_t)c * chunk, nr = std::min<int64_t>(chunk, n_rows - r0);
-        CUDA_TRY(cudaEventSynchronize(p->chunk_ev[4 * c + 3]));
+        B2S_CUDA_TRY(cudaEventSynchronize(p->chunk_ev[4 * c + 3]));
         memcpy((char*)out + r0 * out_row, p->h_stage_out + r0 * out_row, (size_t)nr * out_row);
         for (int64_t r = r0; r < r0 + nr; ++r) bad += (h_status[r] & B2S_ROW_NONFINITE_INPUT) ? 1 : 0;
         if (row_status) memcpy(row_status + r0, h_status + r0, (size_t)nr * 4);
       }
-      CUDA_TRY(cudaStreamSynchronize(cs));
+      B2S_CUDA_TRY(cudaStreamSynchronize(cs));
       if (stats) {
         memset(stats, 0, sizeof(*stats));
         stats->rows = n_rows;
@@ -1978,13 +1971,13 @@ extern "C" int b2s_run_host(b2s_plan_t p, const void* rows, int64_t n_rows, int6
     if (zc_out && !merging) {
       const bool zc_in = n_rows * row_bytes <= zc_in_bytes;
       const void* d_src = p->d_stage_in;
-      if (stats) CUDA_TRY(cudaEventRecord(p->ev[0], st));
+      if (stats) B2S_CUDA_TRY(cudaEventRecord(p->ev[0], st));
       if (zc_in) d_src = pinned ? attr.devicePointer : (const void*)p->h_stage_in;
-      else CUDA_TRY(cudaMemcpyAsync(p->d_stage_in, src, (size_t)n_rows * row_bytes, cudaMemcpyHostToDevice, st));
-      if (stats) CUDA_TRY(cudaEventRecord(p->ev[1], st));
+      else B2S_CUDA_TRY(cudaMemcpyAsync(p->d_stage_in, src, (size_t)n_rows * row_bytes, cudaMemcpyHostToDevice, st));
+      if (stats) B2S_CUDA_TRY(cudaEventRecord(p->ev[1], st));
       if (int rc = launch_on(p, d_src, n_rows, row_bytes, p->h_stage_out, (int32_t*)(p->h_stage_out + out_sz), st, zc_in)) return rc;
-      if (stats) CUDA_TRY(cudaEventRecord(p->ev[2], st));
-      CUDA_TRY(cudaStreamSynchronize(st));
+      if (stats) B2S_CUDA_TRY(cudaEventRecord(p->ev[2], st));
+      B2S_CUDA_TRY(cudaStreamSynchronize(st));
       memcpy(out, p->h_stage_out, out_sz);
       const int32_t* hs = (const int32_t*)(p->h_stage_out + out_sz);
       int bad = 0;
@@ -2000,15 +1993,15 @@ extern "C" int b2s_run_host(b2s_plan_t p, const void* rows, int64_t n_rows, int6
       }
       return B2S_OK;
     }
-    CUDA_TRY(cudaEventRecord(p->ev[0], st));
-    CUDA_TRY(cudaMemcpyAsync(p->d_stage_in, src, (size_t)n_rows * row_bytes, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaEventRecord(p->ev[1], st));
+    B2S_CUDA_TRY(cudaEventRecord(p->ev[0], st));
+    B2S_CUDA_TRY(cudaMemcpyAsync(p->d_stage_in, src, (size_t)n_rows * row_bytes, cudaMemcpyHostToDevice, st));
+    B2S_CUDA_TRY(cudaEventRecord(p->ev[1], st));
     if (int rc = launch_on(p, p->d_stage_in, n_rows, row_bytes, p->d_stage_out, p->d_stage_status, st)) return rc;
-    CUDA_TRY(cudaEventRecord(p->ev[2], st));
-    CUDA_TRY(cudaMemcpyAsync(p->h_stage_out, p->d_stage_out, out_sz, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(p->h_stage_out + out_sz, p->d_stage_status, (size_t)n_rows * 4, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaEventRecord(p->ev[3], st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    B2S_CUDA_TRY(cudaEventRecord(p->ev[2], st));
+    B2S_CUDA_TRY(cudaMemcpyAsync(p->h_stage_out, p->d_stage_out, out_sz, cudaMemcpyDeviceToHost, st));
+    B2S_CUDA_TRY(cudaMemcpyAsync(p->h_stage_out + out_sz, p->d_stage_status, (size_t)n_rows * 4, cudaMemcpyDeviceToHost, st));
+    B2S_CUDA_TRY(cudaEventRecord(p->ev[3], st));
+    B2S_CUDA_TRY(cudaStreamSynchronize(st));
     memcpy(out, p->h_stage_out, out_sz);
     const int32_t* hs = (const int32_t*)(p->h_stage_out + out_sz);
     int bad = 0;
@@ -2035,13 +2028,13 @@ extern "C" int b2s_time_device(b2s_plan_t p, const void* const* d_rows, int32_t 
     if (!p || !p->finalized) return fail(B2S_ERR_STATE, "plan not finalized");
     if (n_bufs < 1 || n_iters < 1 || !total_ms) return fail(B2S_ERR_INVALID, "bad arguments");
     cudaStream_t st = G.stream;
-    CUDA_TRY(cudaStreamSynchronize(st));
-    CUDA_TRY(cudaEventRecord(p->ev[0], st));
+    B2S_CUDA_TRY(cudaStreamSynchronize(st));
+    B2S_CUDA_TRY(cudaEventRecord(p->ev[0], st));
     for (int i = 0; i < n_iters; ++i)
       if (int rc = launch_on(p, d_rows[i % n_bufs], n_rows, row_stride_bytes, d_out, nullptr, st)) return rc;
-    CUDA_TRY(cudaEventRecord(p->ev[1], st));
-    CUDA_TRY(cudaEventSynchronize(p->ev[1]));
-    CUDA_TRY(cudaEventElapsedTime(total_ms, p->ev[0], p->ev[1]));
+    B2S_CUDA_TRY(cudaEventRecord(p->ev[1], st));
+    B2S_CUDA_TRY(cudaEventSynchronize(p->ev[1]));
+    B2S_CUDA_TRY(cudaEventElapsedTime(total_ms, p->ev[0], p->ev[1]));
     return B2S_OK;
   } catch (const std::exception& e) {
     return fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
@@ -2195,7 +2188,7 @@ static void ring_free_slot(Slot& s) {
 
 static int ring_start(b2s_plan_s* p) {
   if (!p->slots.empty()) return B2S_OK;
-  CUDA_TRY(cudaSetDevice(G.device));
+  B2S_CUDA_TRY(cudaSetDevice(G.device));
   // built aside and committed only when everything (buffers, events, stream, dispatcher) exists: a failure leaves the
   // plan without a ring, so the next submit retries instead of queueing rows nobody will ever dispatch
   const int64_t cap = p->ring_cfg_max_batch > 0 ? p->ring_cfg_max_batch : G.max_batch;
@@ -2523,7 +2516,7 @@ extern "C" int b2s_plan_set_merge_targets(b2s_plan_t p, void* const* peer_out, i
 extern "C" int b2s_ipc_export(void* dptr, void* handle64) {
   try {  // no C++ exception crosses the C boundary
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
-    CUDA_TRY(cudaIpcGetMemHandle(reinterpret_cast<cudaIpcMemHandle_t*>(handle64), dptr));
+    B2S_CUDA_TRY(cudaIpcGetMemHandle(reinterpret_cast<cudaIpcMemHandle_t*>(handle64), dptr));
     return B2S_OK;
   } catch (const std::exception& e) {
     return fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
@@ -2533,7 +2526,7 @@ extern "C" int b2s_ipc_open(const void* handle64, void** dptr_out) {
   try {  // no C++ exception crosses the C boundary
     cudaIpcMemHandle_t h;
     memcpy(&h, handle64, sizeof(h));
-    CUDA_TRY(cudaIpcOpenMemHandle(dptr_out, h, cudaIpcMemLazyEnablePeerAccess));
+    B2S_CUDA_TRY(cudaIpcOpenMemHandle(dptr_out, h, cudaIpcMemLazyEnablePeerAccess));
     return B2S_OK;
   } catch (const std::exception& e) {
     return fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
@@ -2541,7 +2534,7 @@ extern "C" int b2s_ipc_open(const void* handle64, void** dptr_out) {
 }
 extern "C" int b2s_ipc_close(void* dptr) {
   try {  // no C++ exception crosses the C boundary
-    CUDA_TRY(cudaIpcCloseMemHandle(dptr));
+    B2S_CUDA_TRY(cudaIpcCloseMemHandle(dptr));
     return B2S_OK;
   } catch (const std::exception& e) {
     return fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
@@ -2580,9 +2573,9 @@ extern "C" int b2s_comm_create(int32_t rank, int32_t world, int64_t max_rows_per
     c->out_cols = out_cols;
     c->max_rows = (max_rows_per_rank + 3) / 4 * 4;  // row blocks start 16-byte aligned
     c->bytes = kCommHeader + kCommSlots * c->buf_bytes();
-    CUDA_TRY(cudaSetDevice(G.device));
-    CUDA_TRY(cudaMalloc(&c->base, c->bytes));
-    CUDA_TRY(cudaMemset(c->base, 0, 512 < c->bytes ? 512 : c->bytes));
+    B2S_CUDA_TRY(cudaSetDevice(G.device));
+    B2S_CUDA_TRY(cudaMalloc(&c->base, c->bytes));
+    B2S_CUDA_TRY(cudaMemset(c->base, 0, 512 < c->bytes ? 512 : c->bytes));
     c->peer_base.assign(world, nullptr);
     c->peer_base[rank] = c->base;
     if (world == 1) c->connected = true;
@@ -2596,7 +2589,7 @@ extern "C" int b2s_comm_create(int32_t rank, int32_t world, int64_t max_rows_per
 extern "C" int b2s_comm_handle(b2s_comm_t c, void* handle64) {
   try {
     if (!c || !handle64) return fail(B2S_ERR_INVALID, "null communicator");
-    CUDA_TRY(cudaIpcGetMemHandle(reinterpret_cast<cudaIpcMemHandle_t*>(handle64), c->base));
+    B2S_CUDA_TRY(cudaIpcGetMemHandle(reinterpret_cast<cudaIpcMemHandle_t*>(handle64), c->base));
     return B2S_OK;
   } catch (const std::exception& e) {
     return fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
@@ -2612,7 +2605,7 @@ extern "C" int b2s_comm_connect(b2s_comm_t c, const void* all_handles) {
       cudaIpcMemHandle_t h;
       memcpy(&h, (const char*)all_handles + (size_t)r * 64, 64);
       void* ptr = nullptr;
-      CUDA_TRY(cudaIpcOpenMemHandle(&ptr, h, cudaIpcMemLazyEnablePeerAccess));
+      B2S_CUDA_TRY(cudaIpcOpenMemHandle(&ptr, h, cudaIpcMemLazyEnablePeerAccess));
       c->peer_base[r] = (char*)ptr;
     }
     c->connected = true;
@@ -2707,7 +2700,7 @@ extern "C" int b2s_comm_check(b2s_comm_t c) {
   try {  // after a stream synchronisation: did a wait give up on a peer?
     if (!c) return fail(B2S_ERR_INVALID, "null communicator");
     uint32_t v = 0;
-    CUDA_TRY(cudaMemcpy(&v, reinterpret_cast<uint32_t*>(c->base) + 65, 4, cudaMemcpyDeviceToHost));
+    B2S_CUDA_TRY(cudaMemcpy(&v, reinterpret_cast<uint32_t*>(c->base) + 65, 4, cudaMemcpyDeviceToHost));
     if (v) return fail(B2S_ERR_TIMEOUT, "ensemble-merge: rank %u did not signal its shard in time (B2S_COMM_TIMEOUT_MS)", v - 1);
     return B2S_OK;
   } catch (const std::exception& e) {
@@ -2739,7 +2732,7 @@ extern "C" void* b2s_alloc_pinned(size_t bytes) {
 }
 extern "C" int b2s_free_pinned(void* p) {
   try {  // no C++ exception crosses the C boundary
-    CUDA_TRY(cudaFreeHost(p));
+    B2S_CUDA_TRY(cudaFreeHost(p));
     return B2S_OK;
   } catch (const std::exception& e) {
     return fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
@@ -2755,7 +2748,7 @@ extern "C" void* b2s_device_alloc(size_t bytes) {
 }
 extern "C" int b2s_device_free(void* p) {
   try {  // no C++ exception crosses the C boundary
-    CUDA_TRY(cudaFree(p));
+    B2S_CUDA_TRY(cudaFree(p));
     return B2S_OK;
   } catch (const std::exception& e) {
     return fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
@@ -2767,8 +2760,8 @@ extern "C" int b2s_memcpy_h2d(void* d, const void* h, size_t bytes) {
     // (non-blocking) library stream that launches the kernels is not ordered behind the legacy stream -- a kernel launched
     // right after the call read the tail of the previous batch (found by the 2-GPU test of ShardedGraphServer, r2n)
     cudaStream_t st = G.inited ? G.stream : (cudaStream_t)0;
-    CUDA_TRY(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    B2S_CUDA_TRY(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, st));
+    B2S_CUDA_TRY(cudaStreamSynchronize(st));
     return B2S_OK;
   } catch (const std::exception& e) {
     return fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
@@ -2777,8 +2770,8 @@ extern "C" int b2s_memcpy_h2d(void* d, const void* h, size_t bytes) {
 extern "C" int b2s_memcpy_d2h(void* h, const void* d, size_t bytes) {
   try {  // no C++ exception crosses the C boundary
     cudaStream_t st = G.inited ? G.stream : (cudaStream_t)0;  // ordered behind the kernels of the library stream
-    CUDA_TRY(cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    B2S_CUDA_TRY(cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, st));
+    B2S_CUDA_TRY(cudaStreamSynchronize(st));
     return B2S_OK;
   } catch (const std::exception& e) {
     return fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
@@ -2786,7 +2779,7 @@ extern "C" int b2s_memcpy_d2h(void* h, const void* d, size_t bytes) {
 }
 extern "C" int b2s_device_sync(void) {
   try {  // no C++ exception crosses the C boundary
-    CUDA_TRY(cudaDeviceSynchronize());
+    B2S_CUDA_TRY(cudaDeviceSynchronize());
     return B2S_OK;
   } catch (const std::exception& e) {
     return fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());

@@ -8,6 +8,7 @@
 
 #include "../../include/b200serve.h"
 #include "b2s_internal.h"
+#include "b2s_stage.h"
 
 namespace b2s_sort {
 
@@ -25,13 +26,6 @@ __host__ __device__ inline uint32_t radix_digit(uint64_t key, int shift) {
 }
 
 }  // namespace b2s_sort
-
-#define SORT_TRY(expr)                                                                                                 \
-  do {                                                                                                                 \
-    cudaError_t _e = (expr);                                                                                           \
-    if (_e != cudaSuccess)                                                                                             \
-      return b2s_int_fail(B2S_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
-  } while (0)
 
 namespace {
 
@@ -121,16 +115,39 @@ __global__ void __launch_bounds__(kSortThreads) radix_scatter_kernel(const uint6
   }
 }
 
+// the sort's buffers, allocated on stream st and freed on it when they leave scope
 struct SortBufs {
-  uint64_t* k[2];
-  uint32_t* v[2];
-  uint32_t* hist;
+  explicit SortBufs(cudaStream_t s) : st(s) {}
+  SortBufs(const SortBufs&) = delete;
+  SortBufs& operator=(const SortBufs&) = delete;
+  ~SortBufs() {
+    for (int i = 0; i < 2; ++i) {
+      if (k[i]) cudaFreeAsync(k[i], st);
+      if (v[i]) cudaFreeAsync(v[i], st);
+    }
+    if (hist) cudaFreeAsync(hist, st);
+  }
+  int alloc(int64_t n) {
+    const int64_t n_blocks = (n + kSortTile - 1) / kSortTile;
+    for (int i = 0; i < 2; ++i) {
+      B2S_CUDA_TRY(cudaMallocAsync(&k[i], n * 8, st));
+      B2S_CUDA_TRY(cudaMallocAsync(&v[i], n * 4, st));
+    }
+    B2S_CUDA_TRY(cudaMallocAsync(&hist, n_blocks * 256 * 4, st));
+    return B2S_OK;
+  }
+
+  cudaStream_t st;
+  uint64_t* k[2] = {};
+  uint32_t* v[2] = {};
+  uint32_t* hist = nullptr;
 };
 
 // stable sort of k[0] (signed 64-bit keys) carrying v[0] (null: the payload is the input position); the result ends in
 // k[0] / v[0] (an even number of passes)
-int radix_sort(SortBufs& b, bool payload, int64_t n, cudaStream_t st) {
+int radix_sort(SortBufs& b, bool payload, int64_t n, Launches& launches) {
   const int n_blocks = (int)((n + kSortTile - 1) / kSortTile);
+  const cudaStream_t st = b.st;
   for (int pass = 0; pass < 8; ++pass) {
     const int src = pass & 1, shift = pass * 8;
     radix_hist_kernel<<<n_blocks, kSortThreads, 0, st>>>(b.k[src], n, shift, b.hist, n_blocks);
@@ -138,30 +155,17 @@ int radix_sort(SortBufs& b, bool payload, int64_t n, cudaStream_t st) {
     radix_scatter_kernel<<<n_blocks, kSortThreads, 0, st>>>(b.k[src], (pass == 0 && !payload) ? nullptr : b.v[src], b.k[src ^ 1],
                                                             b.v[src ^ 1], n, shift, b.hist, n_blocks);
   }
-  b2s_int_count_launches(24);
+  launches.add(24);
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return b2s_int_fail(B2S_ERR_CUDA, "radix sort launch failed: %s", cudaGetErrorString(e));
   return B2S_OK;
 }
 
-int alloc_sort(SortBufs& b, int64_t n, cudaStream_t st) {
-  const int64_t n_blocks = (n + kSortTile - 1) / kSortTile;
-  b = SortBufs{};
-  for (int i = 0; i < 2; ++i) {
-    SORT_TRY(cudaMallocAsync(&b.k[i], n * 8, st));
-    SORT_TRY(cudaMallocAsync(&b.v[i], n * 4, st));
-  }
-  SORT_TRY(cudaMallocAsync(&b.hist, n_blocks * 256 * 4, st));
-  return B2S_OK;
-}
-
-void free_sort(SortBufs& b, cudaStream_t st) {
-  for (int i = 0; i < 2; ++i) {
-    if (b.k[i]) cudaFreeAsync(b.k[i], st);
-    if (b.v[i]) cudaFreeAsync(b.v[i], st);
-  }
-  if (b.hist) cudaFreeAsync(b.hist, st);
-  b = SortBufs{};
+// the n signed keys at d_keys (device memory) in order: b.k[0] ends as the sorted keys, b.v[0] as their input positions
+int sort_keys(SortBufs& b, const int64_t* d_keys, int64_t n, Launches& launches) {
+  if (int rc = b.alloc(n)) return rc;
+  B2S_CUDA_TRY(cudaMemcpyAsync(b.k[0], d_keys, n * 8, cudaMemcpyDeviceToDevice, b.st));
+  return radix_sort(b, false, n, launches);
 }
 
 }  // namespace

@@ -25,13 +25,6 @@
 #include "b2s_internal.h"
 #include "b2s_hash.cuh"
 
-#define TAB_TRY(expr)                                                                                       \
-  do {                                                                                                      \
-    cudaError_t _e = (expr);                                                                                \
-    if (_e != cudaSuccess)                                                                                  \
-      return b2s_int_fail(B2S_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
-  } while (0)
-
 namespace {
 
 using Slot = b2s::TableSlot;
@@ -181,15 +174,15 @@ extern "C" int b2s_table_create(const int64_t* keys, int64_t n_keys, const float
     t->n_keys = n_keys;
     t->n_feat = n_features;
     t->cap = cap;
-    TAB_TRY(cudaSetDevice(b2s_int_device()));
-    TAB_TRY(cudaMalloc(&t->d_slots, cap * sizeof(Slot)));
-    TAB_TRY(cudaMemcpy(t->d_slots, slots.data(), cap * sizeof(Slot), cudaMemcpyHostToDevice));
+    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
+    B2S_CUDA_TRY(cudaMalloc(&t->d_slots, cap * sizeof(Slot)));
+    B2S_CUDA_TRY(cudaMemcpy(t->d_slots, slots.data(), cap * sizeof(Slot), cudaMemcpyHostToDevice));
     // one more row than keys: row n_keys is all NaN, what the fused gather copies for an unknown key
-    TAB_TRY(cudaMalloc(&t->d_values, ((size_t)n_keys + 1) * n_features * 4));
-    TAB_TRY(cudaMemcpy(t->d_values, values, (size_t)n_keys * n_features * 4, cudaMemcpyHostToDevice));
+    B2S_CUDA_TRY(cudaMalloc(&t->d_values, ((size_t)n_keys + 1) * n_features * 4));
+    B2S_CUDA_TRY(cudaMemcpy(t->d_values, values, (size_t)n_keys * n_features * 4, cudaMemcpyHostToDevice));
     {
       const std::vector<float> nan_row((size_t)n_features, NAN);
-      TAB_TRY(cudaMemcpy(t->d_values + (size_t)n_keys * n_features, nan_row.data(), (size_t)n_features * 4, cudaMemcpyHostToDevice));
+      B2S_CUDA_TRY(cudaMemcpy(t->d_values + (size_t)n_keys * n_features, nan_row.data(), (size_t)n_features * 4, cudaMemcpyHostToDevice));
     }
     std::vector<float> imp(((size_t)n_features + 3) / 4 * 4, NAN);
     if (impute)
@@ -198,12 +191,12 @@ extern "C" int b2s_table_create(const int64_t* keys, int64_t n_keys, const float
         if (impute[c] == impute[c]) t->any_impute = 1;
       }
     t->h_impute = imp;
-    TAB_TRY(cudaMalloc(&t->d_impute, imp.size() * 4));
-    TAB_TRY(cudaMemcpy(t->d_impute, imp.data(), imp.size() * 4, cudaMemcpyHostToDevice));
+    B2S_CUDA_TRY(cudaMalloc(&t->d_impute, imp.size() * 4));
+    B2S_CUDA_TRY(cudaMemcpy(t->d_impute, imp.data(), imp.size() * 4, cudaMemcpyHostToDevice));
     int occ = 0;
-    TAB_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, table_lookup_kernel, 256, 0));
+    B2S_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, table_lookup_kernel, 256, 0));
     t->grid = b2s_int_sm_count() * std::max(occ, 1);
-    for (int i = 0; i < 4; ++i) TAB_TRY(cudaEventCreate(&t->ev[i]));
+    for (int i = 0; i < 4; ++i) B2S_CUDA_TRY(cudaEventCreate(&t->ev[i]));
     *out = t;
     return B2S_OK;
   } catch (const std::exception& e) {
@@ -242,8 +235,6 @@ static int launch_lookup(b2s_table_t t, const int64_t* d_keys, int64_t n, float*
 
 // the kernels load keys as 8-byte words and store rows, flags and status words as 4-byte words (rows also as 16-byte
 // words where the base allows): a pointer off those boundaries is refused before anything is launched
-static bool misaligned(const void* ptr, uintptr_t bytes) { return ((uintptr_t)ptr & (bytes - 1)) != 0; }
-
 extern "C" int b2s_table_lookup_device(b2s_table_t t, const int64_t* d_keys, int64_t n, float* d_rows, int64_t row_stride_bytes,
                                        int32_t* d_found, void* stream) {
   try {  // no C++ exception crosses the C boundary
@@ -253,7 +244,7 @@ extern "C" int b2s_table_lookup_device(b2s_table_t t, const int64_t* d_keys, int
     if (misaligned(d_keys, 8) || misaligned(d_rows, 4) || misaligned(d_found, 4))
       return b2s_int_fail(B2S_ERR_INVALID, "keys must be 8-byte aligned, rows and found 4-byte aligned");
     if (n == 0) return B2S_OK;
-    TAB_TRY(cudaSetDevice(b2s_int_device()));
+    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
     return launch_lookup(t, d_keys, n, d_rows, row_stride_bytes, d_found, stream ? (cudaStream_t)stream : b2s_int_stream());
   } catch (const std::exception& e) {
     return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
@@ -265,27 +256,27 @@ extern "C" int b2s_table_lookup_host(b2s_table_t t, const int64_t* keys, int64_t
     if (!t || !keys || !rows || n < 0) return b2s_int_fail(B2S_ERR_INVALID, "bad arguments");
     if (n == 0) return B2S_OK;
     std::lock_guard<std::mutex> lk(t->mu);
-    TAB_TRY(cudaSetDevice(b2s_int_device()));
+    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
     if (n > t->cap_rows) {
       if (t->d_keys) { cudaFree(t->d_keys); cudaFree(t->d_out); cudaFree(t->d_found); t->d_keys = nullptr; }
       t->cap_rows = 0;
       const int64_t cap = std::max<int64_t>(n, 4096);
-      TAB_TRY(cudaMalloc(&t->d_keys, cap * 8));
-      TAB_TRY(cudaMalloc(&t->d_out, (size_t)cap * t->n_feat * 4));
-      TAB_TRY(cudaMalloc(&t->d_found, cap * 4));
+      B2S_CUDA_TRY(cudaMalloc(&t->d_keys, cap * 8));
+      B2S_CUDA_TRY(cudaMalloc(&t->d_out, (size_t)cap * t->n_feat * 4));
+      B2S_CUDA_TRY(cudaMalloc(&t->d_found, cap * 4));
       t->cap_rows = cap;
     }
     cudaStream_t st = b2s_int_stream();
     const int64_t stride = (int64_t)t->n_feat * 4;
-    TAB_TRY(cudaEventRecord(t->ev[0], st));
-    TAB_TRY(cudaMemcpyAsync(t->d_keys, keys, n * 8, cudaMemcpyHostToDevice, st));
-    TAB_TRY(cudaEventRecord(t->ev[1], st));
+    B2S_CUDA_TRY(cudaEventRecord(t->ev[0], st));
+    B2S_CUDA_TRY(cudaMemcpyAsync(t->d_keys, keys, n * 8, cudaMemcpyHostToDevice, st));
+    B2S_CUDA_TRY(cudaEventRecord(t->ev[1], st));
     if (int rc = launch_lookup(t, t->d_keys, n, t->d_out, stride, t->d_found, st)) return rc;
-    TAB_TRY(cudaEventRecord(t->ev[2], st));
-    TAB_TRY(cudaMemcpyAsync(rows, t->d_out, (size_t)n * stride, cudaMemcpyDeviceToHost, st));
-    if (found) TAB_TRY(cudaMemcpyAsync(found, t->d_found, n * 4, cudaMemcpyDeviceToHost, st));
-    TAB_TRY(cudaEventRecord(t->ev[3], st));
-    TAB_TRY(cudaStreamSynchronize(st));
+    B2S_CUDA_TRY(cudaEventRecord(t->ev[2], st));
+    B2S_CUDA_TRY(cudaMemcpyAsync(rows, t->d_out, (size_t)n * stride, cudaMemcpyDeviceToHost, st));
+    if (found) B2S_CUDA_TRY(cudaMemcpyAsync(found, t->d_found, n * 4, cudaMemcpyDeviceToHost, st));
+    B2S_CUDA_TRY(cudaEventRecord(t->ev[3], st));
+    B2S_CUDA_TRY(cudaStreamSynchronize(st));
     if (stats) {
       memset(stats, 0, sizeof(*stats));
       stats->rows = n;
@@ -320,7 +311,7 @@ extern "C" int b2s_table_enrich_device(b2s_table_t t, b2s_plan_t plan, const int
     if (misaligned(d_keys, 8) || misaligned(d_out, 4) || misaligned(d_status, 4))
       return b2s_int_fail(B2S_ERR_INVALID, "keys must be 8-byte aligned, out and status 4-byte aligned");
     if (n == 0) return B2S_OK;
-    TAB_TRY(cudaSetDevice(b2s_int_device()));
+    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
     return launch_fused(t, plan, d_keys, n, d_out, d_status, stream ? (cudaStream_t)stream : b2s_int_stream());
   } catch (const std::exception& e) {
     return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
@@ -344,15 +335,15 @@ extern "C" int b2s_table_enrich_host(b2s_table_t t, b2s_plan_t plan, const int64
     if (out_bytes < n * out_cols * 4) return b2s_int_fail(B2S_ERR_INVALID, "out buffer too small");
     if (n == 0) return B2S_OK;
     std::lock_guard<std::mutex> lk(t->mu);
-    TAB_TRY(cudaSetDevice(b2s_int_device()));
+    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
     const int64_t stride = (int64_t)t->n_feat * 4;
     if (n > t->cap_rows) {
       if (t->d_keys) { cudaFree(t->d_keys); cudaFree(t->d_out); cudaFree(t->d_found); t->d_keys = nullptr; }
       t->cap_rows = 0;
       const int64_t cap = std::max<int64_t>(n, 4096);
-      TAB_TRY(cudaMalloc(&t->d_keys, cap * 8));
-      TAB_TRY(cudaMalloc(&t->d_out, (size_t)cap * stride));
-      TAB_TRY(cudaMalloc(&t->d_found, cap * 4));
+      B2S_CUDA_TRY(cudaMalloc(&t->d_keys, cap * 8));
+      B2S_CUDA_TRY(cudaMalloc(&t->d_out, (size_t)cap * stride));
+      B2S_CUDA_TRY(cudaMalloc(&t->d_found, cap * 4));
       t->cap_rows = cap;
     }
     if (n > t->enr_rows || out_cols > t->enr_out_cols) {
@@ -360,9 +351,9 @@ extern "C" int b2s_table_enrich_host(b2s_table_t t, b2s_plan_t plan, const int64
       t->enr_rows = 0;
       const int64_t cap = std::max<int64_t>(n, 4096);
       const int32_t oc = std::max(out_cols, t->enr_out_cols);
-      TAB_TRY(cudaMalloc(&t->d_votes, (size_t)cap * oc * 4));
-      TAB_TRY(cudaMalloc(&t->d_status, cap * 4));
-      TAB_TRY(cudaMallocHost(&t->h_pin, (size_t)cap * (8 + (size_t)oc * 4 + 4)));
+      B2S_CUDA_TRY(cudaMalloc(&t->d_votes, (size_t)cap * oc * 4));
+      B2S_CUDA_TRY(cudaMalloc(&t->d_status, cap * 4));
+      B2S_CUDA_TRY(cudaMallocHost(&t->h_pin, (size_t)cap * (8 + (size_t)oc * 4 + 4)));
       t->enr_rows = cap;
       t->enr_out_cols = oc;
     }
@@ -379,9 +370,9 @@ extern "C" int b2s_table_enrich_host(b2s_table_t t, b2s_plan_t plan, const int64
     }
     void* v_dst = host_pinned(out) ? out : (void*)h_votes;
     int32_t* s_dst = row_status ? (host_pinned(row_status) ? row_status : h_status) : nullptr;
-    TAB_TRY(cudaEventRecord(t->ev[0], st));
-    TAB_TRY(cudaMemcpyAsync(t->d_keys, k_src, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-    TAB_TRY(cudaEventRecord(t->ev[1], st));
+    B2S_CUDA_TRY(cudaEventRecord(t->ev[0], st));
+    B2S_CUDA_TRY(cudaMemcpyAsync(t->d_keys, k_src, (size_t)n * 8, cudaMemcpyHostToDevice, st));
+    B2S_CUDA_TRY(cudaEventRecord(t->ev[1], st));
     int n_kernels = 1;
     int rc = launch_fused(t, plan, t->d_keys, n, t->d_votes, t->d_status, st);  // gather inside the scoring kernel
     if (rc == B2S_ERR_UNSUPPORTED) {  // plans the gather loader does not cover: gather, score, fold the flags (3 launches)
@@ -396,11 +387,11 @@ extern "C" int b2s_table_enrich_host(b2s_table_t t, b2s_plan_t plan, const int64
     } else if (rc) {
       return rc;
     }
-    TAB_TRY(cudaEventRecord(t->ev[2], st));
-    TAB_TRY(cudaMemcpyAsync(v_dst, t->d_votes, votes_sz, cudaMemcpyDeviceToHost, st));
-    if (s_dst) TAB_TRY(cudaMemcpyAsync(s_dst, t->d_status, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
-    TAB_TRY(cudaEventRecord(t->ev[3], st));
-    TAB_TRY(cudaStreamSynchronize(st));
+    B2S_CUDA_TRY(cudaEventRecord(t->ev[2], st));
+    B2S_CUDA_TRY(cudaMemcpyAsync(v_dst, t->d_votes, votes_sz, cudaMemcpyDeviceToHost, st));
+    if (s_dst) B2S_CUDA_TRY(cudaMemcpyAsync(s_dst, t->d_status, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+    B2S_CUDA_TRY(cudaEventRecord(t->ev[3], st));
+    B2S_CUDA_TRY(cudaStreamSynchronize(st));
     if (v_dst != out) memcpy(out, h_votes, votes_sz);
     if (s_dst && s_dst != row_status) memcpy(row_status, h_status, (size_t)n * 4);
     if (stats) {
@@ -423,15 +414,15 @@ extern "C" int b2s_table_time_device(b2s_table_t t, const int64_t* const* d_keys
                                      int64_t row_stride_bytes, int32_t* d_found, int32_t n_iters, float* total_ms) {
   try {  // no C++ exception crosses the C boundary
     if (!t || !d_keys || n_bufs <= 0 || n_iters <= 0 || !total_ms) return b2s_int_fail(B2S_ERR_INVALID, "bad arguments");
-    TAB_TRY(cudaSetDevice(b2s_int_device()));
+    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
     cudaStream_t st = b2s_int_stream();
     std::lock_guard<std::mutex> lk(t->mu);
-    TAB_TRY(cudaEventRecord(t->ev[0], st));
+    B2S_CUDA_TRY(cudaEventRecord(t->ev[0], st));
     for (int i = 0; i < n_iters; ++i)
       if (int rc = launch_lookup(t, d_keys[i % n_bufs], n, d_rows, row_stride_bytes, d_found, st)) return rc;
-    TAB_TRY(cudaEventRecord(t->ev[1], st));
-    TAB_TRY(cudaStreamSynchronize(st));
-    TAB_TRY(cudaEventElapsedTime(total_ms, t->ev[0], t->ev[1]));
+    B2S_CUDA_TRY(cudaEventRecord(t->ev[1], st));
+    B2S_CUDA_TRY(cudaStreamSynchronize(st));
+    B2S_CUDA_TRY(cudaEventElapsedTime(total_ms, t->ev[0], t->ev[1]));
     return B2S_OK;
   } catch (const std::exception& e) {
     return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
