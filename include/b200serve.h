@@ -498,7 +498,8 @@ int b2s_pit_train_host(const int64_t* ts, int64_t n, const b2s_pit_set* sets, in
  * 715-851), emitting every event: row i gains, per (operation, window), the aggregate over the rows j <= i (input order)
  * of its 64-bit key whose timestamps lie in row i's window.  Windows are aligned to the epoch (floor division, so that
  * rows before 1970 are right): sliding (period_ns > 0, dividing every window): b(t) = floor(t / period), row j is in
- * when b(t_j) >= b(t_i) - window / period + 1; fixed (period_ns = 0): floor(t_j / window) == floor(t_i / window).
+ * when b(t_j) >= b(t_i) - window / period + 1; fixed (period_ns = 0): floor(t_j / window) == floor(t_i / window).  A
+ * window's first timestamp is clamped at INT64_MIN where it would leave the int64 range (near 1677, at any period).
  * Sums accumulate in fp64 over the window's rows alone (a range reduce, never a difference of running sums); stdvar is
  * the sample variance from a pairwise (count, mean, M2) combine, NaN for a window of one row; first is the window's
  * earliest row in input order, last the row itself.  Every output is [n] float64 in input order. */

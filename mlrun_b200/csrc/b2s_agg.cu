@@ -255,8 +255,9 @@ __global__ void __launch_bounds__(kThreads) reduce_kernel(const __grid_constant_
     for (int w = 0; w < p.n_windows; ++w) {
       int64_t start;
       if (p.period) {
-        const int64_t b = floor_div(ti, p.period);
-        start = bucket_start(b - p.window[w] / p.period + 1, p.period);
+        // first bucket b - back, clamped before the subtraction: at a 1 ns period it leaves the int64 range near 1677
+        const int64_t b = floor_div(ti, p.period), back = p.window[w] / p.period - 1;
+        start = b < INT64_MIN + back ? INT64_MIN : bucket_start(b - back, p.period);
       } else {
         start = bucket_start(floor_div(ti, p.window[w]), p.window[w]);
       }

@@ -6,10 +6,14 @@ fsum, so they are held to a bound derived from the window's magnitudes: every pa
 through at most 2 log2(n) + 64 combines (the hierarchy's levels, the warp scans, the final loop), so
 
     |sum - ref| <= 128 eps sum|x|,  |sqr - ref| <= 128 eps sum x^2,  |avg - ref| <= 128 eps sum|x| / count,
-    |stdvar - ref| <= 128 eps sum x^2 / (count - 1),  |stddev - ref| <= sqrt(that)
+    |stdvar - ref| <= tol = 128 eps sqrt(sum x^2 M2) / (count - 1),  |stddev - ref| <= tol / (stddev + ref) + 2 eps ref
 
-with eps = 2^-53 and the sums over the window's rows alone.  A prefix-difference implementation fails the cancellation case:
-its running sums carry +-1e30 from rows outside the window.  Every case also checks the launches the call made."""
+with eps = 2^-53, the sums over the window's rows alone and M2 the oracle's two-pass sum of squared deviations.  The variance
+bound follows Chan, Golub and LeVeque: a pairwise (count, mean, M2) combine errs by O(combines kappa eps M2), with
+kappa M2 = sqrt(sum x^2 M2); sum x^2 - (sum x)^2 / count errs by O(eps sum x^2) and fails it once the mean is large against
+the spread (tests/test_agg_ranges_cpu.py).  A window of equal values must give exactly 0.  A prefix-difference
+implementation fails the cancellation case: its running sums carry +-1e30 from rows outside the window.  Every case also
+checks the launches the call made."""
 
 import ctypes as C
 import math
@@ -80,6 +84,18 @@ def run_host(keys, ts, sources, aggs):
     return outs, counters
 
 
+def var_tol(s_sq, m2, cnt):
+    """the stdvar bound: K eps sqrt(sum x^2 M2) / (count - 1), zero for a window of equal values"""
+    return K * EPS * np.sqrt(s_sq * m2) / (cnt - 1)
+
+
+def std_tol(tol_var, got, ref):
+    """the stddev bound from the stdvar bound: |sqrt(u) - sqrt(v)| = |u - v| / (sqrt(u) + sqrt(v)), plus a rounding of each
+    square root"""
+    den = got + ref
+    return np.divide(tol_var, den, out=np.zeros_like(den), where=den > 0) + 2 * EPS * ref
+
+
 def check(keys, ts, sources, aggs, got, rows=None):
     """got vs the oracle on `rows` (all by default): exact ops exactly, the others within the stated bound"""
     want = oa.aggregate(keys, ts, sources, aggs, rows=rows)
@@ -99,12 +115,13 @@ def check(keys, ts, sources, aggs, got, rows=None):
                 cnt = mags[f"{a['name']}_count_{label}"][sel]
                 tol = {"sum": K * EPS * s_abs, "sqr": K * EPS * s_sq, "avg": K * EPS * s_abs / cnt}.get(op)
                 if op in ("stdvar", "stddev"):
-                    tol = K * EPS * s_sq / np.maximum(cnt - 1, 1)
-                    if op == "stddev":
-                        tol = np.sqrt(tol)
                     assert np.array_equal(np.isnan(g), np.isnan(w)) and np.isnan(w[cnt == 1]).all(), name
                     ok = ~np.isnan(w)
-                    g, w, tol = g[ok], w[ok], tol[ok]
+                    g, w, s_sq, cnt = g[ok], w[ok], s_sq[ok], cnt[ok]
+                    m2 = (w if op == "stdvar" else w * w) * (cnt - 1)  # the oracle's two-pass M2
+                    tol = var_tol(s_sq, m2, cnt)
+                    if op == "stddev":
+                        tol = std_tol(tol, g, w)
                 err = np.abs(g - w)
                 assert (err <= tol).all(), (name, float(err.max()), float(tol[np.argmax(err - tol)]))
 
