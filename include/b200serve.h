@@ -209,17 +209,22 @@ int b2s_plan_out_info(b2s_plan_t plan, int32_t* out_cols, int32_t* out_is_int);
  * d_status may be NULL. */
 int b2s_run_device(b2s_plan_t plan, const void* d_rows, int64_t n_rows, int64_t row_stride_bytes, void* d_out,
                    int32_t* d_status, void* stream);
-/* Synchronous host call: pinned staging -> H2D -> kernels -> D2H -> out.  row_status / stats may be NULL.
- * Batches of at most B2S_ZEROCOPY_ROWS (8192) rows skip both copies: the kernels read the rows from (and write the votes
- * to) pinned host memory over PCIe themselves -- one launch and one synchronisation, the latency path of a serving batch;
- * pinned batches of 128 Ki rows and more are pipelined in chunks (copy of chunk c + 1 under the kernels of chunk c). */
+/* Synchronous host call: rows -> kernels -> out.  row_status / stats may be NULL.  Pageable or strided rows are first
+ * packed into the plan's pinned staging area; pinned rows are used where they are.  The kernels write votes and status
+ * words straight to pinned host memory (no D2H copy), and read a batch of at most 64 KiB of rows from pinned host memory
+ * too (no H2D copy: one launch and one synchronisation, the latency path of a serving batch); larger batches are copied
+ * to the device first.  Pinned batches of 128 Ki rows and more are pipelined in chunks of 64 Ki rows or more (copy of
+ * chunk c + 1 under the kernels of chunk c, results copied back per chunk).  A plan with merge targets or an attached
+ * communicator writes no local results: B2S_ERR_UNSUPPORTED, before anything runs (use b2s_run_device). */
 int b2s_run_host(b2s_plan_t plan, const void* rows, int64_t n_rows, int64_t row_stride_bytes, void* out,
                  int64_t out_bytes, int32_t* row_status, b2s_stats* stats);
 /* Coalescing path (thread-safe, many producers): rows are copied into a pinned ring slot; a dispatcher
  * thread seals a batch when it holds max_batch rows or the oldest row waited max_wait_us (0: as soon as the dispatcher is
- * free -- batches form while the previous one runs), and runs it on its own stream (small batches zero-copy, like b2s_run_host).  b2s_wait blocks until the ticket's batch completed and copies
- * that ticket's rows out.  This is the replacement of storey's SyncEmitSource.emit / await_result hand-off
- * (serving/states.py:1283-1287).  A ring slot is recycled when every ticket of its batch was collected, and the ring
+ * free -- batches form while the previous one runs), and runs it on its own stream as one b2s_run_host batch that is
+ * never pipelined (results straight to the slot's pinned memory, rows read from there up to 64 KiB).  b2s_wait blocks
+ * until the ticket's batch completed and copies that ticket's rows out; a batch that failed, or of a plan with merge
+ * targets or an attached communicator (B2S_ERR_UNSUPPORTED), gives every one of its tickets the error.  This is the
+ * replacement of storey's SyncEmitSource.emit / await_result hand-off (serving/states.py:1283-1287).  A ring slot is recycled when every ticket of its batch was collected, and the ring
  * has `ring_slots` (b2s_init cfg, default 4) batches: a producer that keeps submitting without collecting its tickets
  * eventually blocks in b2s_submit -- emit and await per request, as the reference's callers do. */
 int b2s_submit(b2s_plan_t plan, const void* rows, int64_t n_rows, int64_t row_stride_bytes, uint64_t* ticket);
@@ -241,7 +246,8 @@ int b2s_ring_bench(b2s_plan_t plan, const void* rows, int64_t n_src_rows, int64_
  * serving/routers.py:797-810).  The only exchange is the merge of every shard's votes into the full
  * response.  Instead of a separate all-gather, a plan can be given the output buffers of all ranks
  * (peer-mapped over NVLink with the IPC calls below); its kernels then store each output row into every
- * target at row `row_offset + row` straight from the epilogue.  n_peers = 0 restores local output. */
+ * target at row `row_offset + row` straight from the epilogue (b2s_run_device only: b2s_run_host and the ring refuse
+ * the plan).  n_peers = 0 restores local output. */
 int b2s_plan_set_merge_targets(b2s_plan_t plan, void* const* peer_out, int32_t n_peers, int64_t row_offset);
 int b2s_ipc_export(void* dptr, void* handle64 /* 64 bytes out */);
 int b2s_ipc_open(const void* handle64, void** dptr_out);
@@ -252,8 +258,8 @@ int b2s_ipc_close(void* dptr);
  * that can all-gather 64 bytes per rank (torch.distributed, MPI, a file, a socket ...):
  *     b2s_comm_create(rank, world, max_rows_per_rank, out_cols, &c);  b2s_comm_handle(c, mine);
  *     <all-gather the 64-byte handles>;  b2s_comm_connect(c, all);  b2s_plan_attach_comm(plan, c);
- * Every b2s_run_device / b2s_run_host / ring batch of an attached plan is then one STEP (epoch e = 1, 2, ...) of the
- * ensemble-merge (serving/routers.py:414-455 fans the event out to the routes, :789-810 reduces them; here the rows are
+ * Every b2s_run_device launch of an attached plan (the host entry points refuse it) is then one STEP (epoch e = 1, 2,
+ * ...) of the ensemble-merge (serving/routers.py:414-455 fans the event out to the routes, :789-810 reduces them; here the rows are
  * sharded and the votes merged): the kernels store this rank's votes into slot e & 3 of EVERY rank's merged rows at row
  * block `rank`, and the launch's last CTA publishes e in every rank's flag array (st.release.sys).  b2s_comm_wait enqueues
  * a one-warp kernel that acquires all `world` flags of THIS rank at the current epoch, so work enqueued behind it (a D2H copy,

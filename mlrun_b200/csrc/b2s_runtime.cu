@@ -28,28 +28,31 @@
 #include "b2s_rowthread.cuh"
 #include "b2s_trees3.cuh"
 #include "b2s_dense.cuh"
+#include "b2s_stage.h"
 #include <nvtx3/nvToolsExt.h>  // header-only: ranges cost nothing unless a profiler is attached
 
 using namespace b2s;
 
 // ------------------------------------------------------------------------------------------ errors
 static thread_local std::string g_err;
-static int fail(int code, const char* fmt, ...) {
+static int vfail(int code, const char* fmt, va_list ap) {
   char buf[1024];
-  va_list ap;
-  va_start(ap, fmt);
   vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
   g_err = buf;
   return code;
 }
-int b2s_int_fail(int code, const char* fmt, ...) {
-  char buf[1024];
+static int fail(int code, const char* fmt, ...) {
   va_list ap;
   va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
+  vfail(code, fmt, ap);
   va_end(ap);
-  g_err = buf;
+  return code;
+}
+int b2s_int_fail(int code, const char* fmt, ...) {
+  va_list ap;
+  va_start(ap, fmt);
+  vfail(code, fmt, ap);
+  va_end(ap);
   return code;
 }
 // ------------------------------------------------------------------------------------------ globals
@@ -101,16 +104,46 @@ struct HostModel {
   bool any_cat() const { return !node_cat.empty(); }
 };
 
+namespace {
+
+// The buffers and events of one host batch (b2s_run_host, or a slot of the coalescing ring), for up to `rows` rows: the
+// rows in pinned memory (h_in) and on the device (d_in), the results in pinned memory (h_out: out words, then status words
+// from status()) and on the device (d_out, d_status: the chunks of a pipelined b2s_run_host), and the batch's events.
+struct Stage {
+  PinnedArray<char> h_in, h_out;
+  DeviceArray<char> d_in, d_out;
+  DeviceArray<int32_t> d_status;
+  Events ev;  // batch begins, rows are on the device, kernels done
+  int64_t rows = 0;
+  int out_cols = 0;
+
+  int reserve(int64_t n, int64_t row_bytes, int n_out_cols) {
+    if (n <= rows) return B2S_OK;
+    rows = 0;  // until every buffer exists
+    if (!ev.size()) {
+      if (int rc = ev.create(3)) return rc;
+    }
+    out_cols = n_out_cols;
+    if (int rc = allocate(h_in, (size_t)n * row_bytes)) return rc;
+    if (int rc = allocate(h_out, (size_t)n * (out_cols + 1) * 4)) return rc;
+    if (int rc = allocate(d_in, (size_t)n * row_bytes)) return rc;
+    if (int rc = allocate(d_out, (size_t)n * out_cols * 4)) return rc;
+    if (int rc = allocate(d_status, (size_t)n * 4)) return rc;
+    rows = n;
+    return B2S_OK;
+  }
+  int32_t* status() const { return reinterpret_cast<int32_t*>(h_out.get() + (size_t)rows * out_cols * 4); }
+};
+
+struct StreamDestroy {
+  void operator()(cudaStream_t s) const { cudaStreamDestroy(s); }
+};
+
 struct Slot {  // one in-flight batch of the coalescing ring
-  char* h_in = nullptr;
-  char* h_out = nullptr;     // out words then status words
-  char* d_in = nullptr;
-  char* d_out = nullptr;
-  int32_t* d_status = nullptr;
+  Stage stage;
   int64_t rows = 0;
   uint64_t batch_id = 0;
   int state = 0;  // 0 free/open, 1 sealed (queued for the dispatcher), 2 in flight, 3 done
-  cudaEvent_t e0 = nullptr, e1 = nullptr, e2 = nullptr, e3 = nullptr;
   std::chrono::steady_clock::time_point first_submit;
   b2s_stats stats{};
   int waiters = 0;      // tickets issued on this batch not yet collected
@@ -119,6 +152,8 @@ struct Slot {  // one in-flight batch of the coalescing ring
   int err = 0;          // b2s_status of the batch (a failed copy / launch): every ticket of the batch gets it
   std::string err_msg;
 };
+
+}  // namespace
 
 // Ensemble-merge communicator: ONE device allocation per rank, exported over CUDA IPC and mapped by every peer:
 //   [flags: 64 x uint32][CTA counter][timeout word][pad to kCommHeader = 512 B][merged rows, slot 0] .. [merged rows, slot 3]
@@ -130,7 +165,7 @@ constexpr uint32_t kCommSlots = 4;
 struct b2s_comm_s {
   int rank = 0, world = 1, out_cols = 1;
   int64_t max_rows = 0;
-  char* base = nullptr;            // this rank's allocation
+  DeviceArray<char> base;          // this rank's allocation
   std::vector<char*> peer_base;    // [world] every rank's allocation as mapped here (peer_base[rank] == base)
   uint32_t epoch = 0;              // launches signalled so far
   int fused_lag = -1;              // b2s_comm_set_fused_wait: -1 off, 0 / 1: the launches wait in their own last CTA
@@ -140,7 +175,8 @@ struct b2s_comm_s {
   size_t buf_bytes() const { return (size_t)world * max_rows * out_cols * 4; }
   char* buf(int r, uint32_t e) const { return peer_base[r] + kCommHeader + (size_t)(e & (kCommSlots - 1u)) * buf_bytes(); }
   uint32_t* flags(int r) const { return reinterpret_cast<uint32_t*>(peer_base[r]); }
-  uint32_t* counter() const { return reinterpret_cast<uint32_t*>(base) + 64; }
+  uint32_t* counter() const { return reinterpret_cast<uint32_t*>(base.get()) + 64; }
+  uint32_t* timeout_flag() const { return reinterpret_cast<uint32_t*>(base.get()) + 65; }
 };
 
 struct b2s_plan_s {
@@ -160,7 +196,7 @@ struct b2s_plan_s {
   int out_cols = 0;
   int out_is_int = 0;
   KParams kp{};
-  char* d_blob = nullptr;
+  DeviceArray<char> d_blob;
   size_t blob_bytes = 0;
   int grid = 0, block = 0;
   int kernels_per_batch = 1;
@@ -186,29 +222,34 @@ struct b2s_plan_s {
   T3Params t3{};
   T3Prep t3_prep{};
   int t3_prep_smem = 0;
-  char* d_t3_blob = nullptr;
+  DeviceArray<char> d_t3_blob;
   const int32_t* d_t3_col_score = nullptr;
   const int32_t* d_t3_col_order = nullptr;   // the columns by score (t3_vote_kernel)
   const int32_t* d_t3_model_cols = nullptr;  // [n_models + 1] each model's range of d_t3_col_order
   // trees3's partial sums, row flags and transposed tiles: one scratch per stream the plan is launched on
   // (launches on one stream are ordered; the ring's stream, the library stream and caller streams may overlap)
   struct TreeScratch {
-    double* partial = nullptr;   // per-column partial sums, column-major (trees3_kernel -> t3_vote_kernel)
-    int32_t* row_bad = nullptr;  // per-row non-finite input flags (t3_prep_kernel -> t3_vote_kernel)
-    uint32_t* xt = nullptr;      // the batch transposed into tiles (t3_prep_kernel -> trees3_kernel)
+    DeviceArray<double> partial;   // per-column partial sums, column-major (trees3_kernel -> t3_vote_kernel)
+    DeviceArray<int32_t> row_bad;  // per-row non-finite input flags (t3_prep_kernel -> t3_vote_kernel)
+    DeviceArray<uint32_t> xt;      // the batch transposed into tiles (t3_prep_kernel -> trees3_kernel)
     int64_t rows = 0;
+    // room for n rows of `cols` partial-sum columns; cudaFree waits for the work that still reads the old arrays
+    int reserve(int64_t n, int cols, int xt_words) {
+      if (n <= rows) return B2S_OK;
+      rows = 0;
+      const int64_t cap = std::max<int64_t>((n + 63) / 64 * 64, 65536);
+      if (int rc = allocate(partial, (size_t)cap * cols * 8)) return rc;
+      if (int rc = allocate(row_bad, (size_t)cap * 4)) return rc;
+      if (int rc = allocate(xt, (size_t)(cap / kT3TR) * xt_words * 4)) return rc;
+      rows = cap;
+      return B2S_OK;
+    }
   };
   std::map<cudaStream_t, TreeScratch> tree_scratch;
   std::mutex scratch_mu;
-  // host staging for run_host
-  char* h_stage_in = nullptr;
-  char* h_stage_out = nullptr;
-  char* d_stage_in = nullptr;
-  char* d_stage_out = nullptr;
-  int32_t* d_stage_status = nullptr;
-  int64_t stage_rows = 0;
-  cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
-  std::vector<cudaEvent_t> chunk_ev;  // 4 per chunk of a pipelined run_host: copied-in, kernel begin, kernel end, copied-out
+  Stage host_stage;    // b2s_run_host's batch
+  Events ev;           // b2s_time_device: first launch, last launch
+  Events chunk_ev;     // 4 per chunk of a pipelined run_host: copied-in, kernel begin, kernel end, copied-out
   std::mutex host_mu;
   // coalescing ring
   std::vector<Slot> slots;
@@ -221,7 +262,7 @@ struct b2s_plan_s {
   std::thread dispatcher;
   bool stop = false;
   bool dispatch_busy = false;  // a batch is on the ring's stream (run by the dispatcher thread or by a waiting caller)
-  cudaStream_t ring_stream = nullptr;
+  std::unique_ptr<CUstream_st, StreamDestroy> ring_stream;
   int64_t ring_cap = 0;
   // per-plan ring configuration (b2s_plan_set_ring; 0 / negative: the library defaults of b2s_init)
   std::atomic<int> spinners{0};  // waiters currently polling instead of sleeping (b2s_wait)
@@ -1095,13 +1136,13 @@ static int t3_build(b2s_plan_s* p, const KParams& k, bool any_fill) {
   const size_t o_cols = tb.add(col_score), o_order = tb.add(col_order), o_mcols = tb.add(model_cols);
   const size_t o_parts = align_up(tb.data.size(), 16);
   tb.data.resize(o_parts + sizeof(T3Part) * P);
-  B2S_CUDA_TRY(cudaMalloc(&p->d_t3_blob, tb.data.size()));
+  if (int rc = allocate(p->d_t3_blob, tb.data.size())) return rc;
   std::vector<T3Part> dev(P);
   int cta0 = 0;
   for (int i = 0; i < P; ++i) {
     T3Part& d = dev[i];
-    d.nodes = parts[i].n_trees ? (const uint2*)(p->d_t3_blob + o_nodes[i]) : nullptr;
-    d.leaves = (const double*)(p->d_t3_blob + o_leaves[i]);
+    d.nodes = parts[i].n_trees ? (const uint2*)(p->d_t3_blob.get() + o_nodes[i]) : nullptr;
+    d.leaves = (const double*)(p->d_t3_blob.get() + o_leaves[i]);
     d.n_trees = parts[i].n_trees;
     d.n_cols = parts[i].n_cols;
     d.col0 = parts[i].col0;
@@ -1111,14 +1152,14 @@ static int t3_build(b2s_plan_s* p, const KParams& k, bool any_fill) {
     cta0 += n_ctas[i];
   }
   memcpy(tb.data.data() + o_parts, dev.data(), sizeof(T3Part) * P);
-  B2S_CUDA_TRY(cudaMemcpy(p->d_t3_blob, tb.data.data(), tb.data.size(), cudaMemcpyHostToDevice));
-  p->d_t3_col_score = (const int32_t*)(p->d_t3_blob + o_cols);
-  p->d_t3_col_order = (const int32_t*)(p->d_t3_blob + o_order);
-  p->d_t3_model_cols = (const int32_t*)(p->d_t3_blob + o_mcols);
+  B2S_CUDA_TRY(cudaMemcpy(p->d_t3_blob.get(), tb.data.data(), tb.data.size(), cudaMemcpyHostToDevice));
+  p->d_t3_col_score = (const int32_t*)(p->d_t3_blob.get() + o_cols);
+  p->d_t3_col_order = (const int32_t*)(p->d_t3_blob.get() + o_order);
+  p->d_t3_model_cols = (const int32_t*)(p->d_t3_blob.get() + o_mcols);
 
   T3Params& t = p->t3;
   memset(&t, 0, sizeof(t));
-  t.parts = (const T3Part*)(p->d_t3_blob + o_parts);
+  t.parts = (const T3Part*)(p->d_t3_blob.get() + o_parts);
   t.n_in = n_in;
   t.n_parts = P;
   t.warps = W;
@@ -1152,8 +1193,7 @@ static int t3_build(b2s_plan_s* p, const KParams& k, bool any_fill) {
     t.sm_lin_part = alias ? (int32_t)w_end : t.sm_part;
   }
   if (off > (size_t)smem_cap) {  // cannot happen with the budget above; stay on the safe side
-    cudaFree(p->d_t3_blob);
-    p->d_t3_blob = nullptr;
+    p->d_t3_blob.reset();
     return B2S_OK;
   }
   // ---- the prepare kernel: transposed tile | landing tile (TMA boxes or padded rows) | fill | flags | mbarrier
@@ -1179,8 +1219,7 @@ static int t3_build(b2s_plan_s* p, const KParams& k, bool any_fill) {
     pr.sm_bar = ptake(16, 16);
     p->t3_prep_smem = (int)align_up(po, 16);
     if (p->t3_prep_smem > smem_cap) {
-      cudaFree(p->d_t3_blob);
-      p->d_t3_blob = nullptr;
+      p->d_t3_blob.reset();
       return B2S_OK;
     }
   }
@@ -1437,10 +1476,10 @@ extern "C" int b2s_plan_finalize(b2s_plan_t p) {
                  o_troot = bb.add(tree_root), o_tslot = bb.add(tree_slot), o_tscale = bb.add(tree_scale),
                  o_chunk = bb.add(chunk_kind);
     B2S_CUDA_TRY(cudaSetDevice(G.device));
-    B2S_CUDA_TRY(cudaMalloc(&p->d_blob, bb.data.size()));
-    B2S_CUDA_TRY(cudaMemcpy(p->d_blob, bb.data.data(), bb.data.size(), cudaMemcpyHostToDevice));
+    if (int rc = allocate(p->d_blob, bb.data.size())) return rc;
+    B2S_CUDA_TRY(cudaMemcpy(p->d_blob.get(), bb.data.data(), bb.data.size(), cudaMemcpyHostToDevice));
     p->blob_bytes = bb.data.size();
-    char* B = p->d_blob;
+    char* B = p->d_blob.get();
 
     KParams& k = p->kp;
     memset(&k, 0, sizeof(k));
@@ -1644,7 +1683,7 @@ extern "C" int b2s_plan_finalize(b2s_plan_t p) {
     if (p->mode == MODE_TREES && identity_schema && !any_map) {
       if (int rc = t3_build(p, k, any_fill)) return rc;
     }
-    for (int i = 0; i < 4; ++i) B2S_CUDA_TRY(cudaEventCreate(&p->ev[i]));
+    if (int rc = p->ev.create(2)) return rc;
     p->finalized = true;
     return B2S_OK;
   } catch (const std::exception& e) {
@@ -1723,7 +1762,7 @@ static int launch_on(b2s_plan_t p, const void* d_rows, int64_t n_rows, int64_t s
       static const long long fused_timeout_ns = (getenv("B2S_COMM_TIMEOUT_MS") ? atoll(getenv("B2S_COMM_TIMEOUT_MS")) : 10000ll) * 1000000ll;
       k.sig.wait_epoch = e - (uint32_t)c->fused_lag;
       k.sig.wait_flags = c->flags(c->rank);
-      k.sig.timeout_flag = reinterpret_cast<uint32_t*>(c->base) + 65;
+      k.sig.timeout_flag = c->timeout_flag();
       k.sig.timeout_ns = fused_timeout_ns;
       c->fused_epoch = k.sig.wait_epoch;
     }
@@ -1731,29 +1770,25 @@ static int launch_on(b2s_plan_t p, const void* d_rows, int64_t n_rows, int64_t s
   if (p->t3_ok) {
     const int C = p->t3_cols;
     const int64_t n_tiles = (n_rows + kT3TR - 1) / kT3TR;
-    b2s_plan_s::TreeScratch sc;
+    double* partial;
+    int32_t* row_bad;
+    uint32_t* xt;
+    int64_t col_stride;
     {
       std::lock_guard<std::mutex> lk(p->scratch_mu);
       b2s_plan_s::TreeScratch& mine = p->tree_scratch[st];
-      if (n_rows > mine.rows) {  // cudaFree waits for the work that still reads the old buffers
-        if (mine.partial) cudaFree(mine.partial);
-        if (mine.row_bad) cudaFree(mine.row_bad);
-        if (mine.xt) cudaFree(mine.xt);
-        mine = b2s_plan_s::TreeScratch{};
-        const int64_t cap = std::max<int64_t>(align_up((size_t)n_rows, 64), 65536);
-        B2S_CUDA_TRY(cudaMalloc(&mine.partial, (size_t)cap * C * 8));
-        B2S_CUDA_TRY(cudaMalloc(&mine.row_bad, (size_t)cap * 4));
-        B2S_CUDA_TRY(cudaMalloc(&mine.xt, (size_t)(cap / kT3TR) * p->t3.xt_words * 4));
-        mine.rows = cap;
-      }
-      sc = mine;
+      if (int rc = mine.reserve(n_rows, C, p->t3.xt_words)) return rc;
+      partial = mine.partial.get();
+      row_bad = mine.row_bad.get();
+      xt = mine.xt.get();
+      col_stride = mine.rows;
     }
     T3Prep pr = p->t3_prep;
     pr.rows = (const char*)d_rows;
     pr.row_stride = stride;
     pr.n_rows = n_rows;
-    pr.xt = sc.xt;
-    pr.row_bad = sc.row_bad;
+    pr.xt = xt;
+    pr.row_bad = row_bad;
     pr.vec_ok = k.vec_ok;
     alignas(64) CUtensorMap tmap;
     memset(&tmap, 0, sizeof(tmap));
@@ -1766,14 +1801,14 @@ static int launch_on(b2s_plan_t p, const void* d_rows, int64_t n_rows, int64_t s
     cudaError_t e3 = t3_launch_prep(pr, tmap, p->t3_miss, pgrid, p->t3_prep_smem, (int)G.prop.sharedMemPerBlockOptin, st);
     if (e3 != cudaSuccess) return fail(B2S_ERR_CUDA, "tree prepare kernel launch failed: %s", cudaGetErrorString(e3));
     T3Params t = p->t3;
-    t.xt = sc.xt;
+    t.xt = xt;
     t.n_rows = n_rows;
-    t.partial = sc.partial;
-    t.col_stride = sc.rows;
+    t.partial = partial;
+    t.col_stride = col_stride;
     e3 = t3_launch_walk(t, p->t3_D, p->t3_miss, p->t3_cat, p->t3_grid, p->t3_block, p->t3_smem, (int)G.prop.sharedMemPerBlockOptin, st);
     if (e3 != cudaSuccess) return fail(B2S_ERR_CUDA, "tree kernel launch failed: %s", cudaGetErrorString(e3));
     const int vgrid = (int)std::max<int64_t>(1, std::min<int64_t>(4 * G.prop.multiProcessorCount, (n_rows + 255) / 256));
-    e3 = t3_launch_vote(k, sc.partial, sc.rows, p->d_t3_col_score, p->d_t3_col_order, p->d_t3_model_cols, sc.row_bad, vgrid, st);
+    e3 = t3_launch_vote(k, partial, col_stride, p->d_t3_col_score, p->d_t3_col_order, p->d_t3_model_cols, row_bad, vgrid, st);
     if (e3 != cudaSuccess) return fail(B2S_ERR_CUDA, "vote kernel launch failed: %s", cudaGetErrorString(e3));
     return B2S_OK;
   }
@@ -1843,29 +1878,17 @@ int b2s_int_launch_gathered(b2s_plan_s* p, const B2SGather& g, long long n, void
   return B2S_OK;
 }
 
-static int ensure_stage(b2s_plan_t p, int64_t n_rows) {
-  if (n_rows <= p->stage_rows) return B2S_OK;
-  // free first, and forget the old buffers before anything can fail: a failed allocation below must leave the plan
-  // with no staging area (stage_rows = 0) rather than with dangling pointers a later call would copy into / free twice
-  if (p->h_stage_in) cudaFreeHost(p->h_stage_in);
-  if (p->h_stage_out) cudaFreeHost(p->h_stage_out);
-  if (p->d_stage_in) cudaFree(p->d_stage_in);
-  if (p->d_stage_out) cudaFree(p->d_stage_out);
-  if (p->d_stage_status) cudaFree(p->d_stage_status);
-  p->h_stage_in = nullptr;
-  p->h_stage_out = nullptr;
-  p->d_stage_in = nullptr;
-  p->d_stage_out = nullptr;
-  p->d_stage_status = nullptr;
-  p->stage_rows = 0;
-  const int64_t cap = std::max<int64_t>(n_rows, 4096);
-  B2S_CUDA_TRY(cudaMallocHost(&p->h_stage_in, (size_t)cap * p->n_in * 4));
-  B2S_CUDA_TRY(cudaMallocHost(&p->h_stage_out, (size_t)cap * (p->out_cols + 1) * 4));
-  B2S_CUDA_TRY(cudaMalloc(&p->d_stage_in, (size_t)cap * p->n_in * 4));
-  B2S_CUDA_TRY(cudaMalloc(&p->d_stage_out, (size_t)cap * p->out_cols * 4));
-  B2S_CUDA_TRY(cudaMalloc(&p->d_stage_status, (size_t)cap * 4));
-  p->stage_rows = cap;
-  return B2S_OK;
+// Host batches: up to kZeroCopyInBytes of rows are read by the kernels straight from pinned host memory (no H2D copy: the
+// latency path of a small serving batch); larger batches cross PCIe on the copy engine first, which is where the bandwidth
+// is.  A pinned b2s_run_host batch of at least two chunks of kHostChunkRows runs as a pipeline of chunks.
+constexpr int64_t kZeroCopyInBytes = 64 << 10;
+constexpr int64_t kHostChunkRows = 65536;
+
+// With merge targets or an attached communicator the kernels store their votes there, not into the batch's results: a host
+// batch of such a plan would hand out rows no kernel wrote.
+static int refuse_merging(const b2s_plan_s* p) {
+  if (p->peers.empty() && !p->comm) return B2S_OK;
+  return fail(B2S_ERR_UNSUPPORTED, "the plan stores its votes to merge targets or a communicator: run it with b2s_run_device");
 }
 
 static void pack_rows(char* dst, const void* rows, int64_t n_rows, int64_t stride, int64_t row_bytes) {
@@ -1877,6 +1900,41 @@ static void pack_rows(char* dst, const void* rows, int64_t n_rows, int64_t strid
   }
 }
 
+// One host batch of n rows in pinned memory (`rows` as the host addresses them, `mapped` as the device does) on stream st.
+// The kernels write votes and status words straight into s.h_out (posted PCIe writes of a few bytes per row: no D2H copy).
+// Returns once the stream is idle, failures included; fills rows, h2d_ms, kernel_ms and kernels of `stats`.
+static int run_batch(b2s_plan_s* p, Stage& s, const void* rows, const void* mapped, int64_t n, cudaStream_t st,
+                     b2s_stats& stats) {
+  const int64_t row_bytes = (int64_t)p->n_in * 4;
+  const bool zero_copy = n * row_bytes <= kZeroCopyInBytes;
+  {
+    SyncOnExit sync{st};
+    B2S_CUDA_TRY(cudaEventRecord(s.ev[0], st));
+    if (!zero_copy) B2S_CUDA_TRY(cudaMemcpyAsync(s.d_in.get(), rows, (size_t)n * row_bytes, cudaMemcpyHostToDevice, st));
+    B2S_CUDA_TRY(cudaEventRecord(s.ev[1], st));
+    if (int rc = launch_on(p, zero_copy ? mapped : s.d_in.get(), n, row_bytes, s.h_out.get(), s.status(), st, zero_copy)) return rc;
+    B2S_CUDA_TRY(cudaEventRecord(s.ev[2], st));
+  }
+  stats = b2s_stats{};
+  stats.rows = n;
+  B2S_CUDA_TRY(cudaEventElapsedTime(&stats.h2d_ms, s.ev[0], s.ev[1]));  // also reports a fault of the batch's work
+  cudaEventElapsedTime(&stats.kernel_ms, s.ev[1], s.ev[2]);              // includes the PCIe writes of the results
+  stats.kernels = p->kernels_per_batch;
+  return B2S_OK;
+}
+
+// Rows [r0, r0 + n) of a finished batch to the caller: `out` and `row_status` (may be NULL) point at where row r0 goes.
+// Returns how many of the rows are flagged B2S_ROW_NONFINITE_INPUT.
+static int hand_out(const Stage& s, int64_t r0, int64_t n, void* out, int32_t* row_status) {
+  const size_t out_row = (size_t)s.out_cols * 4;
+  memcpy(out, s.h_out.get() + r0 * out_row, (size_t)n * out_row);
+  const int32_t* hs = s.status() + r0;
+  if (row_status) memcpy(row_status, hs, (size_t)n * 4);
+  int bad = 0;
+  for (int64_t r = 0; r < n; ++r) bad += (hs[r] & B2S_ROW_NONFINITE_INPUT) ? 1 : 0;
+  return bad;
+}
+
 extern "C" int b2s_run_host(b2s_plan_t p, const void* rows, int64_t n_rows, int64_t row_stride_bytes, void* out,
                             int64_t out_bytes, int32_t* row_status, b2s_stats* stats) {
   try {  // no C++ exception crosses the C boundary
@@ -1884,136 +1942,74 @@ extern "C" int b2s_run_host(b2s_plan_t p, const void* rows, int64_t n_rows, int6
     const int64_t row_bytes = (int64_t)p->n_in * 4;
     if (n_rows < 0 || row_stride_bytes < row_bytes) return fail(B2S_ERR_INVALID, "bad n_rows/stride");
     if (out_bytes < n_rows * p->out_cols * 4) return fail(B2S_ERR_INVALID, "out buffer too small");
+    if (int rc = refuse_merging(p)) return rc;
     if (n_rows == 0) return B2S_OK;
     std::lock_guard<std::mutex> lk(p->host_mu);
     B2S_CUDA_TRY(cudaSetDevice(G.device));
-    if (int rc = ensure_stage(p, n_rows)) return rc;
-    cudaStream_t st = G.stream;
+    Stage& s = p->host_stage;
+    if (int rc = s.reserve(std::max<int64_t>(n_rows, 4096), row_bytes, p->out_cols)) return rc;
     cudaPointerAttributes attr{};
     const bool pinned = cudaPointerGetAttributes(&attr, rows) == cudaSuccess && attr.type == cudaMemoryTypeHost &&
                         row_stride_bytes == row_bytes;
     cudaGetLastError();
     const void* src = rows;
+    const void* mapped = attr.devicePointer;
     if (!pinned) {
-      pack_rows(p->h_stage_in, rows, n_rows, row_stride_bytes, row_bytes);
-      src = p->h_stage_in;
+      pack_rows(s.h_in.get(), rows, n_rows, row_stride_bytes, row_bytes);
+      src = mapped = s.h_in.get();
     }
-    const size_t out_sz = (size_t)n_rows * p->out_cols * 4;
-    // Large pinned batches run as a pipeline of chunks: chunk c+1 crosses PCIe while chunk c is computed, copied back and
-    // post-processed on the host, so the call costs about one H2D of the batch.  (Not with merge targets: their row offset
-    // is per launch.)
-    static const int64_t pipe_rows = getenv("B2S_HOST_CHUNK") ? atoll(getenv("B2S_HOST_CHUNK")) : 65536;
-    if (pinned && pipe_rows > 0 && n_rows >= 2 * pipe_rows && p->peers.empty()) {
-      // whole tiles per chunk keep every chunk's base 16-byte (and tensor-map) aligned
-      const int64_t chunk = (int64_t)align_up((size_t)std::max<int64_t>(pipe_rows, (n_rows + 63) / 64), 1024);
+    b2s_stats batch{};
+    int bad = 0;
+    if (!pinned || n_rows < 2 * kHostChunkRows) {
+      if (int rc = run_batch(p, s, src, mapped, n_rows, G.stream, batch)) return rc;
+      bad = hand_out(s, 0, n_rows, out, row_status);
+    } else {
+      // chunk c+1 crosses PCIe on the copy stream while chunk c is computed, copied back and handed to the caller, so the
+      // call costs about one H2D of the batch; whole tiles per chunk keep every chunk's base 16-byte (and tensor-map) aligned
+      cudaStream_t st = G.stream, cs = G.copy_stream;
+      SyncOnExit sync_kernels{st}, sync_copies{cs};
+      const int64_t chunk = (int64_t)align_up((size_t)std::max<int64_t>(kHostChunkRows, (n_rows + 63) / 64), 1024);
       const int n_chunks = (int)((n_rows + chunk - 1) / chunk);
-      while ((int)p->chunk_ev.size() < 4 * n_chunks) {
-        cudaEvent_t e;
-        B2S_CUDA_TRY(cudaEventCreate(&e));
-        p->chunk_ev.push_back(e);
+      if ((int)p->chunk_ev.size() < 4 * n_chunks) {
+        if (int rc = p->chunk_ev.create(4 * n_chunks - (int)p->chunk_ev.size())) return rc;
       }
-      cudaStream_t cs = G.copy_stream;
-      int32_t* h_status = (int32_t*)(p->h_stage_out + out_sz);
       const size_t out_row = (size_t)p->out_cols * 4;
-      B2S_CUDA_TRY(cudaEventRecord(p->ev[0], cs));
+      B2S_CUDA_TRY(cudaEventRecord(s.ev[0], cs));
       for (int c = 0; c < n_chunks; ++c) {
         const int64_t r0 = (int64_t)c * chunk, nr = std::min<int64_t>(chunk, n_rows - r0);
-        cudaEvent_t* ce = &p->chunk_ev[4 * c];
-        B2S_CUDA_TRY(cudaMemcpyAsync(p->d_stage_in + r0 * row_bytes, (const char*)src + r0 * row_bytes, (size_t)nr * row_bytes,
-                                 cudaMemcpyHostToDevice, cs));
+        const cudaEvent_t* ce = p->chunk_ev.data() + 4 * c;
+        B2S_CUDA_TRY(cudaMemcpyAsync(s.d_in.get() + r0 * row_bytes, (const char*)src + r0 * row_bytes, (size_t)nr * row_bytes,
+                                     cudaMemcpyHostToDevice, cs));
         B2S_CUDA_TRY(cudaEventRecord(ce[0], cs));
         B2S_CUDA_TRY(cudaStreamWaitEvent(st, ce[0], 0));
         B2S_CUDA_TRY(cudaEventRecord(ce[1], st));
-        if (int rc = launch_on(p, p->d_stage_in + r0 * row_bytes, nr, row_bytes, p->d_stage_out + r0 * out_row,
-                               p->d_stage_status + r0, st)) {
-          cudaStreamSynchronize(cs);
-          cudaStreamSynchronize(st);
+        if (int rc = launch_on(p, s.d_in.get() + r0 * row_bytes, nr, row_bytes, s.d_out.get() + r0 * out_row,
+                               s.d_status.get() + r0, st))
           return rc;
-        }
         B2S_CUDA_TRY(cudaEventRecord(ce[2], st));
-        B2S_CUDA_TRY(cudaMemcpyAsync(p->h_stage_out + r0 * out_row, p->d_stage_out + r0 * out_row, (size_t)nr * out_row,
-                                 cudaMemcpyDeviceToHost, st));
-        B2S_CUDA_TRY(cudaMemcpyAsync(h_status + r0, p->d_stage_status + r0, (size_t)nr * 4, cudaMemcpyDeviceToHost, st));
+        B2S_CUDA_TRY(cudaMemcpyAsync(s.h_out.get() + r0 * out_row, s.d_out.get() + r0 * out_row, (size_t)nr * out_row,
+                                     cudaMemcpyDeviceToHost, st));
+        B2S_CUDA_TRY(cudaMemcpyAsync(s.status() + r0, s.d_status.get() + r0, (size_t)nr * 4, cudaMemcpyDeviceToHost, st));
         B2S_CUDA_TRY(cudaEventRecord(ce[3], st));
       }
-      int bad = 0;
       for (int c = 0; c < n_chunks; ++c) {  // hand each chunk to the caller as it lands
         const int64_t r0 = (int64_t)c * chunk, nr = std::min<int64_t>(chunk, n_rows - r0);
         B2S_CUDA_TRY(cudaEventSynchronize(p->chunk_ev[4 * c + 3]));
-        memcpy((char*)out + r0 * out_row, p->h_stage_out + r0 * out_row, (size_t)nr * out_row);
-        for (int64_t r = r0; r < r0 + nr; ++r) bad += (h_status[r] & B2S_ROW_NONFINITE_INPUT) ? 1 : 0;
-        if (row_status) memcpy(row_status + r0, h_status + r0, (size_t)nr * 4);
+        bad += hand_out(s, r0, nr, (char*)out + r0 * out_row, row_status ? row_status + r0 : nullptr);
       }
-      B2S_CUDA_TRY(cudaStreamSynchronize(cs));
-      if (stats) {
-        memset(stats, 0, sizeof(*stats));
-        stats->rows = n_rows;
-        cudaEventElapsedTime(&stats->h2d_ms, p->ev[0], p->chunk_ev[4 * (n_chunks - 1)]);
-        for (int c = 0; c < n_chunks; ++c) {  // the phases of different chunks overlap: these are sums over chunks
-          float k = 0.f, d = 0.f;
-          cudaEventElapsedTime(&k, p->chunk_ev[4 * c + 1], p->chunk_ev[4 * c + 2]);
-          cudaEventElapsedTime(&d, p->chunk_ev[4 * c + 2], p->chunk_ev[4 * c + 3]);
-          stats->kernel_ms += k;
-          stats->d2h_ms += d;
-        }
-        stats->kernels = p->kernels_per_batch * n_chunks;
-        stats->nonfinite_rows = bad;
+      batch.rows = n_rows;
+      cudaEventElapsedTime(&batch.h2d_ms, s.ev[0], p->chunk_ev[4 * (n_chunks - 1)]);
+      for (int c = 0; c < n_chunks; ++c) {  // the phases of different chunks overlap: these are sums over chunks
+        float k = 0.f, d = 0.f;
+        cudaEventElapsedTime(&k, p->chunk_ev[4 * c + 1], p->chunk_ev[4 * c + 2]);
+        cudaEventElapsedTime(&d, p->chunk_ev[4 * c + 2], p->chunk_ev[4 * c + 3]);
+        batch.kernel_ms += k;
+        batch.d2h_ms += d;
       }
-      return B2S_OK;
+      batch.kernels = p->kernels_per_batch * n_chunks;
     }
-    // Not pipelined: the kernels write votes and status words straight into pinned host memory (posted PCIe writes of a few
-    // bytes per row: no D2H copy, one synchronisation).  A tiny batch is also READ from pinned host memory by the kernels
-    // (no H2D copy: the latency path of a small serving batch); larger ones cross PCIe on the copy engine first, which is
-    // where the bandwidth is.  Not with merge targets: those kernels write to the targets.
-    static const int64_t zc_in_bytes = getenv("B2S_ZEROCOPY_IN_BYTES") ? atoll(getenv("B2S_ZEROCOPY_IN_BYTES")) : 65536;
-    static const int zc_out = getenv("B2S_ZEROCOPY_OUT") ? atoi(getenv("B2S_ZEROCOPY_OUT")) : 1;
-    const bool merging = !p->peers.empty() || p->comm;
-    if (zc_out && !merging) {
-      const bool zc_in = n_rows * row_bytes <= zc_in_bytes;
-      const void* d_src = p->d_stage_in;
-      if (stats) B2S_CUDA_TRY(cudaEventRecord(p->ev[0], st));
-      if (zc_in) d_src = pinned ? attr.devicePointer : (const void*)p->h_stage_in;
-      else B2S_CUDA_TRY(cudaMemcpyAsync(p->d_stage_in, src, (size_t)n_rows * row_bytes, cudaMemcpyHostToDevice, st));
-      if (stats) B2S_CUDA_TRY(cudaEventRecord(p->ev[1], st));
-      if (int rc = launch_on(p, d_src, n_rows, row_bytes, p->h_stage_out, (int32_t*)(p->h_stage_out + out_sz), st, zc_in)) return rc;
-      if (stats) B2S_CUDA_TRY(cudaEventRecord(p->ev[2], st));
-      B2S_CUDA_TRY(cudaStreamSynchronize(st));
-      memcpy(out, p->h_stage_out, out_sz);
-      const int32_t* hs = (const int32_t*)(p->h_stage_out + out_sz);
-      int bad = 0;
-      for (int64_t r = 0; r < n_rows; ++r) bad += (hs[r] & B2S_ROW_NONFINITE_INPUT) ? 1 : 0;
-      if (row_status) memcpy(row_status, hs, (size_t)n_rows * 4);
-      if (stats) {
-        memset(stats, 0, sizeof(*stats));
-        stats->rows = n_rows;
-        cudaEventElapsedTime(&stats->h2d_ms, p->ev[0], p->ev[1]);
-        cudaEventElapsedTime(&stats->kernel_ms, p->ev[1], p->ev[2]);  // includes the PCIe writes of the results
-        stats->kernels = p->kernels_per_batch;
-        stats->nonfinite_rows = bad;
-      }
-      return B2S_OK;
-    }
-    B2S_CUDA_TRY(cudaEventRecord(p->ev[0], st));
-    B2S_CUDA_TRY(cudaMemcpyAsync(p->d_stage_in, src, (size_t)n_rows * row_bytes, cudaMemcpyHostToDevice, st));
-    B2S_CUDA_TRY(cudaEventRecord(p->ev[1], st));
-    if (int rc = launch_on(p, p->d_stage_in, n_rows, row_bytes, p->d_stage_out, p->d_stage_status, st)) return rc;
-    B2S_CUDA_TRY(cudaEventRecord(p->ev[2], st));
-    B2S_CUDA_TRY(cudaMemcpyAsync(p->h_stage_out, p->d_stage_out, out_sz, cudaMemcpyDeviceToHost, st));
-    B2S_CUDA_TRY(cudaMemcpyAsync(p->h_stage_out + out_sz, p->d_stage_status, (size_t)n_rows * 4, cudaMemcpyDeviceToHost, st));
-    B2S_CUDA_TRY(cudaEventRecord(p->ev[3], st));
-    B2S_CUDA_TRY(cudaStreamSynchronize(st));
-    memcpy(out, p->h_stage_out, out_sz);
-    const int32_t* hs = (const int32_t*)(p->h_stage_out + out_sz);
-    int bad = 0;
-    for (int64_t r = 0; r < n_rows; ++r) bad += (hs[r] & B2S_ROW_NONFINITE_INPUT) ? 1 : 0;
-    if (row_status) memcpy(row_status, hs, (size_t)n_rows * 4);
     if (stats) {
-      memset(stats, 0, sizeof(*stats));
-      stats->rows = n_rows;
-      cudaEventElapsedTime(&stats->h2d_ms, p->ev[0], p->ev[1]);
-      cudaEventElapsedTime(&stats->kernel_ms, p->ev[1], p->ev[2]);
-      cudaEventElapsedTime(&stats->d2h_ms, p->ev[2], p->ev[3]);
-      stats->kernels = p->kernels_per_batch;
+      *stats = batch;
       stats->nonfinite_rows = bad;
     }
     return B2S_OK;
@@ -2042,7 +2038,7 @@ extern "C" int b2s_time_device(b2s_plan_t p, const void* const* d_rows, int32_t 
 }
 
 // ------------------------------------------------------------------------------------------ coalescing ring
-// One coalesced batch on the ring's stream: pinned slot -> (H2D) -> kernels -> (D2H) -> pinned slot, then the host waits for it.
+// One coalesced batch on the ring's stream: run_batch from the slot's stage, then the host waits for it.
 // Runs WITHOUT the plan's lock, either on the dispatcher thread or on a caller blocked in b2s_wait (see there); `dispatch_busy`
 // keeps it to one batch at a time.
 struct BatchResult {
@@ -2055,56 +2051,18 @@ constexpr int kRingGraceUs = 50;
 
 static BatchResult ring_run_batch(b2s_plan_s* p, Slot& s) {
   BatchResult res;
-  const int64_t rows = s.rows;
   const float queue_us =
       std::chrono::duration<float, std::micro>(std::chrono::steady_clock::now() - s.first_submit).count();
-  cudaStream_t st = p->ring_stream;
-  const int64_t row_bytes = (int64_t)p->n_in * 4;
-  const size_t out_sz = (size_t)rows * p->out_cols * 4;
-  // every step is checked: a batch whose copy or launch failed is reported to all of its tickets (b2s_wait returns
-  // the error and copies nothing) instead of handing out whatever an earlier batch left in the pinned slot
-  int& err = res.err;
-  std::string& err_msg = res.err_msg;
-  auto step = [&](cudaError_t e, const char* what) {
-    if (e != cudaSuccess && !err) {
-      err = B2S_ERR_CUDA;
-      err_msg = std::string("coalesced batch: ") + what + ": " + cudaGetErrorString(e);
-    }
-  };
-  static const int64_t zc_in_bytes = getenv("B2S_ZEROCOPY_IN_BYTES") ? atoll(getenv("B2S_ZEROCOPY_IN_BYTES")) : 65536;
-  static const int zc_out = getenv("B2S_ZEROCOPY_OUT") ? atoi(getenv("B2S_ZEROCOPY_OUT")) : 1;
-  const bool zero_out = zc_out && p->peers.empty() && !p->comm;  // results go straight into the slot's pinned result area
-  const bool zero_in = zero_out && rows * row_bytes <= zc_in_bytes;  // a tiny batch is read from the pinned slot as well
-  step(cudaEventRecord(s.e0, st), "event record");
-  if (!zero_in) step(cudaMemcpyAsync(s.d_in, s.h_in, (size_t)rows * row_bytes, cudaMemcpyHostToDevice, st), "H2D copy");
-  step(cudaEventRecord(s.e1, st), "event record");
-  if (!err) {
-    int32_t* h_status = (int32_t*)(s.h_out + (size_t)p->ring_cap * p->out_cols * 4);
-    const int rc = zero_out ? launch_on(p, zero_in ? s.h_in : s.d_in, rows, row_bytes, s.h_out, h_status, st, zero_in)
-                            : launch_on(p, s.d_in, rows, row_bytes, s.d_out, s.d_status, st);
-    if (rc) {
-      err = rc;
-      err_msg = std::string("coalesced batch: ") + g_err;
-    }
-  }
-  step(cudaEventRecord(s.e2, st), "event record");
-  if (!err && !zero_out) {
-    step(cudaMemcpyAsync(s.h_out, s.d_out, out_sz, cudaMemcpyDeviceToHost, st), "D2H copy");
-    step(cudaMemcpyAsync(s.h_out + (size_t)p->ring_cap * p->out_cols * 4, s.d_status, (size_t)rows * 4, cudaMemcpyDeviceToHost, st), "D2H copy");
-  }
-  step(cudaEventRecord(s.e3, st), "event record");
-  step(cudaEventSynchronize(s.e3), "execution");
-  b2s_stats& stt = res.stats;
-  stt.rows = rows;
-  if (!err) {
-    cudaEventElapsedTime(&stt.h2d_ms, s.e0, s.e1);
-    cudaEventElapsedTime(&stt.kernel_ms, s.e1, s.e2);
-    cudaEventElapsedTime(&stt.d2h_ms, s.e2, s.e3);
-  } else {
+  // a batch that fails is reported to all of its tickets (b2s_wait returns the error and copies nothing) instead of
+  // handing out whatever an earlier batch left in the pinned slot
+  int rc = refuse_merging(p);
+  if (!rc) rc = run_batch(p, s.stage, s.stage.h_in.get(), s.stage.h_in.get(), s.rows, p->ring_stream.get(), res.stats);
+  if (rc) {
+    res.err = rc;
+    res.err_msg = std::string("coalesced batch: ") + g_err;
     cudaGetLastError();  // the error is reported through the tickets
   }
-  stt.queue_us = queue_us;
-  stt.kernels = p->kernels_per_batch;
+  res.stats.queue_us = queue_us;
   return res;
 }
 
@@ -2175,17 +2133,6 @@ static void dispatcher_main(b2s_plan_s* p) {
   }
 }
 
-static void ring_free_slot(Slot& s) {
-  if (s.h_in) cudaFreeHost(s.h_in);
-  if (s.h_out) cudaFreeHost(s.h_out);
-  if (s.d_in) cudaFree(s.d_in);
-  if (s.d_out) cudaFree(s.d_out);
-  if (s.d_status) cudaFree(s.d_status);
-  for (cudaEvent_t e : {s.e0, s.e1, s.e2, s.e3})
-    if (e) cudaEventDestroy(e);
-  s = Slot{};
-}
-
 static int ring_start(b2s_plan_s* p) {
   if (!p->slots.empty()) return B2S_OK;
   B2S_CUDA_TRY(cudaSetDevice(G.device));
@@ -2194,35 +2141,24 @@ static int ring_start(b2s_plan_s* p) {
   const int64_t cap = p->ring_cfg_max_batch > 0 ? p->ring_cfg_max_batch : G.max_batch;
   const int n_slots = p->ring_cfg_slots > 0 ? p->ring_cfg_slots : G.ring_slots;
   std::vector<Slot> slots(n_slots);
-  cudaStream_t stream = nullptr;
-  const int64_t row_bytes = (int64_t)p->n_in * 4;
-  cudaError_t e = cudaSuccess;
-  auto ok = [&](cudaError_t r) { return e == cudaSuccess && (e = r) == cudaSuccess; };
   for (auto& s : slots) {
     s.done_cv = std::make_shared<std::condition_variable>();
-    if (!(ok(cudaMallocHost(&s.h_in, (size_t)cap * row_bytes)) && ok(cudaMallocHost(&s.h_out, (size_t)cap * (p->out_cols + 1) * 4)) &&
-          ok(cudaMalloc(&s.d_in, (size_t)cap * row_bytes)) && ok(cudaMalloc(&s.d_out, (size_t)cap * p->out_cols * 4)) &&
-          ok(cudaMalloc(&s.d_status, (size_t)cap * 4)) && ok(cudaEventCreate(&s.e0)) && ok(cudaEventCreate(&s.e1)) &&
-          ok(cudaEventCreate(&s.e2)) && ok(cudaEventCreate(&s.e3))))
-      break;
+    if (s.stage.reserve(cap, (int64_t)p->n_in * 4, p->out_cols)) {
+      cudaGetLastError();
+      return fail(B2S_ERR_CUDA, "coalescing ring of %d x %lld rows: %s", n_slots, (long long)cap, g_err.c_str());
+    }
   }
-  if (e == cudaSuccess) ok(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-  if (e != cudaSuccess) {
-    for (auto& s : slots) ring_free_slot(s);
-    cudaGetLastError();
-    return fail(B2S_ERR_CUDA, "coalescing ring of %d x %lld rows: %s", n_slots, (long long)cap, cudaGetErrorString(e));
-  }
+  cudaStream_t stream = nullptr;
+  B2S_CUDA_TRY(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
   p->ring_cap = cap;
   p->slots = std::move(slots);
-  p->ring_stream = stream;
+  p->ring_stream.reset(stream);
   p->stop = false;
   try {
     p->dispatcher = std::thread(dispatcher_main, p);
   } catch (const std::exception& ex) {
-    for (auto& s : p->slots) ring_free_slot(s);
     p->slots.clear();
-    cudaStreamDestroy(p->ring_stream);
-    p->ring_stream = nullptr;
+    p->ring_stream.reset();
     return fail(B2S_ERR_STATE, "coalescing ring: cannot start the dispatcher thread: %s", ex.what());
   }
   return B2S_OK;
@@ -2262,7 +2198,7 @@ extern "C" int b2s_submit(b2s_plan_t p, const void* rows, int64_t n_rows, int64_
     Slot& s = p->slots[p->open_slot];
     if (s.rows == 0) s.first_submit = std::chrono::steady_clock::now();
     const int64_t off = s.rows;
-    pack_rows(s.h_in + off * row_bytes, rows, n_rows, row_stride_bytes, row_bytes);
+    pack_rows(s.stage.h_in.get() + off * row_bytes, rows, n_rows, row_stride_bytes, row_bytes);
     s.rows += n_rows;
     s.waiters += 1;
     *ticket = (s.batch_id << 24) | (uint64_t)off;
@@ -2383,13 +2319,9 @@ extern "C" int b2s_wait(b2s_plan_t p, uint64_t ticket, void* out, int64_t out_by
       // tickets of a batch are collected side by side
       const b2s_stats batch_stats = s.stats;
       lk.unlock();
-      memcpy(out, s.h_out + (size_t)off * p->out_cols * 4, (size_t)n_rows * p->out_cols * 4);
-      const int32_t* hs = (const int32_t*)(s.h_out + (size_t)p->ring_cap * p->out_cols * 4) + off;
-      if (row_status) memcpy(row_status, hs, (size_t)n_rows * 4);
+      const int bad = hand_out(s.stage, off, n_rows, out, row_status);
       if (stats) {
         *stats = batch_stats;
-        int bad = 0;
-        for (int64_t r = 0; r < n_rows; ++r) bad += (hs[r] & B2S_ROW_NONFINITE_INPUT) ? 1 : 0;
         stats->nonfinite_rows = bad;
       }
       lk.lock();
@@ -2479,20 +2411,6 @@ extern "C" int b2s_plan_destroy(b2s_plan_t p) {
       }
       p->dispatcher.join();
     }
-    for (auto& s : p->slots) ring_free_slot(s);
-    if (p->ring_stream) cudaStreamDestroy(p->ring_stream);
-    if (p->h_stage_in) cudaFreeHost(p->h_stage_in);
-    if (p->h_stage_out) cudaFreeHost(p->h_stage_out);
-    if (p->d_stage_in) cudaFree(p->d_stage_in);
-    if (p->d_stage_out) cudaFree(p->d_stage_out);
-    if (p->d_stage_status) cudaFree(p->d_stage_status);
-    for (int i = 0; i < 4; ++i)
-      if (p->ev[i]) cudaEventDestroy(p->ev[i]);
-    for (cudaEvent_t e : p->chunk_ev) cudaEventDestroy(e);
-    if (p->d_blob) cudaFree(p->d_blob);
-    if (p->d_t3_blob) cudaFree(p->d_t3_blob);
-    for (auto& kv : p->tree_scratch)
-      if (kv.second.partial) { cudaFree(kv.second.partial); cudaFree(kv.second.row_bad); if (kv.second.xt) cudaFree(kv.second.xt); }
     delete p;
     return B2S_OK;
   } catch (const std::exception& e) {
@@ -2574,10 +2492,10 @@ extern "C" int b2s_comm_create(int32_t rank, int32_t world, int64_t max_rows_per
     c->max_rows = (max_rows_per_rank + 3) / 4 * 4;  // row blocks start 16-byte aligned
     c->bytes = kCommHeader + kCommSlots * c->buf_bytes();
     B2S_CUDA_TRY(cudaSetDevice(G.device));
-    B2S_CUDA_TRY(cudaMalloc(&c->base, c->bytes));
-    B2S_CUDA_TRY(cudaMemset(c->base, 0, 512 < c->bytes ? 512 : c->bytes));
+    if (int rc = allocate(c->base, c->bytes)) return rc;
+    B2S_CUDA_TRY(cudaMemset(c->base.get(), 0, 512 < c->bytes ? 512 : c->bytes));
     c->peer_base.assign(world, nullptr);
-    c->peer_base[rank] = c->base;
+    c->peer_base[rank] = c->base.get();
     if (world == 1) c->connected = true;
     *out = c.release();
     return B2S_OK;
@@ -2589,7 +2507,7 @@ extern "C" int b2s_comm_create(int32_t rank, int32_t world, int64_t max_rows_per
 extern "C" int b2s_comm_handle(b2s_comm_t c, void* handle64) {
   try {
     if (!c || !handle64) return fail(B2S_ERR_INVALID, "null communicator");
-    B2S_CUDA_TRY(cudaIpcGetMemHandle(reinterpret_cast<cudaIpcMemHandle_t*>(handle64), c->base));
+    B2S_CUDA_TRY(cudaIpcGetMemHandle(reinterpret_cast<cudaIpcMemHandle_t*>(handle64), c->base.get()));
     return B2S_OK;
   } catch (const std::exception& e) {
     return fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
@@ -2668,11 +2586,10 @@ static int comm_wait_epoch(b2s_comm_t c, void* stream, uint32_t e, const void** 
       if (epoch_out) *epoch_out = e;
       return B2S_OK;
     }
-    uint32_t* timeout_flag = reinterpret_cast<uint32_t*>(c->base) + 65;
     // how long a rank may lag behind before the step is declared dead (B2S_COMM_TIMEOUT_MS, default 10 s)
     static const long long timeout_ns = (getenv("B2S_COMM_TIMEOUT_MS") ? atoll(getenv("B2S_COMM_TIMEOUT_MS")) : 10000ll) * 1000000ll;
     // a one-warp polling kernel; the cheap form is the fused wait (b2s_comm_set_fused_wait), which launches nothing
-    merge_wait_kernel<<<1, 32, 0, st>>>(c->flags(c->rank), c->world, e, timeout_flag, timeout_ns);
+    merge_wait_kernel<<<1, 32, 0, st>>>(c->flags(c->rank), c->world, e, c->timeout_flag(), timeout_ns);
     cudaError_t err = cudaGetLastError();
     if (err != cudaSuccess) return fail(B2S_ERR_CUDA, "merge wait launch failed: %s", cudaGetErrorString(err));
     G.launches.fetch_add(1, std::memory_order_relaxed);
@@ -2700,7 +2617,7 @@ extern "C" int b2s_comm_check(b2s_comm_t c) {
   try {  // after a stream synchronisation: did a wait give up on a peer?
     if (!c) return fail(B2S_ERR_INVALID, "null communicator");
     uint32_t v = 0;
-    B2S_CUDA_TRY(cudaMemcpy(&v, reinterpret_cast<uint32_t*>(c->base) + 65, 4, cudaMemcpyDeviceToHost));
+    B2S_CUDA_TRY(cudaMemcpy(&v, c->timeout_flag(), 4, cudaMemcpyDeviceToHost));
     if (v) return fail(B2S_ERR_TIMEOUT, "ensemble-merge: rank %u did not signal its shard in time (B2S_COMM_TIMEOUT_MS)", v - 1);
     return B2S_OK;
   } catch (const std::exception& e) {
@@ -2713,7 +2630,6 @@ extern "C" int b2s_comm_destroy(b2s_comm_t c) {
     if (!c) return B2S_OK;
     for (int r = 0; r < c->world; ++r)
       if (r != c->rank && c->peer_base[r]) cudaIpcCloseMemHandle(c->peer_base[r]);
-    if (c->base) cudaFree(c->base);
     delete c;
     return B2S_OK;
   } catch (const std::exception& e) {

@@ -1,11 +1,13 @@
-// b2s_stage.h -- host-side staging that the point-in-time join (b2s_pit.cu) and the windowed aggregations (b2s_agg.cu)
-// share: one device block per call for its inputs, outputs and scratch, CUDA events that destroy themselves, and the
-// call's launch count.  Host code only.  Its names live in the including unit's anonymous namespace, so none is exported.
+// b2s_stage.h -- host-side staging that the serving runtime (b2s_runtime.cu), the point-in-time join (b2s_pit.cu) and the
+// windowed aggregations (b2s_agg.cu) share: one device block per call for its inputs, outputs and scratch, device and
+// pinned arrays and CUDA events that free themselves, and the call's launch count.  Host code only.  Its names live in the
+// including unit's anonymous namespace, so none is exported.
 #pragma once
 #include <cuda_runtime.h>
 
 #include <cstddef>
 #include <cstdint>
+#include <memory>
 #include <vector>
 
 #include "../../include/b200serve.h"
@@ -48,10 +50,41 @@ class Events {
   }
   cudaEvent_t operator[](size_t i) const { return ev_[i]; }
   const cudaEvent_t* data() const { return ev_.data(); }
+  size_t size() const { return ev_.size(); }
 
  private:
   std::vector<cudaEvent_t> ev_;
 };
+
+// Device and pinned host arrays, freed when their owner goes.  allocate() frees the old array before it makes the new one:
+// a failed allocation leaves the owner empty, never dangling.
+struct CudaFree {
+  void operator()(void* p) const { cudaFree(p); }
+};
+struct CudaFreeHost {
+  void operator()(void* p) const { cudaFreeHost(p); }
+};
+template <class T>
+using DeviceArray = std::unique_ptr<T[], CudaFree>;
+template <class T>
+using PinnedArray = std::unique_ptr<T[], CudaFreeHost>;
+
+template <class T>
+int allocate(DeviceArray<T>& a, size_t bytes) {
+  a.reset();
+  void* p = nullptr;
+  B2S_CUDA_TRY(cudaMalloc(&p, bytes));
+  a.reset(static_cast<T*>(p));
+  return B2S_OK;
+}
+template <class T>
+int allocate(PinnedArray<T>& a, size_t bytes) {
+  a.reset();
+  void* p = nullptr;
+  B2S_CUDA_TRY(cudaMallocHost(&p, bytes));
+  a.reset(static_cast<T*>(p));
+  return B2S_OK;
+}
 
 // Every device array of one call in a single cudaMallocAsync, each region 256-byte aligned.  Regions are laid out first,
 // each with the pointer that is to address it; alloc() makes the block and sets those pointers.  An input is uploaded by
