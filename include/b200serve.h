@@ -222,9 +222,11 @@ int b2s_run_host(b2s_plan_t plan, const void* rows, int64_t n_rows, int64_t row_
  * thread seals a batch when it holds max_batch rows or the oldest row waited max_wait_us (0: as soon as the dispatcher is
  * free -- batches form while the previous one runs), and runs it on its own stream as one b2s_run_host batch that is
  * never pipelined (results straight to the slot's pinned memory, rows read from there up to 64 KiB).  b2s_wait blocks
- * until the ticket's batch completed and copies that ticket's rows out; a batch that failed, or of a plan with merge
- * targets or an attached communicator (B2S_ERR_UNSUPPORTED), gives every one of its tickets the error.  This is the
- * replacement of storey's SyncEmitSource.emit / await_result hand-off (serving/states.py:1283-1287).  A ring slot is recycled when every ticket of its batch was collected, and the ring
+ * until the ticket's batch completed and copies that ticket's rows out (out_bytes must hold them); a batch that failed,
+ * or of a plan with merge targets or an attached communicator (B2S_ERR_UNSUPPORTED), gives every one of its tickets the
+ * error.  A ticket is collected once: waiting on it again, or on a ticket that was never issued, is B2S_ERR_INVALID and
+ * leaves the other tickets of its batch alone.  This is the replacement of storey's SyncEmitSource.emit / await_result
+ * hand-off (serving/states.py:1283-1287).  A ring slot is recycled when every ticket of its batch was collected, and the ring
  * has `ring_slots` (b2s_init cfg, default 4) batches: a producer that keeps submitting without collecting its tickets
  * eventually blocks in b2s_submit -- emit and await per request, as the reference's callers do. */
 int b2s_submit(b2s_plan_t plan, const void* rows, int64_t n_rows, int64_t row_stride_bytes, uint64_t* ticket);

@@ -146,7 +146,9 @@ struct Slot {  // one in-flight batch of the coalescing ring
   int state = 0;  // 0 free/open, 1 sealed (queued for the dispatcher), 2 in flight, 3 done
   std::chrono::steady_clock::time_point first_submit;
   b2s_stats stats{};
-  int waiters = 0;      // tickets issued on this batch not yet collected
+  // offset -> rows of every ticket issued on this batch and not yet collected (-1 while its caller copies it out): a
+  // ticket is collected once, and the slot is recycled when the map is empty
+  std::map<int64_t, int64_t> tickets;
   std::shared_ptr<std::condition_variable> done_cv;  // the batch's own waiters (one wake-up per batch, not a herd over all tickets)
   bool wanted = false;  // a caller is blocked in b2s_wait on this (still open) batch: it leaves as soon as the dispatcher is free
   int err = 0;          // b2s_status of the batch (a failed copy / launch): every ticket of the batch gets it
@@ -233,6 +235,9 @@ struct b2s_plan_s {
     DeviceArray<int32_t> row_bad;  // per-row non-finite input flags (t3_prep_kernel -> t3_vote_kernel)
     DeviceArray<uint32_t> xt;      // the batch transposed into tiles (t3_prep_kernel -> trees3_kernel)
     int64_t rows = 0;
+    // held from reserve until the batch's prep, walk and vote are enqueued: two callers on one stream (b2s_run_host and
+    // b2s_run_device(NULL) both use the library stream) must not interleave their launches over one scratch
+    std::mutex mu;
     // room for n rows of `cols` partial-sum columns; cudaFree waits for the work that still reads the old arrays
     int reserve(int64_t n, int cols, int xt_words) {
       if (n <= rows) return B2S_OK;
@@ -271,6 +276,8 @@ struct b2s_plan_s {
   int ring_cfg_wait_us = -1;
   int wait_us() const { return ring_cfg_wait_us >= 0 ? ring_cfg_wait_us : G.max_wait_us; }
 };
+
+int b2s_int_plan_kernels(const b2s_plan_s* p) { return p->kernels_per_batch; }
 
 int b2s_int_plan_shape(b2s_plan_s* p, int* n_in, int* out_cols) {
   if (!p || !p->finalized) return fail(B2S_ERR_STATE, "plan not finalized");
@@ -1774,15 +1781,17 @@ static int launch_on(b2s_plan_t p, const void* d_rows, int64_t n_rows, int64_t s
     int32_t* row_bad;
     uint32_t* xt;
     int64_t col_stride;
+    b2s_plan_s::TreeScratch* mine;
     {
       std::lock_guard<std::mutex> lk(p->scratch_mu);
-      b2s_plan_s::TreeScratch& mine = p->tree_scratch[st];
-      if (int rc = mine.reserve(n_rows, C, p->t3.xt_words)) return rc;
-      partial = mine.partial.get();
-      row_bad = mine.row_bad.get();
-      xt = mine.xt.get();
-      col_stride = mine.rows;
+      mine = &p->tree_scratch[st];  // std::map nodes stay where they are
     }
+    std::lock_guard<std::mutex> own(mine->mu);  // this batch's scratch until its three launches are enqueued
+    if (int rc = mine->reserve(n_rows, C, p->t3.xt_words)) return rc;
+    partial = mine->partial.get();
+    row_bad = mine->row_bad.get();
+    xt = mine->xt.get();
+    col_stride = mine->rows;
     T3Prep pr = p->t3_prep;
     pr.rows = (const char*)d_rows;
     pr.row_stride = stride;
@@ -2099,7 +2108,7 @@ static void dispatcher_main(b2s_plan_s* p) {
         // that submits many tickets before it collects any fills a batch instead of exhausting the ring.
         int spare = p->slots[p->open_slot].wanted ? 1 : 0;  // a caller blocked on this batch: holding it back gains nothing
         for (int i = 0; i < (int)p->slots.size(); ++i)
-          spare += (i != p->open_slot && p->slots[i].state == 0 && p->slots[i].rows == 0 && p->slots[i].waiters == 0) ? 1 : 0;
+          spare += (i != p->open_slot && p->slots[i].state == 0 && p->slots[i].rows == 0 && p->slots[i].tickets.empty()) ? 1 : 0;
         if (spare == 0) {
           p->cv_work.wait(lk);  // a slot is collected, the batch fills up, a waiter or a flush seals it
           continue;
@@ -2182,7 +2191,7 @@ extern "C" int b2s_submit(b2s_plan_t p, const void* rows, int64_t n_rows, int64_
       }
       if (p->open_slot < 0) {
         for (int i = 0; i < (int)p->slots.size(); ++i)
-          if (p->slots[i].state == 0 && p->slots[i].rows == 0 && p->slots[i].waiters == 0) {
+          if (p->slots[i].state == 0 && p->slots[i].rows == 0 && p->slots[i].tickets.empty()) {
             p->open_slot = i;
             p->slots[i].batch_id = p->next_batch++;
             p->batch_slot[p->slots[i].batch_id] = i;
@@ -2200,7 +2209,7 @@ extern "C" int b2s_submit(b2s_plan_t p, const void* rows, int64_t n_rows, int64_
     const int64_t off = s.rows;
     pack_rows(s.stage.h_in.get() + off * row_bytes, rows, n_rows, row_stride_bytes, row_bytes);
     s.rows += n_rows;
-    s.waiters += 1;
+    s.tickets[off] = n_rows;
     *ticket = (s.batch_id << 24) | (uint64_t)off;
     if (s.rows >= p->ring_cap) {
       s.state = 1;
@@ -2208,7 +2217,6 @@ extern "C" int b2s_submit(b2s_plan_t p, const void* rows, int64_t n_rows, int64_
       p->open_slot = -1;
     }
     p->cv_work.notify_one();
-    // remember how many rows this ticket covers (low 24 bits hold the offset; the count travels in a side map)
     return B2S_OK;
   } catch (const std::exception& e) {
     return fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
@@ -2252,11 +2260,17 @@ extern "C" int b2s_wait(b2s_plan_t p, uint64_t ticket, void* out, int64_t out_by
     if (!p || !p->finalized) return fail(B2S_ERR_STATE, "plan not finalized");
     const uint64_t batch = ticket >> 24;
     const int64_t off = (int64_t)(ticket & ((1u << 24) - 1));
-    const int64_t n_rows = out_bytes / ((int64_t)p->out_cols * 4);
     std::unique_lock<std::mutex> lk(p->mu);
     auto it = p->batch_slot.find(batch);
     if (it == p->batch_slot.end()) return fail(B2S_ERR_INVALID, "unknown ticket");
     Slot& s = p->slots[it->second];
+    // a ticket of a live batch that was never issued, or was already collected, must not touch the batch: a second
+    // collection would recycle the slot under tickets still outstanding
+    auto issued = [&] {
+      auto t = s.tickets.find(off);
+      return t != s.tickets.end() && t->second >= 0;
+    };
+    if (!issued()) return fail(B2S_ERR_INVALID, "unknown or already collected ticket");
     // Who runs the batch?  With max_wait_us = 0 the caller that blocks on it does, right here, as soon as the ring's stream is
     // free (no hand-off to another thread and back: that costs more than a small batch takes on the device, and under many
     // request threads the dispatcher thread would queue for a core behind them).  While a batch is in flight the rows of other
@@ -2308,15 +2322,19 @@ extern "C" int b2s_wait(b2s_plan_t p, uint64_t ticket, void* out, int64_t out_by
       }
       s.done_cv->wait(lk);  // woken when the batch is done, or to take the stream over
     }
-    // the batch is done: whatever this call returns, the ticket is spent and the last one recycles the slot
+    // the batch is done: whatever this call returns, the ticket is spent and the last one recycles the slot.  Another
+    // caller of the same ticket may have collected it meanwhile.
+    if (!issued()) return fail(B2S_ERR_INVALID, "unknown or already collected ticket");
+    auto tk = s.tickets.find(off);
+    const int64_t n_rows = tk->second;
+    tk->second = -1;  // being collected: the slot stays while this caller copies without the lock
     int rc = B2S_OK;
     if (s.err) {
       rc = fail(s.err, "%s", s.err_msg.c_str());
-    } else if (off + n_rows > s.rows) {
-      rc = fail(B2S_ERR_INVALID, "ticket range exceeds its batch");
+    } else if (out_bytes < n_rows * p->out_cols * 4) {
+      rc = fail(B2S_ERR_INVALID, "out buffer too small for the ticket's %lld rows", (long long)n_rows);
     } else {
-      // the slot cannot be recycled while this ticket is outstanding (waiters > 0): copy without the lock, so that the
-      // tickets of a batch are collected side by side
+      // copy without the lock, so that the tickets of a batch are collected side by side
       const b2s_stats batch_stats = s.stats;
       lk.unlock();
       const int bad = hand_out(s.stage, off, n_rows, out, row_status);
@@ -2326,7 +2344,8 @@ extern "C" int b2s_wait(b2s_plan_t p, uint64_t ticket, void* out, int64_t out_by
       }
       lk.lock();
     }
-    if (--s.waiters == 0) {  // last collector frees the slot
+    s.tickets.erase(tk);
+    if (s.tickets.empty()) {  // last collector frees the slot
       p->batch_slot.erase(it);
       s.rows = 0;
       s.state = 0;

@@ -375,8 +375,8 @@ extern "C" int b2s_table_enrich_host(b2s_table_t t, b2s_plan_t plan, const int64
     B2S_CUDA_TRY(cudaEventRecord(t->ev[1], st));
     int n_kernels = 1;
     int rc = launch_fused(t, plan, t->d_keys, n, t->d_votes, t->d_status, st);  // gather inside the scoring kernel
-    if (rc == B2S_ERR_UNSUPPORTED) {  // plans the gather loader does not cover: gather, score, fold the flags (3 launches)
-      n_kernels = 3;
+    if (rc == B2S_ERR_UNSUPPORTED) {  // plans the gather loader does not cover: gather, score, fold the flags
+      n_kernels = 2 + b2s_int_plan_kernels(plan);
       if ((rc = launch_lookup(t, t->d_keys, n, t->d_out, stride, t->d_found, st))) return rc;
       if ((rc = b2s_run_device(plan, t->d_out, n, stride, t->d_votes, t->d_status, st))) return rc;
       const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(4 * b2s_int_sm_count(), (n + 255) / 256));
@@ -400,7 +400,7 @@ extern "C" int b2s_table_enrich_host(b2s_table_t t, b2s_plan_t plan, const int64
       cudaEventElapsedTime(&stats->h2d_ms, t->ev[0], t->ev[1]);
       cudaEventElapsedTime(&stats->kernel_ms, t->ev[1], t->ev[2]);
       cudaEventElapsedTime(&stats->d2h_ms, t->ev[2], t->ev[3]);
-      stats->kernels = n_kernels;  // 1: gather fused into the scoring kernel; 3: gather + the plan + mark_unknown
+      stats->kernels = n_kernels;  // 1: gather fused into the scoring kernel; else gather + the plan's launches + mark_unknown
       if (row_status)
         for (int64_t r = 0; r < n; ++r) stats->nonfinite_rows += (row_status[r] & B2S_ROW_NONFINITE_INPUT) ? 1 : 0;
     }

@@ -165,9 +165,10 @@ def test_enrich_host_equals_lookup_then_plan_for_pinned_and_pageable_keys():
         table.enrich(other.compile().plan, np.array([1], dtype=np.int64))
 
 
-def test_enrich_device_one_launch_and_the_plans_it_does_not_cover():
+def test_enrich_device_one_launch_and_the_fallback_of_tree_plans():
     """b2s_table_enrich_device on device-resident keys: one launch, same bits as gather-then-score; a tree ensemble is
-    not covered by the gather loader (B2S_ERR_UNSUPPORTED -> enrich_host gathers first, three launches)"""
+    not covered by the gather loader (B2S_ERR_UNSUPPORTED -> enrich_host gathers first: the lookup, the three trees3
+    launches and mark_unknown, five launches in the stats and in the library's count)"""
     from sklearn.ensemble import GradientBoostingRegressor
 
     bvec, _ovec, keys, vals, feat = _vectors(n_keys=4000, n_feat=16, seed=12, key_kind="int")
@@ -192,7 +193,8 @@ def test_enrich_device_one_launch_and_the_plans_it_does_not_cover():
     np.testing.assert_array_equal(got.view(np.uint32), want.view(np.uint32))
     np.testing.assert_array_equal(st, want_st | np.where(found, 0, nat.ROW_UNKNOWN_KEY))
 
-    # a tree ensemble behind the same router: not fusable, same results through the three-launch path
+    # a tree ensemble behind the same router: not fusable, same results through the fallback (lookup, the three trees3
+    # launches, mark_unknown)
     api_b200.register_feature_vector("store://vec", bvec)
     fn = api_b200.new_function("enrich-trees", kind="serving")
     graph = fn.set_topology("router", api_b200.EnrichmentVotingEnsemble(feature_vector_uri="store://vec", impute_policy={"*": 0.0},
@@ -204,11 +206,13 @@ def test_enrich_device_one_launch_and_the_plans_it_does_not_cover():
         graph.add_route(f"t{i}", class_name="SKLearnModelServer", model=m, model_path="")
     tserver = fn.to_mock_server(namespace={"SKLearnModelServer": api_b200.SKLearnModelServer})
     tplan = tserver.compile().plan
+    assert tplan.kernel.startswith("t3_prep_kernel + trees3_kernel<"), tplan.kernel
     ttable = tserver.graph._object._feature_service.table
     assert ttable.enrich_device(tplan, d_keys.ptr, n, d_out.ptr, d_st.ptr) is False
     rows, found = ttable.lookup(ask)
     want, want_st = tplan.run(rows, with_status=True)
+    before = nat.launch_count()
     got, st, stats = ttable.enrich(tplan, ask, with_stats=True)
-    assert stats["kernels"] == 3
+    assert stats["kernels"] == 5 and nat.launch_count() - before == 5
     np.testing.assert_array_equal(got.view(np.uint32), want.view(np.uint32))
     np.testing.assert_array_equal(st, want_st | np.where(found, 0, nat.ROW_UNKNOWN_KEY))

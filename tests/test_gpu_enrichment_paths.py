@@ -8,8 +8,8 @@ A batch of entity keys reaches the scoring plan one of three ways (csrc/b2s_tabl
   * the gather loader of rowthread_kernel<NCH, NS, TPR, LM = 1> (b2s_table_enrich_device, and b2s_table_enrich_host
     when the plan is fusable): each tile row's key is probed one tile ahead (g_probe_finish) and its row fetched with
     one bulk copy; the table's impute policy folds into the plan's Imputer operands.  `last_kernel` is "rowthread/bulk";
-  * the three-launch fallback of b2s_table_enrich_host for plans the loader declines: lookup, the plan, then
-    mark_unknown_kernel.
+  * the fallback of b2s_table_enrich_host for plans the loader declines: lookup, the plan's launches (three for trees3),
+    then mark_unknown_kernel.
 
 References: gathered rows are a lookup of the table's keys in numpy, then `~isfinite -> policy` wherever the policy is
 not NaN; unknown keys give an all-NaN row.  Rows are compared bit for bit (NaN payloads, +-FLT_MAX, -0.0 and denormals
@@ -444,36 +444,42 @@ def test_fused_onehot_without_policy(sms):
 
 
 # ------------------------------------------------------------------------------------------ the three-launch fallback
-DECLINED = ["dense-12x64", "map-values", "onehot-policy", "f13"]
+DECLINED = ["dense-12x64", "map-values", "onehot-policy", "f13", "trees3"]
 
 
 def declined_case(case, rng):
-    """(F, flow, models, policy, the kernel the plan finalizes to, what serves the fallback's launch)"""
+    """(F, flow, models, policy, the kernel the plan finalizes to, what serves the fallback's launch, plan launches)"""
     if case == "dense-12x64":
         flow = Flow(64)
-        return 64, flow, scorers(64, 12, seed=12), policy_of("half", 64, rng), "dense_head_kernel", "dense"
+        return 64, flow, scorers(64, 12, seed=12), policy_of("half", 64, rng), "dense_head_kernel", "dense", 1
     if case == "map-values":
         F = 20
         flow = Flow(F).map_values(all_mapped(names(F), {"f0": {0: 10, 1: -2}, "f4": {"ranges": {1: ["-inf", 0], 2: [0, "inf"]}}}))
-        return F, flow, scorers(flow.width, 2, seed=20), policy_of("half", F, rng), "rows_kernel<LINEAR,NS=2>", "rows"
+        return F, flow, scorers(flow.width, 2, seed=20), policy_of("half", F, rng), "rows_kernel<LINEAR,NS=2>", "rows", 1
     if case == "onehot-policy":
         F = 16
         flow = Flow(F).one_hot({"f2": [0, 1, 2]})
         pol = policy_of("all", F, rng)
         pol[2] = 1.0  # NaN in the one-hot source becomes category 1
-        return F, flow, scorers(flow.width, 3, seed=16), pol, rowthread(4, 4), "rowthread/bulk"
+        return F, flow, scorers(flow.width, 3, seed=16), pol, rowthread(4, 4), "rowthread/bulk", 1
+    if case == "trees3":  # scikit-learn trees (NaN flags its row), read by the tree prep kernel through a tensor map
+        from tests.test_gpu_tree_paths import gbr, pk
+
+        F = 32
+        models = [pk(gbr(F, 5, 15, seed=3)), pk(gbr(F, 4, 10, seed=4))]
+        return F, Flow(F), models, policy_of("half", F, rng), "t3_prep_kernel + trees3_kernel<", "trees3/tma", 3
     F = 13
     flow = Flow(F).imputer({"f1": 0.5})
-    return F, flow, scorers(F, 3, seed=13), policy_of("half", F, rng), rowthread(4, 4), "rowthread/ldgsts"
+    return F, flow, scorers(F, 3, seed=13), policy_of("half", F, rng), rowthread(4, 4), "rowthread/ldgsts", 1
 
 
 @pytest.mark.parametrize("case", DECLINED)
 def test_declined_plans_through_enrich_host(sms, case):
     """plans the gather loader declines (the dense head with 12 scores, MapValues on rows_kernel, a one-hot source under a
-    table policy, 13 columns): b2s_table_enrich_device launches nothing, b2s_table_enrich_host gathers, runs the plan
-    and marks unknown keys (three launches)"""
+    table policy, 13 columns, trees3): b2s_table_enrich_device launches nothing, b2s_table_enrich_host gathers, runs the
+    plan and marks unknown keys (2 + the plan's launches, reported in stats and counted by the library)"""
     rng = np.random.default_rng(DECLINED.index(case))
-    F, flow, models, pol, kernel, served = declined_case(case, rng)
+    F, flow, models, pol, kernel, served, plan_launches = declined_case(case, rng)
     tab_keys = distinct_keys(6000, rng)
     vals = table_values(len(tab_keys), F, rng, specials=NAN_INF, p=0.05)
     if case == "map-values":
@@ -491,8 +497,10 @@ def test_declined_plans_through_enrich_host(sms, case):
     before = nat.launch_count()
     assert table.enrich_device(plan, d_keys.ptr, n, d_out.ptr, d_st.ptr) is False
     assert nat.launch_count() == before
+    before = nat.launch_count()
     out, st, stats = table.enrich(plan, ask, with_stats=True)
-    assert stats["kernels"] == 3 and stats["rows"] == n
+    assert nat.launch_count() - before == 2 + plan_launches
+    assert stats["kernels"] == 2 + plan_launches and stats["rows"] == n
     assert plan.last_kernel == served, plan.last_kernel
     np.testing.assert_array_equal((st & UNKNOWN) != 0, ~found)
     if case != "dense-12x64":
