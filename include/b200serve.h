@@ -501,6 +501,50 @@ int b2s_pit_train_host(const int64_t* ts, int64_t n, const b2s_pit_set* sets, in
                        int32_t n_cols, const b2s_pit_label* label, int64_t* order, uint64_t* miss, int64_t* kept,
                        float* phase_ms, b2s_stats* stats);
 
+/* Device arrays the library allocated for its caller (cudaMalloc on the library's device), reference counted: the memory
+ * is freed when the last reference goes.  b2s_darray_release drops one.  b2s_darray_dlpack returns a DLPack
+ * DLManagedTensor (the unversioned ABI: kDLCUDA, compact row-major, byte_offset 0) that holds one more; its deleter is a
+ * function of this library that drops it and frees the struct.  b2s_dlpack_delete calls that deleter, for a producer
+ * whose capsule was never consumed.  b2s_darray_live counts the arrays not yet freed. */
+typedef struct b2s_darray_s* b2s_darray_t;
+int b2s_darray_info(b2s_darray_t a, void** ptr, int64_t* bytes);
+int b2s_darray_release(b2s_darray_t a);
+void* b2s_darray_dlpack(b2s_darray_t a, int32_t ndim, const int64_t* shape, int32_t code, int32_t bits);
+int b2s_dlpack_delete(void* managed);
+int64_t b2s_darray_live(void);
+
+/* Training sets as device tensors: b2s_pit_train_host's join and kept rows, packed into one row-major matrix in HBM
+ * instead of copied back.  Matrix column i is feats[i]: output `out` of set `set`, or with set -1 entity column `out`, a
+ * source of `bytes` bytes (the output's or column's own width) of kind B2S_PIT_FEAT_*: a FLOAT of 4 or 8 bytes, an INT
+ * (signed) or UINT of 1, 2, 4 or 8, a BOOL of any of those (nonzero is 1).  Each value is converted to x_bytes (4: float32,
+ * 8: float64) rounding to nearest; a set's value is NaN where the set found no row.  label_vec (may be NULL) is compacted
+ * alongside: a FLOAT keeps its width, an INT / UINT becomes int64, a BOOL one byte 0 / 1.  The library allocates
+ * out->features [kept][n_feats], out->order [kept] (int64: the entity row of each matrix row) and out->label [kept] (NULL
+ * without label_vec) once it knows kept, and the caller releases each with b2s_darray_release; they are ready when the call
+ * returns.  Only the host inputs of `sets` and `cols` are read: every output, found flag, ts_out and entity destination
+ * lives in library scratch, so their pointers may be NULL.  phase_ms (may be NULL) gets 4 times: the sort, the join, the
+ * compaction (keep, scan and pack) and the pack launch alone; stats->kernels counts every launch: the sort's 24 (with ts), the join's max(1, n_sets,
+ * ceil(n_cols / 64)), 2 to find the kept rows and 1 pack launch that writes the matrix, order and label.  B2S_ERR_INVALID
+ * before any launch for what b2s_pit_train_host refuses, a feature or label_vec that names no output or column, or whose
+ * width or kind does not fit, and x_bytes other than 4 or 8; B2S_ERR_CUDA when an allocation fails (*out is then empty). */
+enum { B2S_PIT_FEAT_FLOAT = 0, B2S_PIT_FEAT_INT = 1, B2S_PIT_FEAT_UINT = 2, B2S_PIT_FEAT_BOOL = 3 };
+typedef struct b2s_pit_feat {
+  int32_t set;    /* index of the set, or -1: an entity column */
+  int32_t out;    /* output of that set, or entity column */
+  int32_t bytes;  /* the source's width */
+  int32_t kind;   /* B2S_PIT_FEAT_* */
+} b2s_pit_feat;
+typedef struct b2s_pit_tensors {
+  b2s_darray_t features;  /* [kept][n_feats] float32 or float64, row-major */
+  b2s_darray_t label;     /* [kept], or NULL */
+  b2s_darray_t order;     /* [kept] int64 */
+  int64_t kept;
+} b2s_pit_tensors;
+int b2s_pit_train_pack(const int64_t* ts, int64_t n, const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols,
+                       int32_t n_cols, const b2s_pit_label* label, const b2s_pit_feat* feats, int32_t n_feats,
+                       const b2s_pit_feat* label_vec, int32_t x_bytes, b2s_pit_tensors* out, float* phase_ms,
+                       b2s_stats* stats);
+
 /* ---- windowed aggregations at feature-set ingest ------------------------------------------------------------------
  * storey.AggregateByKey as FeatureSet.add_aggregation places it in a feature set's graph (feature_store/feature_set.py:
  * 715-851), emitting every event: row i gains, per (operation, window), the aggregate over the rows j <= i (input order)

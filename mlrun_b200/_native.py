@@ -78,6 +78,17 @@ class PitLabel(C.Structure):
     _fields_ = [("set", _i32), ("out", _i32), ("kind", _i32)]
 
 
+PIT_FEAT_FLOAT, PIT_FEAT_INT, PIT_FEAT_UINT, PIT_FEAT_BOOL = 0, 1, 2, 3
+
+
+class PitFeat(C.Structure):
+    _fields_ = [("set", _i32), ("out", _i32), ("bytes", _i32), ("kind", _i32)]
+
+
+class PitTensors(C.Structure):
+    _fields_ = [("features", _vp), ("label", _vp), ("order", _vp), ("kept", _i64)]
+
+
 # B2S_AGG_* operation bits, in the order of the outputs of one aggregation
 AGG_OPS = {"count": 1, "sum": 2, "sqr": 4, "max": 8, "min": 16, "first": 32, "last": 64, "avg": 128, "stdvar": 256, "stddev": 512}
 
@@ -176,6 +187,15 @@ SIGNATURES = {
                                        _vp, _vp]),
     "b2s_pit_train_host": (C.c_int, [_vp, _i64, C.POINTER(PitSet), _i32, C.POINTER(PitCol), _i32, C.POINTER(PitLabel), _vp, _vp, _vp,
                                      _pf32, C.POINTER(Stats)]),
+    "b2s_pit_train_pack": (C.c_int, [_vp, _i64, C.POINTER(PitSet), _i32, C.POINTER(PitCol), _i32, C.POINTER(PitLabel),
+                                     C.POINTER(PitFeat), _i32, C.POINTER(PitFeat), _i32, C.POINTER(PitTensors), _pf32,
+                                     C.POINTER(Stats)]),
+    # device arrays handed to the caller
+    "b2s_darray_info": (C.c_int, [_vp, C.POINTER(_vp), C.POINTER(_i64)]),
+    "b2s_darray_release": (C.c_int, [_vp]),
+    "b2s_darray_dlpack": (_vp, [_vp, _i32, C.POINTER(_i64), _i32, _i32]),
+    "b2s_dlpack_delete": (C.c_int, [_vp]),
+    "b2s_darray_live": (_i64, []),
     # windowed aggregations
     "b2s_agg_run_device": (C.c_int, [_vp, _vp, _i64, C.POINTER(AggSpec), _i32, _vp, _vp]),
     "b2s_agg_run_host": (C.c_int, [_vp, _vp, _i64, C.POINTER(AggSpec), _i32, _vp, C.POINTER(Stats)]),
@@ -388,3 +408,89 @@ class PinnedPool:
 
 
 PINNED = PinnedPool()
+
+
+# DLPack data type codes of the typestrs a DeviceArray can have
+_DLPACK_CODES = {"f": 2, "i": 0, "u": 1, "b": 6}
+_DLTENSOR = b"dltensor"
+_pyapi = C.PyDLL(None)  # own function objects: other modules retype the ones ctypes.pythonapi shares
+_capsule_new = _pyapi.PyCapsule_New
+_capsule_new.restype, _capsule_new.argtypes = C.py_object, [C.c_void_p, C.c_char_p, C.c_void_p]
+_capsule_valid = _pyapi.PyCapsule_IsValid
+_capsule_valid.restype, _capsule_valid.argtypes = C.c_int, [C.c_void_p, C.c_char_p]
+_capsule_pointer = _pyapi.PyCapsule_GetPointer
+_capsule_pointer.restype, _capsule_pointer.argtypes = C.c_void_p, [C.c_void_p, C.c_char_p]
+
+
+@C.CFUNCTYPE(None, C.c_void_p)
+def _capsule_destructor(capsule):
+    """a capsule that no consumer took still holds its tensor: the library's deleter frees it (a consumer renames the
+    capsule and calls the deleter itself)"""
+    if _capsule_valid(capsule, _DLTENSOR):
+        load().b2s_dlpack_delete(_capsule_pointer(capsule, _DLTENSOR))
+
+
+class DeviceArray:
+    """a C-order array in device memory the library allocated (b2s_darray_t), freed when the last owner lets go: this
+    object, a consumer of `__cuda_array_interface__` (which keeps this object alive) or of `__dlpack__` (which holds its
+    own reference, dropped by the library's deleter).  Ready when it is handed out."""
+
+    def __init__(self, handle, shape, dtype):
+        self._h = handle
+        self.shape = tuple(int(d) for d in shape)
+        self.dtype = np.dtype(dtype)
+        ptr, nbytes = C.c_void_p(), C.c_int64()
+        check(load().b2s_darray_info(handle, C.byref(ptr), C.byref(nbytes)))
+        self.ptr = ptr.value
+
+    @property
+    def nbytes(self):
+        return int(np.prod(self.shape)) * self.dtype.itemsize
+
+    @property
+    def __cuda_array_interface__(self):
+        return {"shape": self.shape, "typestr": self.dtype.str, "data": (self.ptr, False), "version": 3, "strides": None,
+                "stream": None}
+
+    def __dlpack_device__(self):
+        return (2, _device_ordinal())  # kDLCUDA
+
+    def __dlpack__(self, *, stream=None, max_version=None, dl_device=None, copy=None):
+        if copy:
+            raise BufferError("a DeviceArray is handed over without a copy")
+        if dl_device is not None and tuple(dl_device) != self.__dlpack_device__():
+            raise BufferError(f"the array is on {self.__dlpack_device__()}, not {tuple(dl_device)}")
+        shape = (C.c_int64 * max(len(self.shape), 1))(*self.shape)
+        managed = load().b2s_darray_dlpack(self._h, len(self.shape), shape, _DLPACK_CODES[self.dtype.kind], self.dtype.itemsize * 8)
+        if not managed:
+            raise NativeError(f"DLPack export failed: {load().b2s_last_error().decode()}")
+        return _capsule_new(managed, _DLTENSOR, C.cast(_capsule_destructor, C.c_void_p))
+
+    def numpy(self):
+        """a host copy"""
+        out = np.empty(self.shape, dtype=self.dtype)
+        if out.nbytes:
+            check(load().b2s_memcpy_d2h(out.ctypes.data, self.ptr, out.nbytes))
+        return out
+
+    def release(self):
+        if self._h:
+            load().b2s_darray_release(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.release()
+        except Exception:
+            pass
+
+
+def _device_ordinal():
+    info = DevInfo()
+    check(load().b2s_device_info(C.byref(info)))
+    return int(info.ordinal)
+
+
+def darray_live():
+    """device arrays the library has handed out and not yet freed"""
+    return int(load().b2s_darray_live())

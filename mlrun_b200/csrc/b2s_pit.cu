@@ -12,6 +12,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <atomic>
 #include <cstdint>
 #include <cstring>
 #include <exception>
@@ -565,6 +566,133 @@ __global__ void __launch_bounds__(kTile) scatter_kernel(const __grid_constant__ 
   }
 }
 
+// ---- training sets as device tensors: the kept rows of the selected columns, packed into one row-major matrix -----------
+constexpr int kPackCols = 32;  // matrix columns one pack block writes: a 128-byte (float32) / 256-byte (float64) row segment
+
+struct PackCol {
+  const void* src;       // [n] the join's column, in sorted order
+  const uint8_t* found;  // [n] its set's found flags (NaN where 0); null: an entity column
+  int32_t bytes, kind;   // B2S_PIT_FEAT_*
+};
+
+struct PackParams {
+  const PackCol* cols;  // [n_feats] device memory
+  int32_t n_feats;
+  void* x;              // [kept][n_feats] float / double
+  PackCol label;
+  void* y;              // [kept] the label (FLOAT: its width, INT / UINT: int64, BOOL: one byte); null: none
+  const int64_t* order_src;
+  int64_t* order;       // [kept]
+  int64_t n;
+};
+
+template <class T>
+__device__ __forceinline__ T nan_of();
+template <>
+__device__ __forceinline__ float nan_of<float>() { return __int_as_float(0x7fc00000); }
+template <>
+__device__ __forceinline__ double nan_of<double>() { return __longlong_as_double(0x7ff8000000000000ll); }
+
+// element q of a column as T: C conversions, which round to nearest
+template <class T>
+__device__ __forceinline__ T convert(const void* src, int64_t q, int bytes, int kind) {
+  switch (kind) {
+    case B2S_PIT_FEAT_FLOAT:
+      return bytes == 4 ? (T)static_cast<const float*>(src)[q] : (T)static_cast<const double*>(src)[q];
+    case B2S_PIT_FEAT_INT:
+      switch (bytes) {
+        case 1: return (T)static_cast<const int8_t*>(src)[q];
+        case 2: return (T)static_cast<const int16_t*>(src)[q];
+        case 4: return (T)static_cast<const int32_t*>(src)[q];
+        default: return (T)static_cast<const int64_t*>(src)[q];
+      }
+    case B2S_PIT_FEAT_UINT:
+      switch (bytes) {
+        case 1: return (T)static_cast<const uint8_t*>(src)[q];
+        case 2: return (T)static_cast<const uint16_t*>(src)[q];
+        case 4: return (T)static_cast<const uint32_t*>(src)[q];
+        default: return (T)static_cast<const uint64_t*>(src)[q];
+      }
+    default: {  // BOOL
+      bool nz;
+      switch (bytes) {
+        case 1: nz = static_cast<const uint8_t*>(src)[q] != 0; break;
+        case 2: nz = static_cast<const uint16_t*>(src)[q] != 0; break;
+        case 4: nz = static_cast<const uint32_t*>(src)[q] != 0; break;
+        default: nz = static_cast<const uint64_t*>(src)[q] != 0; break;
+      }
+      return nz ? T(1) : T(0);
+    }
+  }
+}
+
+template <class T>
+__device__ __forceinline__ T pack_value(const PackCol& c, int64_t q) {
+  return c.found && !c.found[q] ? nan_of<T>() : convert<T>(c.src, q, c.bytes, c.kind);
+}
+
+// Block (tile, chunk): the tile's kept rows of matrix columns [32 * chunk, + 32), at tile_off[tile] onward.  Each step
+// gathers rows x columns of the chunk into shared memory, a warp reading consecutive kept rows of one column, and writes
+// them out along the matrix rows, so that consecutive threads write consecutive addresses (one contiguous run of the
+// matrix when the chunk is the whole row).  The chunk-0 blocks also compact order and the label.
+template <class T>
+__global__ void __launch_bounds__(kTile) pack_kernel(const __grid_constant__ PackParams p, const uint8_t* __restrict__ keep,
+                                                     const int64_t* __restrict__ tile_off) {
+  __shared__ int s_warp[kTile / 32];
+  __shared__ int s_row[kTile];           // the tile's kept rows in order, as offsets in the tile
+  __shared__ PackCol s_col[kPackCols];
+  __shared__ T s_tile[kTile + kTile / 2];  // rows x (columns | 1) with rows = kTile / columns: at most 1.5 kTile
+  const int64_t q0 = (int64_t)blockIdx.x * kTile;
+  const bool k = q0 + threadIdx.x < p.n && keep[q0 + threadIdx.x];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned bal = __ballot_sync(0xffffffffu, k);
+  if (lane == 0) s_warp[warp] = __popc(bal);
+  const int c0 = blockIdx.y * kPackCols, cw = min(kPackCols, p.n_feats - c0);
+  if ((int)threadIdx.x < cw) s_col[threadIdx.x] = p.cols[c0 + threadIdx.x];
+  const int count = __syncthreads_count(k);
+  if (warp == 0) {  // exclusive scan of the 32 warp counts
+    const int c = s_warp[lane];
+    int v = c;
+    for (int off = 1; off < 32; off <<= 1) {
+      const int u = __shfl_up_sync(0xffffffffu, v, off);
+      if (lane >= off) v += u;
+    }
+    s_warp[lane] = v - c;
+  }
+  __syncthreads();
+  if (k) s_row[s_warp[warp] + __popc(bal & ((1u << lane) - 1u))] = threadIdx.x;
+  __syncthreads();
+  const int64_t base = tile_off[blockIdx.x];
+  if (blockIdx.y == 0 && (int)threadIdx.x < count) {
+    const int64_t q = q0 + s_row[threadIdx.x], d = base + threadIdx.x;
+    p.order[d] = p.order_src[q];
+    if (p.y) {
+      const PackCol& l = p.label;
+      switch (l.kind) {
+        case B2S_PIT_FEAT_FLOAT:
+          if (l.bytes == 4) static_cast<float*>(p.y)[d] = static_cast<const float*>(l.src)[q];
+          else static_cast<double*>(p.y)[d] = static_cast<const double*>(l.src)[q];
+          break;
+        case B2S_PIT_FEAT_BOOL: static_cast<uint8_t*>(p.y)[d] = convert<int>(l.src, q, l.bytes, l.kind); break;
+        case B2S_PIT_FEAT_UINT: static_cast<int64_t*>(p.y)[d] = (int64_t)convert<uint64_t>(l.src, q, l.bytes, l.kind); break;
+        default: static_cast<int64_t*>(p.y)[d] = convert<int64_t>(l.src, q, l.bytes, l.kind); break;
+      }
+    }
+  }
+  if (cw <= 0) return;  // no feature columns: this launch only compacts order and the label
+  const int rows = kTile / cw, stride = cw | 1;  // an odd row stride: a warp's column reads hit distinct banks
+  const int gr = threadIdx.x % rows, gc = threadIdx.x / rows;  // gather: lanes run down the kept rows of column gc
+  const int wr = threadIdx.x / cw, wc = threadIdx.x % cw;      // write: lanes run along matrix row wr
+  T* x = static_cast<T*>(p.x);
+  for (int r0 = 0; r0 < count; r0 += rows) {
+    const int nr = min(rows, count - r0);
+    if (gc < cw && gr < nr) s_tile[gr * stride + gc] = pack_value<T>(s_col[gc], q0 + s_row[r0 + gr]);
+    __syncthreads();
+    if (wr < nr) x[(base + r0 + wr) * p.n_feats + c0 + wc] = s_tile[wr * stride + wc];
+    __syncthreads();
+  }
+}
+
 int check_train(const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols, int32_t n_cols, const int64_t* ts, int64_t n,
                 const b2s_pit_label* label, const void* miss, const void* kept) {
   if (int rc = check_sets(sets, n_sets, cols, n_cols, ts, n)) return rc;
@@ -587,12 +715,27 @@ int check_train(const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols
   return B2S_OK;
 }
 
+// What b2s_pit_train_pack asks of train_run: the matrix columns, the label vector and x_bytes; the results go to *out.
+// ev: two events recorded around the pack launch (may be null).
+struct Pack {
+  const b2s_pit_feat* feats;
+  int32_t n_feats;
+  const b2s_pit_feat* label;
+  int32_t x_bytes;
+  b2s_pit_tensors* out;
+  const cudaEvent_t* ev;
+};
+
 // The join of n rows into scratch copies of every output, then the kept rows of each into the caller's arrays (device
 // memory: sets[s].outs[j].out, ts_out, found, cols[c].dst, d_order).  d_miss and *d_kept are written.  ev (may be null):
 // four events recorded before the sort, after it, after the join and after the compaction.
+// With `pack`, the kept rows are packed into the matrix it describes instead (pack_rows), and ev[3] is recorded before that.
+int pack_rows(const Pack& pk, const DeviceDescs& d, const uint8_t* d_keep, const int64_t* d_off, const int64_t* d_kept, PackCol* d_cols,
+              int64_t n, cudaStream_t st, Launches& launches);
+
 int train_run(const int64_t* d_ts, int64_t n, const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols, int32_t n_cols,
               const b2s_pit_label* label, int64_t* d_order, unsigned long long* d_miss, int64_t* d_kept, cudaStream_t st,
-              const cudaEvent_t* ev, Launches& launches) {
+              const cudaEvent_t* ev, Launches& launches, const Pack* pack = nullptr) {
   const int64_t n_tiles = (n + kTile - 1) / kTile;
   // scratch: one n-row copy of every output, the join's own miss counters, the keep flags and the tile counts
   DeviceBlock blk(st);
@@ -601,6 +744,8 @@ int train_run(const int64_t* d_ts, int64_t n, const b2s_pit_set* sets, int32_t n
   int64_t* d_count = nullptr;
   blk.scratch(d_keep, (size_t)n);
   blk.scratch(d_count, (size_t)n_tiles * 8);
+  PackCol* d_pack_cols = nullptr;
+  if (pack) blk.scratch(d_pack_cols, sizeof(PackCol) * (size_t)std::max(pack->n_feats, 1));
   if (int rc = blk.alloc()) return rc;
   B2S_CUDA_TRY(cudaMemsetAsync(d.miss, 0, 8 * (size_t)std::max(n_sets, 1), st));
   if (n_sets) B2S_CUDA_TRY(cudaMemsetAsync(d_miss, 0, 8 * (size_t)n_sets, st));
@@ -634,6 +779,10 @@ int train_run(const int64_t* d_ts, int64_t n, const b2s_pit_set* sets, int32_t n
   keep_kernel<<<(unsigned)n_tiles, kTile, 0, st>>>(kp, d_keep, d_count, d_miss);
   scan_tiles_kernel<<<1, 1024, 0, st>>>(d_count, n_tiles, d_kept);
   launches.add(2);
+  if (pack) {
+    if (ev) B2S_CUDA_TRY(cudaEventRecord(ev[3], st));
+    return pack_rows(*pack, d, d_keep, d_count, d_kept, d_pack_cols, n, st, launches);
+  }
   // each scratch copy's kept rows go to the array it stands for
   const std::vector<DeviceBlock::Out>& moves = blk.outputs();
   for (size_t i = 0; i < moves.size(); i += kScatterCols) {
@@ -728,6 +877,301 @@ extern "C" int b2s_pit_train_host(const int64_t* ts, int64_t n, const b2s_pit_se
     }
     return B2S_OK;
   } catch (const std::exception& e) {
+    return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
+  }
+}
+
+// ---- training sets as device tensors ---------------------------------------------------------------------------------
+struct b2s_darray_s {
+  void* ptr;
+  int64_t bytes;
+  std::atomic<int> refs{1};
+};
+
+namespace {
+
+std::atomic<int64_t> g_darrays{0};  // arrays not yet freed (b2s_darray_live)
+// the destination of every output b2s_pit_train_pack joins: train_run gives each a scratch region and never writes here
+alignas(8) char g_stand_in[8];
+
+int darray_new(b2s_darray_t& a, int64_t bytes) {
+  void* p = nullptr;
+  B2S_CUDA_TRY(cudaMalloc(&p, (size_t)std::max<int64_t>(bytes, 1)));  // never null: an empty array still has an address
+  a = new b2s_darray_s();
+  a->ptr = p;
+  a->bytes = bytes;
+  ++g_darrays;
+  return B2S_OK;
+}
+
+void darray_unref(b2s_darray_t a) {
+  if (a && a->refs.fetch_sub(1) == 1) {
+    cudaFree(a->ptr);
+    delete a;
+    --g_darrays;
+  }
+}
+
+// the DLPack ABI (dlpack.h, unversioned DLManagedTensor)
+struct DLDevice {
+  int32_t device_type;  // kDLCUDA = 2
+  int32_t device_id;
+};
+struct DLDataType {
+  uint8_t code;  // kDLInt 0, kDLUInt 1, kDLFloat 2, kDLBool 6
+  uint8_t bits;
+  uint16_t lanes;
+};
+struct DLTensor {
+  void* data;
+  DLDevice device;
+  int32_t ndim;
+  DLDataType dtype;
+  int64_t* shape;
+  int64_t* strides;  // null: compact row-major
+  uint64_t byte_offset;
+};
+struct DLManagedTensor {
+  DLTensor dl_tensor;
+  void* manager_ctx;
+  void (*deleter)(DLManagedTensor* self);
+};
+struct Managed {
+  DLManagedTensor m;
+  b2s_darray_t array;
+  int64_t shape[8];
+};
+
+void dlpack_deleter(DLManagedTensor* self) {
+  Managed* h = static_cast<Managed*>(self->manager_ctx);
+  darray_unref(h->array);
+  delete h;
+}
+
+void release_tensors(b2s_pit_tensors& t) {
+  darray_unref(t.features);
+  darray_unref(t.label);
+  darray_unref(t.order);
+  t = b2s_pit_tensors{};
+}
+
+int label_vec_bytes(const b2s_pit_feat& f) {
+  return f.kind == B2S_PIT_FEAT_FLOAT ? f.bytes : f.kind == B2S_PIT_FEAT_BOOL ? 1 : 8;
+}
+
+PackCol pack_source(const DeviceDescs& d, const b2s_pit_feat& f) {
+  if (f.set >= 0) return PackCol{d.outs[f.set][f.out].out, d.sets[f.set].found, f.bytes, f.kind};
+  return PackCol{d.cols[f.out].dst, nullptr, f.bytes, f.kind};
+}
+
+}  // namespace
+
+namespace {
+
+// the matrix, order and label of the kept rows: allocated once *d_kept is known, then one pack launch
+int pack_rows(const Pack& pk, const DeviceDescs& d, const uint8_t* d_keep, const int64_t* d_off, const int64_t* d_kept, PackCol* d_cols,
+              int64_t n, cudaStream_t st, Launches& launches) {
+  int64_t kept = 0;
+  B2S_CUDA_TRY(cudaMemcpyAsync(&kept, d_kept, 8, cudaMemcpyDeviceToHost, st));
+  B2S_CUDA_TRY(cudaStreamSynchronize(st));
+  b2s_pit_tensors& o = *pk.out;
+  o.kept = kept;
+  if (int rc = darray_new(o.features, kept * pk.n_feats * pk.x_bytes)) return rc;
+  if (int rc = darray_new(o.order, kept * 8)) return rc;
+  if (pk.label)
+    if (int rc = darray_new(o.label, kept * label_vec_bytes(*pk.label))) return rc;
+  std::vector<PackCol> cols(pk.n_feats);
+  for (int i = 0; i < pk.n_feats; ++i) cols[i] = pack_source(d, pk.feats[i]);
+  if (pk.n_feats) B2S_CUDA_TRY(cudaMemcpyAsync(d_cols, cols.data(), sizeof(PackCol) * cols.size(), cudaMemcpyHostToDevice, st));
+  PackParams p{};
+  p.cols = d_cols;
+  p.n_feats = pk.n_feats;
+  p.x = o.features->ptr;
+  if (pk.label) {
+    p.label = pack_source(d, *pk.label);
+    p.y = o.label->ptr;
+  }
+  p.order_src = d.order;
+  p.order = static_cast<int64_t*>(o.order->ptr);
+  p.n = n;
+  const dim3 grid((unsigned)((n + kTile - 1) / kTile), (unsigned)std::max(1, (pk.n_feats + kPackCols - 1) / kPackCols));
+  if (pk.ev) B2S_CUDA_TRY(cudaEventRecord(pk.ev[0], st));
+  if (pk.x_bytes == 4) pack_kernel<float><<<grid, kTile, 0, st>>>(p, d_keep, d_off);
+  else pack_kernel<double><<<grid, kTile, 0, st>>>(p, d_keep, d_off);
+  launches.add(1);
+  if (pk.ev) B2S_CUDA_TRY(cudaEventRecord(pk.ev[1], st));
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return b2s_int_fail(B2S_ERR_CUDA, "pack launch failed: %s", cudaGetErrorString(e));
+  return B2S_OK;
+}
+
+int check_feat(const b2s_pit_feat& f, const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols, int32_t n_cols, const char* what,
+               int i) {
+  int width = 0;
+  if (f.set >= 0 && f.set < n_sets && f.out >= 0 && f.out < sets[f.set].n_out)
+    width = sets[f.set].outs[f.out].bytes;
+  else if (f.set == -1 && f.out >= 0 && f.out < n_cols)
+    width = cols[f.out].bytes;
+  if (!width) return b2s_int_fail(B2S_ERR_INVALID, "%s %d (set %d, output %d): no such output or entity column", what, i, f.set, f.out);
+  const bool fits = f.kind == B2S_PIT_FEAT_FLOAT ? (f.bytes == 4 || f.bytes == 8)
+                                                  : (f.kind == B2S_PIT_FEAT_INT || f.kind == B2S_PIT_FEAT_UINT || f.kind == B2S_PIT_FEAT_BOOL);
+  if (f.bytes != width || !fits)
+    return b2s_int_fail(B2S_ERR_INVALID, "%s %d: kind %d of %d bytes does not fit a %d-byte source", what, i, f.kind, f.bytes, width);
+  return B2S_OK;
+}
+
+}  // namespace
+
+namespace {
+
+// n = 0: empty arrays, no launch
+int pack_empty(b2s_pit_tensors& out, bool label) {
+  if (int rc = darray_new(out.features, 0)) return rc;
+  if (int rc = darray_new(out.order, 0)) return rc;
+  return label ? darray_new(out.label, 0) : B2S_OK;
+}
+
+// b2s_pit_train_pack over n > 0 rows: sets / cols are checked host descriptors whose destinations are stand-ins
+int pack_call(const int64_t* ts, int64_t n, b2s_pit_set* sets, int32_t n_sets, b2s_pit_col* cols, int32_t n_cols,
+              const b2s_pit_label* label, Pack pk, float* phase_ms, b2s_stats* stats) {
+  cudaStream_t st = b2s_int_stream();
+  Events ev;
+  if (int rc = ev.create(7)) return rc;
+  pk.ev = ev.data() + 5;
+  Launches launches;
+  {
+    // one device block for the inputs and the counters: the outputs are train_run's scratch
+    SyncOnExit done{st};
+    DeviceBlock blk(st);
+    const int64_t* d_ts = nullptr;
+    if (ts) blk.input(d_ts, ts, (size_t)n * 8);
+    for (int s = 0; s < n_sets; ++s) blk.input(sets[s].keys, sets[s].keys, (size_t)n * 8);
+    for (int c = 0; c < n_cols; ++c) blk.input(cols[c].src, cols[c].src, (size_t)n * cols[c].bytes);
+    unsigned long long* d_miss = nullptr;
+    int64_t* d_kept = nullptr;
+    blk.scratch(d_miss, 8 * (size_t)std::max(n_sets, 1));
+    blk.scratch(d_kept, 8);
+    if (int rc = blk.alloc()) return rc;
+    B2S_CUDA_TRY(cudaEventRecord(ev[0], st));
+    if (int rc = blk.upload()) return rc;
+    if (int rc = train_run(d_ts, n, sets, n_sets, cols, n_cols, label, reinterpret_cast<int64_t*>(g_stand_in),
+                           d_miss, d_kept, st, ev.data() + 1, launches, &pk))
+      return rc;
+  }
+  B2S_CUDA_TRY(cudaStreamSynchronize(st));
+  float keep_ms = 0.f, pack_ms = 0.f;
+  cudaEventElapsedTime(&keep_ms, ev[3], ev[4]);  // keep + scan
+  cudaEventElapsedTime(&pack_ms, ev[5], ev[6]);
+  if (phase_ms) {
+    cudaEventElapsedTime(&phase_ms[0], ev[1], ev[2]);  // sort
+    cudaEventElapsedTime(&phase_ms[1], ev[2], ev[3]);  // join
+    phase_ms[2] = keep_ms + pack_ms;                   // compaction (the host reads kept between the two)
+    phase_ms[3] = pack_ms;
+  }
+  if (stats) {
+    stats->rows = n;
+    cudaEventElapsedTime(&stats->h2d_ms, ev[0], ev[1]);
+    cudaEventElapsedTime(&stats->kernel_ms, ev[1], ev[4]);
+    stats->kernel_ms += pack_ms;
+    stats->kernels = launches.n;
+  }
+  return B2S_OK;
+}
+
+}  // namespace
+
+extern "C" int b2s_darray_info(b2s_darray_t a, void** ptr, int64_t* bytes) {
+  if (!a) return b2s_int_fail(B2S_ERR_INVALID, "null array");
+  if (ptr) *ptr = a->ptr;
+  if (bytes) *bytes = a->bytes;
+  return B2S_OK;
+}
+
+extern "C" int b2s_darray_release(b2s_darray_t a) {
+  darray_unref(a);
+  return B2S_OK;
+}
+
+extern "C" void* b2s_darray_dlpack(b2s_darray_t a, int32_t ndim, const int64_t* shape, int32_t code, int32_t bits) {
+  try {  // no C++ exception crosses the C boundary
+    if (!a || ndim < 0 || ndim > 8 || (ndim && !shape) || code < 0 || code > 255 || bits <= 0 || bits % 8) {
+      b2s_int_fail(B2S_ERR_INVALID, "bad arguments");
+      return nullptr;
+    }
+    int64_t elems = 1;
+    for (int i = 0; i < ndim; ++i) elems = shape[i] < 0 ? -1 : elems * shape[i];
+    if (elems < 0 || elems * (bits / 8) > a->bytes) {
+      b2s_int_fail(B2S_ERR_INVALID, "the shape does not fit the array's %lld bytes", (long long)a->bytes);
+      return nullptr;
+    }
+    Managed* h = new Managed();
+    for (int i = 0; i < ndim; ++i) h->shape[i] = shape[i];
+    h->array = a;
+    a->refs.fetch_add(1);
+    DLTensor& t = h->m.dl_tensor;
+    t.data = a->ptr;
+    t.device = DLDevice{2, b2s_int_device()};
+    t.ndim = ndim;
+    t.dtype = DLDataType{(uint8_t)code, (uint8_t)bits, 1};
+    t.shape = h->shape;
+    h->m.manager_ctx = h;
+    h->m.deleter = dlpack_deleter;
+    return &h->m;
+  } catch (const std::exception& e) {
+    b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
+    return nullptr;
+  }
+}
+
+extern "C" int b2s_dlpack_delete(void* managed) {
+  DLManagedTensor* m = static_cast<DLManagedTensor*>(managed);
+  if (m && m->deleter) m->deleter(m);
+  return B2S_OK;
+}
+
+extern "C" int64_t b2s_darray_live(void) { return g_darrays.load(); }
+
+extern "C" int b2s_pit_train_pack(const int64_t* ts, int64_t n, const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols,
+                                  int32_t n_cols, const b2s_pit_label* label, const b2s_pit_feat* feats, int32_t n_feats,
+                                  const b2s_pit_feat* label_vec, int32_t x_bytes, b2s_pit_tensors* out, float* phase_ms,
+                                  b2s_stats* stats) {
+  try {  // no C++ exception crosses the C boundary
+    if (!out || n_sets < 0 || n_cols < 0 || n_feats < 0 || (n_sets && !sets) || (n_cols && !cols) || (n_feats && !feats))
+      return b2s_int_fail(B2S_ERR_INVALID, "bad arguments");
+    if (x_bytes != 4 && x_bytes != 8) return b2s_int_fail(B2S_ERR_INVALID, "x_bytes %d: the matrix is float32 (4) or float64 (8)", x_bytes);
+    *out = b2s_pit_tensors{};
+    // every output, found flag and entity destination lives in scratch: the checks of b2s_pit_train_host run on copies
+    // whose destinations stand in for those regions
+    std::vector<b2s_pit_set> s2(sets, sets + n_sets);
+    std::vector<std::vector<b2s_pit_out>> o2(n_sets);
+    for (int s = 0; s < n_sets; ++s) {
+      if (s2[s].n_out < 0 || s2[s].n_out > kMaxOuts || (s2[s].n_out && !s2[s].outs))
+        return b2s_int_fail(B2S_ERR_INVALID, "set %d: null index / keys / outputs", s);
+      o2[s].assign(s2[s].outs, s2[s].outs + s2[s].n_out);
+      for (b2s_pit_out& o : o2[s]) o.out = g_stand_in;
+      s2[s].outs = o2[s].data();
+      s2[s].found = reinterpret_cast<uint8_t*>(g_stand_in);
+      s2[s].ts_out = nullptr;
+    }
+    std::vector<b2s_pit_col> c2(cols, cols + n_cols);
+    for (b2s_pit_col& c : c2) c.dst = g_stand_in;
+    int64_t counters[2];
+    if (int rc = check_train(s2.data(), n_sets, c2.data(), n_cols, ts, n, label, counters, counters + 1)) return rc;
+    for (int i = 0; i < n_feats; ++i)
+      if (int rc = check_feat(feats[i], s2.data(), n_sets, c2.data(), n_cols, "feature", i)) return rc;
+    if (label_vec)
+      if (int rc = check_feat(*label_vec, s2.data(), n_sets, c2.data(), n_cols, "label", 0)) return rc;
+    if (phase_ms) phase_ms[0] = phase_ms[1] = phase_ms[2] = phase_ms[3] = 0.f;
+    if (stats) memset(stats, 0, sizeof(*stats));
+    if (!b2s_int_inited()) return b2s_int_fail(B2S_ERR_STATE, "b2s_init was not called (no CUDA device: there is no CPU fallback)");
+    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
+    const int rc = n ? pack_call(ts, n, s2.data(), n_sets, c2.data(), n_cols, label, Pack{feats, n_feats, label_vec, x_bytes, out, nullptr},
+                                 phase_ms, stats)
+                     : pack_empty(*out, label_vec != nullptr);
+    if (rc) release_tensors(*out);
+    return rc;
+  } catch (const std::exception& e) {
+    if (out) release_tensors(*out);
     return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
   }
 }

@@ -129,6 +129,55 @@ def pit_train(ts, sets, cols, label, with_stats=False):
     return res + (dict(sort_ms=phase[0], join_ms=phase[1], compact_ms=phase[2], kept=k, **stats.as_dict()),) if with_stats else res
 
 
+def pit_train_pack(ts, sets, cols, label, feats, label_vec, dtype):
+    """pit_train's rows packed on the device (b2s_pit_train_pack): feats [(set index or -1, output or column index,
+    bytes, nat.PIT_FEAT_*)] are the matrix columns, label_vec the label vector's source (or None), dtype float32 /
+    float64 -> (features [kept, F], label [kept] or None, order [kept]: nat.DeviceArray, {sort_ms, join_ms, compact_ms,
+    pack_ms, kept, **stats})"""
+    lib = nat.init()
+    n = len(ts) if ts is not None else len(cols[0]) if cols else len(sets[0][1]) if sets else 0
+    ts = None if ts is None else np.ascontiguousarray(ts, dtype=np.int64)
+    keep = []  # arrays the descriptors point into
+    c_sets = (nat.PitSet * max(len(sets), 1))()
+    for i, (index, keys, asof, outs) in enumerate(sets):
+        keys = np.ascontiguousarray(keys, dtype=np.int64)
+        descs = (nat.PitOut * max(len(outs), 1))(*[nat.PitOut(w, np.dtype(dt).itemsize, m, None) for w, dt, m in outs])
+        keep += [keys, descs]
+        c_sets[i] = nat.PitSet(index._h, keys.ctypes.data, int(asof), len(outs), descs, None, None)
+    srcs = [np.ascontiguousarray(c) for c in cols]
+    c_cols = (nat.PitCol * max(len(cols), 1))(*[nat.PitCol(s.ctypes.data, None, s.dtype.itemsize) for s in srcs])
+    c_label = None if label is None else C.byref(nat.PitLabel(*label))
+    c_feats = (nat.PitFeat * max(len(feats), 1))(*[nat.PitFeat(*f) for f in feats])
+    c_vec = None if label_vec is None else C.byref(nat.PitFeat(*label_vec))
+    out = nat.PitTensors()
+    phase = (C.c_float * 4)()
+    stats = nat.Stats()
+    nat.check(lib.b2s_pit_train_pack(None if ts is None else ts.ctypes.data, n, c_sets, len(sets), c_cols, len(cols), c_label,
+                                     c_feats, len(feats), c_vec, np.dtype(dtype).itemsize, C.byref(out), phase, C.byref(stats)))
+    k = out.kept
+    features = nat.DeviceArray(out.features, (k, len(feats)), dtype)
+    order = nat.DeviceArray(out.order, (k,), np.int64)
+    y = None if label_vec is None else nat.DeviceArray(out.label, (k,), _label_dtype(label_vec))
+    return features, y, order, dict(sort_ms=phase[0], join_ms=phase[1], compact_ms=phase[2], pack_ms=phase[3], kept=k,
+                                    **stats.as_dict())
+
+
+def _label_dtype(label_vec):
+    """the label vector's dtype for its source (set, output, bytes, kind): floats keep their width, ints become int64"""
+    _s, _o, width, kind = label_vec
+    return {nat.PIT_FEAT_FLOAT: np.float32 if width == 4 else np.float64, nat.PIT_FEAT_BOOL: np.bool_}.get(kind, np.int64)
+
+
+class TrainingTensors:
+    """a training set where the device built it: `features` [rows, F] (C order) and `label` [rows] (None without a label
+    feature) as device arrays that any CUDA framework takes without a copy (`__cuda_array_interface__`, `__dlpack__`),
+    `order` [rows] the entity-frame row of each, `columns` the F feature names; `rows` and `stats` are the launch's"""
+
+    def __init__(self, features, label, order, columns, rows, stats):
+        self.features, self.label, self.order = features, label, order
+        self.columns, self.rows, self.stats = list(columns), rows, stats
+
+
 class OfflineSource:
     """one feature set's offline frame, registered with its device index (built once)"""
 
@@ -268,13 +317,15 @@ def _restore(values, dtype, found, missed):
     return out
 
 
-def get_offline_features(feature_vector, entity_rows=None, entity_timestamp_column=None, target=None, run_config=None,
-                         drop_columns=None, start_time=None, end_time=None, with_indexes=False, update_stats=False, engine=None,
-                         engine_args=None, query=None, order_by=None, spark_service=None, timestamp_for_filtering=None,
-                         additional_filters=None):
-    """feature_store/api.py:99 on the local engine: the training frame of `feature_vector` for `entity_rows`, point-in-time
-    correct per feature set.  What the device does not run is refused with LoweringError (there is no pandas fallback)."""
-    vector = feature_vector
+class _Query:
+    """a vector's query, planned (`_plan_query`): what the device is asked and what the host names"""
+
+
+def _plan_query(vector, entity_rows=None, entity_timestamp_column=None, target=None, run_config=None, drop_columns=None,
+                start_time=None, end_time=None, with_indexes=False, update_stats=False, engine=None, engine_args=None, query=None,
+                order_by=None, spark_service=None, timestamp_for_filtering=None, additional_filters=None):
+    """the one planner of `get_offline_features` and `get_offline_tensors`: refusals, the parsed fields and label, the
+    entity-less spine, the join of each set, the entity timestamps and the device descriptors"""
     if entity_rows is None and entity_timestamp_column is not None:  # api.py:228-232
         raise MLRunInvalidArgumentError("entity_timestamp_column param can not be specified without entity_rows param")
     if engine not in (None, "local"):
@@ -297,7 +348,7 @@ def get_offline_features(feature_vector, entity_rows=None, entity_timestamp_colu
         label = tuple(spec.split(".", 1))
     drop_indexes = not (vector.with_indexes or with_indexes)
     fields = _parse(vector, label)
-    spine_alias = {}
+    spine_alias, spine_features = {}, []
     entity_less = entity_rows is None
     if entity_less:
         # the first set's own rows are the frame the others join (base.py:202-216, 268-285, 427-428): its entities, its
@@ -310,7 +361,8 @@ def get_offline_features(feature_vector, entity_rows=None, entity_timestamp_colu
                                     "relations between differently keyed feature sets are not lowered")
         head = spine.entities + ([spine.timestamp_key] if spine.timestamp_key else [])
         entity_rows = spine.frame[head + [f for f, _a in fields[spine_name]]].copy(deep=False)
-        entity_rows.columns = head + [f"{f}_{spine_name}" for f, _a in fields[spine_name]]
+        spine_features = [f"{f}_{spine_name}" for f, _a in fields[spine_name]]
+        entity_rows.columns = head + spine_features
         entity_rows = entity_rows.reset_index(drop=True)
         entity_timestamp_column = spine.timestamp_key
         spine_alias = dict(([(c, c) for c in head] if not drop_indexes else []) +
@@ -373,7 +425,6 @@ def get_offline_features(feature_vector, entity_rows=None, entity_timestamp_colu
     dev_cols = [c for c in entity_rows.columns if entity_rows[c].dtype.kind in "iufMb" and getattr(entity_rows[c].dtype, "tz", None) is None
                 and isinstance(entity_rows[c].dtype, np.dtype)]
     arrays = [entity_rows[c].to_numpy() for c in dev_cols]
-    train = label is not None or entity_less
     dev_label = None
     if label is not None:  # the label's place on the device: an output of its set, or the spine's own column
         lname, lfeat = label
@@ -385,40 +436,30 @@ def get_offline_features(feature_vector, entity_rows=None, entity_timestamp_colu
             dev_label = (s_i, max(j for j, (f, _a) in enumerate(fields[lname]) if f == lfeat), kind)
         else:
             dev_label = (-1, dev_cols.index(f"{lfeat}_{lname}"), kind)
-    if not n:
-        order, joined, permuted, miss = (
-            np.zeros(0, np.int64), [([np.zeros(0, dt) for _w, dt, _m in s[3]], np.zeros(0, np.int64), np.zeros(0, bool)) for s in sets],
-            [a[:0] for a in arrays], np.zeros(len(sets), np.uint64))
-    elif train:
-        order, joined, permuted, miss = pit_train(ts_ns, sets, arrays, dev_label)
-    else:
-        order, joined, permuted, _miss = pit_join(ts_ns, sets, arrays)
-    moved = dict(zip(dev_cols, permuted))
+    q = _Query()
+    q.fields, q.label, q.dev_label, q.plan, q.sets = fields, label, dev_label, plan, sets
+    q.entity_rows, q.entity_ts, q.ts_col, q.ts_ns, q.unit, q.n = entity_rows, entity_ts, ts_col, ts_ns, unit, n
+    q.dev_cols, q.arrays, q.spine_alias, q.spine_features = dev_cols, arrays, spine_alias, spine_features
+    q.index_columns, q.entity_less, q.drop_indexes = index_columns, entity_less, drop_indexes
+    q.train = label is not None or entity_less
+    return q
 
+
+def _layout(q):
+    """the training frame's columns by name alone -> ([(name, source)] in frame order, index columns); a source is
+    ("entity", entity column), ("ts", set) or ("out", set, output)"""
     # the merged frame, set by set (local_merger.py:58-66 / 93-100): right columns after the left ones, the keys and an
     # equally named timestamp once, colliding names suffixed `_<set>_` (then dropped)
-    cols = {}
-    for c in entity_rows.columns:
-        if c in moved:
-            v = moved[c]
-            cols[c] = v.view(entity_rows[c].dtype) if v.dtype != entity_rows[c].dtype else v
-        else:  # strings, categories, objects: permuted on the host in the device's order
-            cols[c] = entity_rows[c].take(order).reset_index(drop=True).array
+    cols = {c: ("entity", c) for c in q.entity_rows.columns}
     merge_drop = []
-    alive = np.ones(len(order), dtype=bool)
-    alias = dict(spine_alias)
-    for s_i, ((name, src, asof), (vals, ts_out, found), (_i, _k, _a, outs)) in enumerate(zip(plan, joined, sets)):
+    alias = dict(q.spine_alias)
+    for s_i, (name, src, asof) in enumerate(q.plan):
         head = src.entities + ([src.timestamp_key] if src.timestamp_key else [])
         right = {}
-        if src.timestamp_key and not (asof and src.timestamp_key == entity_ts):
-            # as-of: cast to the entity column's unit (base.py:389-410); exact: the set's own unit
-            tdt = np.dtype(f"datetime64[{unit}]") if asof else src.frame[src.timestamp_key].dtype
-            right[src.timestamp_key] = np.where(ts_out == _NAT, _NAT, ts_out // _UNIT_NS[np.datetime_data(tdt)[0]]).view(tdt)
-        for (f, _a), v in zip(fields[name], vals):
-            missed = miss[s_i] > 0 if train else not found[alive].all()
-            right[f"{f}_{name}"] = _restore(v, src.features[f][1], found if asof else None, missed)
-        if not asof:
-            alive &= found
+        if src.timestamp_key and not (asof and src.timestamp_key == q.entity_ts):
+            right[src.timestamp_key] = ("ts", s_i)
+        for j, (f, _a) in enumerate(q.fields[name]):
+            right[f"{f}_{name}"] = ("out", s_i, j)
         for c, v in right.items():
             out_name = c
             if c in cols:
@@ -426,35 +467,148 @@ def get_offline_features(feature_vector, entity_rows=None, entity_timestamp_colu
                 if out_name not in merge_drop:
                     merge_drop.append(out_name)
             cols[out_name] = v
-        new = [(c, c) for c in head] if not drop_indexes else []
-        new += [(f"{f}_{name}", a or f) for f, a in fields[name]]
+        new = [(c, c) for c in head] if not q.drop_indexes else []
+        new += [(f"{f}_{name}", a or f) for f, a in q.fields[name]]
         alias.update(dict(new))
 
     # base.py:113-120, 253-254, 325-341: drop keys / timestamps unless with_indexes, rename to aliases
+    index_columns = list(q.index_columns)
     drop = []
-    for c in ([entity_ts] if drop_indexes and entity_ts else []):
+    for c in ([q.entity_ts] if q.drop_indexes and q.entity_ts else []):
         drop.append(c)
-    if entity_less and drop_indexes:
+    if q.entity_less and q.drop_indexes:
         drop += index_columns
-    for name, src, _asof in plan:
-        if drop_indexes and src.timestamp_key:
+    for name, src, _asof in q.plan:
+        if q.drop_indexes and src.timestamp_key:
             drop.append(src.timestamp_key)
         for k in src.entities:
             if k not in index_columns:
                 index_columns.append(k)
-            if drop_indexes:
+            if q.drop_indexes:
                 drop.append(k)
     drop += merge_drop
-    if not drop_indexes and ts_col and ts_col not in alias.values():
-        alias[ts_col] = ts_col
-    result = {}
+    if not q.drop_indexes and q.ts_col and q.ts_col not in alias.values():
+        alias[q.ts_col] = q.ts_col
+    result, names = [], set()
     for c, v in cols.items():
         new = alias.get(c, c)
         if new in drop:
             continue
-        if new in result:
+        if new in names:
             raise LoweringError(f"two columns of the training set are named {new!r}")
-        result[new] = v[alive] if not alive.all() else v
-    if drop_indexes or not all(k in result for k in index_columns):
+        result.append((new, v))
+        names.add(new)
+    if q.drop_indexes or not all(k in names for k in index_columns):
         index_columns = []
+    return result, index_columns
+
+
+def get_offline_features(feature_vector, entity_rows=None, entity_timestamp_column=None, target=None, run_config=None,
+                         drop_columns=None, start_time=None, end_time=None, with_indexes=False, update_stats=False, engine=None,
+                         engine_args=None, query=None, order_by=None, spark_service=None, timestamp_for_filtering=None,
+                         additional_filters=None):
+    """feature_store/api.py:99 on the local engine: the training frame of `feature_vector` for `entity_rows`, point-in-time
+    correct per feature set.  What the device does not run is refused with LoweringError (there is no pandas fallback)."""
+    q = _plan_query(feature_vector, entity_rows, entity_timestamp_column, target=target, run_config=run_config,
+                    drop_columns=drop_columns, start_time=start_time, end_time=end_time, with_indexes=with_indexes,
+                    update_stats=update_stats, engine=engine, engine_args=engine_args, query=query, order_by=order_by,
+                    spark_service=spark_service, timestamp_for_filtering=timestamp_for_filtering,
+                    additional_filters=additional_filters)
+    sets, arrays = q.sets, q.arrays
+    if not q.n:
+        order, joined, permuted, miss = (
+            np.zeros(0, np.int64), [([np.zeros(0, dt) for _w, dt, _m in s[3]], np.zeros(0, np.int64), np.zeros(0, bool)) for s in sets],
+            [a[:0] for a in arrays], np.zeros(len(sets), np.uint64))
+    elif q.train:
+        order, joined, permuted, miss = pit_train(q.ts_ns, sets, arrays, q.dev_label)
+    else:
+        order, joined, permuted, _miss = pit_join(q.ts_ns, sets, arrays)
+    moved = dict(zip(q.dev_cols, permuted))
+    layout, index_columns = _layout(q)
+
+    # the rows every exact-key set matched; per set, whether it missed a row of the merged frame at its place in the merge
+    alive = np.ones(len(order), dtype=bool)
+    missed = []
+    for s_i, ((_name, _src, asof), (_vals, _ts_out, found)) in enumerate(zip(q.plan, joined)):
+        missed.append(miss[s_i] > 0 if q.train else not found[alive].all())
+        if not asof:
+            alive &= found
+    result = {}
+    for new, source in layout:
+        if source[0] == "entity":
+            c = source[1]
+            if c in moved:
+                v = moved[c]
+                v = v.view(q.entity_rows[c].dtype) if v.dtype != q.entity_rows[c].dtype else v
+            else:  # strings, categories, objects: permuted on the host in the device's order
+                v = q.entity_rows[c].take(order).reset_index(drop=True).array
+        elif source[0] == "ts":
+            name, src, asof = q.plan[source[1]]
+            ts_out = joined[source[1]][1]
+            # as-of: cast to the entity column's unit (base.py:389-410); exact: the set's own unit
+            tdt = np.dtype(f"datetime64[{q.unit}]") if asof else src.frame[src.timestamp_key].dtype
+            v = np.where(ts_out == _NAT, _NAT, ts_out // _UNIT_NS[np.datetime_data(tdt)[0]]).view(tdt)
+        else:
+            s_i, j = source[1], source[2]
+            name, src, asof = q.plan[s_i]
+            vals, _ts_out, found = joined[s_i]
+            v = _restore(vals[j], src.features[q.fields[name][j][0]][1], found if asof else None, missed[s_i])
+        result[new] = v[alive] if not alive.all() else v
     return OfflineVectorResponse(result, index_columns)
+
+
+def _feat_kind(dtype):
+    """a device source's dtype -> (bytes, nat.PIT_FEAT_*) as the device holds it"""
+    dtype = np.dtype(dtype)
+    kind = {"f": nat.PIT_FEAT_FLOAT, "i": nat.PIT_FEAT_INT, "u": nat.PIT_FEAT_UINT, "b": nat.PIT_FEAT_BOOL}[dtype.kind]
+    return dtype.itemsize, kind
+
+
+def get_offline_tensors(feature_vector, entity_rows=None, entity_timestamp_column=None, dtype="float32", **options):
+    """the training set of `get_offline_features(feature_vector, entity_rows, entity_timestamp_column, **options)` left in
+    device memory: row i of `features`, `label` and `order` is row i of that call's `to_dataframe()`; the features are its
+    columns without the label, the entity frame's own columns, the keys and the timestamps, converted as
+    `to_numpy(dtype)` converts them (a missing value is NaN, bool 0 / 1).  Refuses what `get_offline_features` refuses,
+    with the same messages, and datetime features, which a matrix of numbers cannot hold."""
+    if np.dtype(dtype) not in (np.float32, np.float64):
+        raise ValueError(f"dtype {dtype!r}: the feature matrix is float32 or float64")
+    dtype = np.dtype(dtype)
+    q = _plan_query(feature_vector, entity_rows, entity_timestamp_column, **options)
+    layout, _index_columns = _layout(q)
+    label_source = None
+    if q.dev_label is not None:
+        s_i, j, _kind = q.dev_label
+        label_source = ("out", s_i, j) if s_i >= 0 else ("entity", q.dev_cols[j])
+    spine = set(q.spine_features)
+    picked = [(name, source) for name, source in layout if source != label_source and
+              (source[0] == "out" or (source[0] == "entity" and source[1] in spine))]
+
+    # each matrix column's source on the device: a set's output as the index stores it, or a spine column as the frame has it
+    used = [c for c in q.dev_cols if c in spine or (label_source is not None and ("entity", c) == label_source)]
+    arrays = [q.arrays[q.dev_cols.index(c)] for c in used]
+
+    def device_source(name, source, what):
+        if source[0] == "out":
+            s_i, j = source[1], source[2]
+            pname, src, _asof = q.plan[s_i]
+            stored = src.features[q.fields[pname][j][0]][1]
+            if stored.startswith("datetime64"):
+                raise LoweringError(f"{what} {name!r} is a {stored} column: a matrix of numbers has no place for it (drop it from "
+                                    "the vector)")
+            width, kind = _feat_kind(stored if stored in ("float32", "float64") else np.int32)
+            return (s_i, j, width, nat.PIT_FEAT_BOOL if stored == "bool" else kind)
+        col = q.entity_rows[source[1]]
+        if col.dtype.kind == "M":
+            raise LoweringError(f"{what} {name!r} is a {col.dtype} column: a matrix of numbers has no place for it (drop it from "
+                                "the vector)")
+        return (-1, used.index(source[1])) + _feat_kind(col.dtype)
+
+    feats = [device_source(name, source, "feature") for name, source in picked]
+    label_vec = None
+    if label_source is not None:
+        label_vec = device_source(f"{q.label[0]}.{q.label[1]}", label_source, "label")
+    dev_label = q.dev_label
+    if dev_label is not None and dev_label[0] < 0:
+        dev_label = (-1, used.index(label_source[1]), dev_label[2])
+    features, label, order, stats = pit_train_pack(q.ts_ns, q.sets, arrays, dev_label, feats, label_vec, dtype)
+    return TrainingTensors(features, label, order, [name for name, _s in picked], stats["kept"], stats)
