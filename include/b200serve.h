@@ -512,6 +512,12 @@ int b2s_darray_release(b2s_darray_t a);
 void* b2s_darray_dlpack(b2s_darray_t a, int32_t ndim, const int64_t* shape, int32_t code, int32_t bits);
 int b2s_dlpack_delete(void* managed);
 int64_t b2s_darray_live(void);
+/* b2s_darray_alloc: a new array of `bytes` (zero != 0: zeroed on the library stream).  b2s_darray_view: an array over
+ * bytes [offset, offset + bytes) of `base`, which it keeps alive; releasing the view drops that reference.  Both refuse a
+ * null out, negative sizes and (view) a range outside the base or an offset that is not a multiple of 8 with
+ * B2S_ERR_INVALID; the view's address is base + offset. */
+int b2s_darray_alloc(int64_t bytes, int32_t zero, b2s_darray_t* out);
+int b2s_darray_view(b2s_darray_t base, int64_t offset, int64_t bytes, b2s_darray_t* out);
 
 /* Training sets as device tensors: b2s_pit_train_host's join and kept rows, packed into one row-major matrix in HBM
  * instead of copied back.  Matrix column i is feats[i]: output `out` of set `set`, or with set -1 entity column `out`, a
@@ -592,6 +598,45 @@ int b2s_agg_run_host(const int64_t* keys, const int64_t* ts, int64_t n, const b2
 /* n_iters device runs on the library stream, CUDA-event timed: the sort alone and the whole run (ms summed over the runs) */
 int b2s_agg_time_device(const int64_t* d_keys, const int64_t* d_ts, int64_t n, const b2s_agg_spec* specs, int32_t n_specs,
                         uint64_t* d_counters, int32_t n_iters, float* sort_ms, float* total_ms);
+
+/* ---- feature-set ingest of device-resident columns -----------------------------------------------------------------
+ * What the host ingest does around b2s_cols_run_* and b2s_agg_run_* for columns that already live in device memory.
+ * b2s_stream: the library stream (NULL before b2s_init), for producers that order their writes before a consumer's
+ * stream (DLPack).  b2s_stream_wait: the library stream waits for the work queued so far on `producer` (a CUDA stream;
+ * 1 / 2 are the legacy / per-thread default streams).  b2s_pointer_device: the device that holds `p`, -1 for host memory. */
+void* b2s_stream(void);
+int b2s_stream_wait(void* producer);
+int b2s_pointer_device(const void* p, int32_t* device);
+/* b2s_cols_convert_device: n_ops elementwise conversions over n rows in ONE launch, asynchronous on `stream` (NULL: the
+ * library stream).  COPY4 / COPY8 and the widenings of 1- and 2-byte ints stage columns into the slot block
+ * b2s_cols_run_device reads (bool is U8); the others give result columns the host ingest's dtypes: int32 -> float64,
+ * float32 -> int32 (numpy's astype: out of range or NaN gives INT32_MIN), a date part (-1 for NaT) -> float64 with NaN,
+ * int32 -> bool (one byte, nonzero is 1).  CHECK_F32 writes nothing: d_counters[counter] (zeroed by the caller) counts
+ * the int32 values float32 cannot hold exactly.  B2S_ERR_INVALID before any launch for n < 0, n_ops outside
+ * 1 .. 65535, an unknown kind, a null (n > 0) or misaligned source or destination (aligned to its element width), or a
+ * CHECK_F32 counter outside [0, n_counters) or without d_counters. */
+enum {
+  B2S_CONV_COPY4 = 0, B2S_CONV_COPY8 = 1, B2S_CONV_I8_I32 = 2, B2S_CONV_U8_I32 = 3, B2S_CONV_I16_I32 = 4, B2S_CONV_U16_I32 = 5,
+  B2S_CONV_I32_F64 = 6, B2S_CONV_F32_I32 = 7, B2S_CONV_DATE_F64 = 8, B2S_CONV_I32_BOOL = 9, B2S_CONV_CHECK_F32 = 10
+};
+typedef struct b2s_convert {
+  const void* src;
+  void* dst;        /* unused by CHECK_F32 */
+  int32_t kind;     /* B2S_CONV_* */
+  int32_t counter;  /* CHECK_F32 only */
+} b2s_convert;
+int b2s_cols_convert_device(const b2s_convert* ops, int32_t n_ops, int64_t n, uint64_t* d_counters, int32_t n_counters,
+                            void* stream);
+/* b2s_keys_encode_device: 64-bit entity keys as the point-in-time join and the aggregations encode them, in one launch:
+ * one int column (1, 2 or 4 bytes signed or unsigned, 8 bytes signed) widened to int64, or two int32 columns as
+ * hi << 32 | (lo & 0xFFFFFFFF).  B2S_ERR_INVALID before any launch for other widths, null (n > 0) or misaligned columns,
+ * or d_keys not 8-byte aligned. */
+typedef struct b2s_key_col {
+  const void* src;
+  int32_t bytes;
+  int32_t is_signed;
+} b2s_key_col;
+int b2s_keys_encode_device(const b2s_key_col* cols, int32_t n_cols, int64_t n, int64_t* d_keys, void* stream);
 
 #ifdef __cplusplus
 }

@@ -97,6 +97,19 @@ class AggSpec(C.Structure):
     _fields_ = [("src", _vp), ("kind", _i32), ("ops", C.c_uint32), ("period_ns", _i64), ("n_windows", _i32),
                 ("windows_ns", C.POINTER(_i64)), ("outs", C.POINTER(_vp))]
 
+# B2S_CONV_* kinds of b2s_cols_convert_device
+CONV_COPY4, CONV_COPY8, CONV_I8_I32, CONV_U8_I32, CONV_I16_I32, CONV_U16_I32 = 0, 1, 2, 3, 4, 5
+CONV_I32_F64, CONV_F32_I32, CONV_DATE_F64, CONV_I32_BOOL, CONV_CHECK_F32 = 6, 7, 8, 9, 10
+
+
+class Convert(C.Structure):
+    _fields_ = [("src", _vp), ("dst", _vp), ("kind", _i32), ("counter", _i32)]
+
+
+class KeyCol(C.Structure):
+    _fields_ = [("src", _vp), ("bytes", _i32), ("is_signed", _i32)]
+
+
 # name -> (restype, argtypes); the single source of truth for the exported surface
 SIGNATURES = {
     "b2s_version": (C.c_int, []),
@@ -196,6 +209,14 @@ SIGNATURES = {
     "b2s_darray_dlpack": (_vp, [_vp, _i32, C.POINTER(_i64), _i32, _i32]),
     "b2s_dlpack_delete": (C.c_int, [_vp]),
     "b2s_darray_live": (_i64, []),
+    "b2s_darray_alloc": (C.c_int, [_i64, _i32, C.POINTER(_vp)]),
+    "b2s_darray_view": (C.c_int, [_vp, _i64, _i64, C.POINTER(_vp)]),
+    # feature-set ingest of device-resident columns
+    "b2s_stream": (_vp, []),
+    "b2s_stream_wait": (C.c_int, [_vp]),
+    "b2s_pointer_device": (C.c_int, [_vp, _pi32]),
+    "b2s_cols_convert_device": (C.c_int, [C.POINTER(Convert), _i32, _i64, _vp, _i32, _vp]),
+    "b2s_keys_encode_device": (C.c_int, [C.POINTER(KeyCol), _i32, _i64, _vp, _vp]),
     # windowed aggregations
     "b2s_agg_run_device": (C.c_int, [_vp, _vp, _i64, C.POINTER(AggSpec), _i32, _vp, _vp]),
     "b2s_agg_run_host": (C.c_int, [_vp, _vp, _i64, C.POINTER(AggSpec), _i32, _vp, C.POINTER(Stats)]),
@@ -410,8 +431,8 @@ class PinnedPool:
 PINNED = PinnedPool()
 
 
-# DLPack data type codes of the typestrs a DeviceArray can have
-_DLPACK_CODES = {"f": 2, "i": 0, "u": 1, "b": 6}
+# DLPack data type codes of the typestrs a DeviceArray can have (datetime64[ns] goes out as int64)
+_DLPACK_CODES = {"f": 2, "i": 0, "u": 1, "b": 6, "M": 0}
 _DLTENSOR = b"dltensor"
 _pyapi = C.PyDLL(None)  # own function objects: other modules retype the ones ctypes.pythonapi shares
 _capsule_new = _pyapi.PyCapsule_New
@@ -483,6 +504,26 @@ class DeviceArray:
             self.release()
         except Exception:
             pass
+
+
+def darray_alloc(nbytes, zero=False):
+    """a new library-owned device array of `nbytes` bytes (zeroed on the library stream with zero=True) -> its handle"""
+    h = C.c_void_p()
+    check(init().b2s_darray_alloc(int(nbytes), int(bool(zero)), C.byref(h)))
+    return h.value
+
+
+def darray_view(base, offset, shape, dtype):
+    """DeviceArray over bytes [offset, ...) of the array `base` (a handle), which it keeps alive"""
+    h = C.c_void_p()
+    nbytes = int(np.prod(shape)) * np.dtype(dtype).itemsize
+    check(load().b2s_darray_view(base, int(offset), nbytes, C.byref(h)))
+    return DeviceArray(h.value, shape, dtype)
+
+
+def library_device():
+    """the device ordinal the library runs on: the one b2s_init took, or the one init() would take"""
+    return _device_ordinal() if _inited else int(os.environ.get("LOCAL_RANK", "0"))
 
 
 def _device_ordinal():

@@ -886,6 +886,7 @@ struct b2s_darray_s {
   void* ptr;
   int64_t bytes;
   std::atomic<int> refs{1};
+  b2s_darray_s* base = nullptr;  // a view holds one reference on the array that owns its memory
 };
 
 namespace {
@@ -906,7 +907,8 @@ int darray_new(b2s_darray_t& a, int64_t bytes) {
 
 void darray_unref(b2s_darray_t a) {
   if (a && a->refs.fetch_sub(1) == 1) {
-    cudaFree(a->ptr);
+    if (a->base) darray_unref(a->base);
+    else cudaFree(a->ptr);
     delete a;
     --g_darrays;
   }
@@ -1130,6 +1132,48 @@ extern "C" int b2s_dlpack_delete(void* managed) {
 }
 
 extern "C" int64_t b2s_darray_live(void) { return g_darrays.load(); }
+
+extern "C" int b2s_darray_alloc(int64_t bytes, int32_t zero, b2s_darray_t* out) {
+  try {  // no C++ exception crosses the C boundary
+    if (!out || bytes < 0) return b2s_int_fail(B2S_ERR_INVALID, "null out or negative size");
+    *out = nullptr;
+    if (!b2s_int_inited()) return b2s_int_fail(B2S_ERR_STATE, "b2s_init was not called (no CUDA device: there is no CPU fallback)");
+    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
+    b2s_darray_t a = nullptr;
+    if (int rc = darray_new(a, bytes)) return rc;
+    if (zero && bytes) {
+      const cudaError_t e = cudaMemsetAsync(a->ptr, 0, (size_t)bytes, b2s_int_stream());
+      if (e != cudaSuccess) {
+        darray_unref(a);
+        return b2s_int_fail(B2S_ERR_CUDA, "cudaMemsetAsync failed: %s", cudaGetErrorString(e));
+      }
+    }
+    *out = a;
+    return B2S_OK;
+  } catch (const std::exception& e) {
+    return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
+  }
+}
+
+extern "C" int b2s_darray_view(b2s_darray_t base, int64_t offset, int64_t bytes, b2s_darray_t* out) {
+  try {  // no C++ exception crosses the C boundary
+    if (!out) return b2s_int_fail(B2S_ERR_INVALID, "null out");
+    *out = nullptr;
+    if (!base || offset < 0 || bytes < 0 || offset % 8 || offset > base->bytes || bytes > base->bytes - offset)
+      return b2s_int_fail(B2S_ERR_INVALID, "view [%lld, +%lld) of a %lld-byte array: outside it, or not 8-byte aligned", (long long)offset,
+                          (long long)bytes, base ? (long long)base->bytes : 0ll);
+    b2s_darray_t v = new b2s_darray_s();
+    v->ptr = static_cast<char*>(base->ptr) + offset;
+    v->bytes = bytes;
+    v->base = base;
+    base->refs.fetch_add(1);
+    ++g_darrays;
+    *out = v;
+    return B2S_OK;
+  } catch (const std::exception& e) {
+    return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
+  }
+}
 
 extern "C" int b2s_pit_train_pack(const int64_t* ts, int64_t n, const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols,
                                   int32_t n_cols, const b2s_pit_label* label, const b2s_pit_feat* feats, int32_t n_feats,

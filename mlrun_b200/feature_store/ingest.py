@@ -481,6 +481,129 @@ class IngestPlan:
         data, _bufs, block, _layout = self._run_arrays(ins, n or 0, reference_dtypes, keys)
         return columnar.ColumnBatch(data, n or 0, block)
 
+    def run_device(self, cols, key_cols=None):
+        """device twin of `run_columns`: `cols` maps every schema column to an acquired `columnar.DeviceColumn` (timestamps
+        as 8-byte columns); `key_cols` are the entity key columns a plan with an aggregation needs.  Returns a
+        `columnar.DeviceColumnBatch` whose columns are the host path's, dtype for dtype and bit for bit, and never leave
+        HBM: the columns are staged into one slot block (one convert launch, which also counts int32 map sources float32
+        would round), keys are encoded on the device, the columns plan and the aggregation run there, and the counters come
+        back in one small copy before one more convert launch gives the result columns their dtypes."""
+        from . import columnar
+
+        n = None
+        for name, kind in self.schema:
+            if name not in cols:
+                raise ValueError(f"column {name!r} of the plan's schema is missing")
+            c = cols[name]
+            want = {F32: ("float32",), I32: _INT_DTYPES, I64: ("datetime64[ns]", "int64")}[kind]
+            if str(c.dtype) not in want:
+                raise ValueError(f"column {name!r}: expected a 1-D {' / '.join(want)} array, got {c.dtype} ({c.n},)")
+            if n is None:
+                n = c.n
+            elif c.n != n:
+                raise ValueError("columns of different lengths")
+        n = n or 0
+        if self.agg is not None and (key_cols is None or any(k.n != n for k in key_cols)):
+            raise ValueError("a plan with an aggregation needs the encoded entity key of every row")
+        lib = nat.init()
+        before = nat.launch_count()
+        stride = max(256, (n * 4 + 255) // 256 * 256)
+        n_cnt = self.plan.n_counters
+        counters = nat.DeviceArray(nat.darray_alloc(8 * (n_cnt + 3 + len(self.rounding_maps)), zero=True),
+                                   (n_cnt + 3 + len(self.rounding_maps),), np.uint64)
+        stage = nat.DeviceArray(nat.darray_alloc(stride * self.plan.n_in), (stride * self.plan.n_in,), np.uint8)
+        widen = {"float32": nat.CONV_COPY4, "int32": nat.CONV_COPY4, "int8": nat.CONV_I8_I32, "uint8": nat.CONV_U8_I32,
+                 "bool": nat.CONV_U8_I32, "int16": nat.CONV_I16_I32, "uint16": nat.CONV_U16_I32, "int64": nat.CONV_COPY8,
+                 "datetime64[ns]": nat.CONV_COPY8}
+        ops = [nat.Convert(cols[name].ptr, stage.ptr + self.prog.in_slot[name] * stride, widen[str(cols[name].dtype)], 0)
+               for name, _kind in self.schema]
+        source_of = {self.prog.in_slot[name]: cols[name] for name, _kind in self.schema}
+        for j, (slot, _name) in enumerate(self.rounding_maps):
+            if str(source_of[slot].dtype) == "int32":  # narrower ints all fit float32
+                ops.append(nat.Convert(source_of[slot].ptr, None, nat.CONV_CHECK_F32, n_cnt + 3 + j))
+        staged = sum(c.n * c.dtype.itemsize for c in cols.values())
+        _convert(lib, ops, n, counters)
+        keys = None
+        if self.agg is not None:
+            keys = nat.DeviceArray(nat.darray_alloc(8 * n), (n,), np.int64)
+            kc = (nat.KeyCol * len(key_cols))(*[nat.KeyCol(k.ptr, k.dtype.itemsize, int(k.dtype.kind == "i")) for k in key_cols])
+            nat.check(lib.b2s_keys_encode_device(kc, len(key_cols), n, keys.ptr, None))
+        specs, _extra = self._landing()
+        agg_names = self.agg.out_names if self.agg is not None else []
+        col_bytes = (n * 8 + 255) // 256 * 256
+        block = nat.darray_alloc(stride * self.plan.n_out + col_bytes * len(agg_names))
+        try:
+            base = C.c_void_p()
+            nat.check(lib.b2s_darray_info(block, C.byref(base), None))
+            base = base.value
+            self.plan.run_device(stage.ptr, stride, n, base, stride, counters.ptr)
+            agg_at = {name: stride * self.plan.n_out + j * col_bytes for j, name in enumerate(agg_names)}
+            if self.agg is not None:
+                slot_of = {name: slot for name, slot, _dt in specs}
+                self.agg.run_device(keys.ptr, stage.ptr + self.agg.ts_slot * stride, n,
+                                    {c: base + slot_of[c] * stride for c in self.agg.sources},
+                                    {name: base + at for name, at in agg_at.items()}, counters.ptr + 8 * n_cnt)
+            got = counters.numpy()  # the one copy back: waits for every launch above
+            self.counters = got[:n_cnt]
+            for j, (_slot, name) in enumerate(self.rounding_maps):
+                if got[n_cnt + 3 + j]:
+                    raise LoweringError(
+                        f"MapValues {name!r}: its values are not all int32 integers, so it writes float32, and the int32 source "
+                        "holds values float32 cannot represent (beyond 2^24): they would be rounded where they pass through. "
+                        "Map to integers, or cast the column to float32 explicitly")
+            if self.agg is not None:
+                self.agg.counters = got[n_cnt: n_cnt + 3]
+                self.agg.check_counters()
+            data, convs, conv_at, conv_bytes = {}, [], {}, 0
+            dt_of = {name: dt for name, _slot, dt in specs}
+            slot_of = {name: slot for name, slot, _dt in specs}
+            for name, _slot, how in self.out:
+                kind, to = None, None
+                if isinstance(how, tuple) and how[0] == "map":
+                    if how[3] and not how[2]:
+                        kind, to = nat.CONV_I32_F64, np.float64
+                    elif not how[3] and how[2] and self.counters[how[1]] == 0:
+                        kind, to = nat.CONV_F32_I32, np.int32
+                elif isinstance(how, tuple) and how[0] == "date":
+                    if self.counters[how[1]]:
+                        kind, to = nat.CONV_DATE_F64, np.float64
+                    elif how[2]:
+                        kind, to = nat.CONV_I32_BOOL, np.bool_
+                if kind is not None:
+                    conv_at[name] = (conv_bytes, kind, np.dtype(to))
+                    conv_bytes += (n * np.dtype(to).itemsize + 255) // 256 * 256
+            conv_block = nat.darray_alloc(conv_bytes) if conv_at else None
+            try:
+                for name, _slot, how in self.out:
+                    if name in conv_at:
+                        at, kind, to = conv_at[name]
+                        data[name] = nat.darray_view(conv_block, at, (n,), to)
+                        convs.append(nat.Convert(base + slot_of[name] * stride, data[name].ptr, kind, 0))
+                    else:
+                        data[name] = nat.darray_view(block, slot_of[name] * stride, (n,),
+                                                     "datetime64[ns]" if how == "dt" else dt_of[name])
+                for name in agg_names:
+                    data[name] = nat.darray_view(block, agg_at[name], (n,), np.float64)
+                if convs:
+                    _convert(lib, convs, n, counters)
+                    nat.check(lib.b2s_device_sync())
+            finally:
+                if conv_block:
+                    lib.b2s_darray_release(conv_block)
+        finally:
+            lib.b2s_darray_release(block)  # the views hold the block from here on
+        self.violations = {name: int(self.counters[cnt]) for cnt, name, _v in self.checks}
+        self.unmatched = {name: int(self.counters[cnt]) for cnt, name, _w in self.miss if self.counters[cnt]}
+        for cnt, name, v in self.checks:
+            if self.counters[cnt]:
+                print(f"{v.severity}! {name} has {int(self.counters[cnt])} values outside [{v.min}, {v.max}]")
+        for step in self.prog.validators:
+            step.violations = getattr(step, "violations", 0) + sum(
+                int(self.counters[cnt]) for cnt, name, v in self.checks if v in step._validators.values())
+        converted = sum(n * to.itemsize for _at, _k, to in conv_at.values())
+        self.stats = {"rows": n, "kernels": nat.launch_count() - before, "staged_bytes": staged, "converted_bytes": converted}
+        return columnar.DeviceColumnBatch(data, n)
+
     def _assemble(self, data, bufs, block, layout, n, index):
         """the result frame.  Columns that stayed in their landing buffers and sit next to each other in the result block
         with one dtype become ONE 2-D pandas block (a strided view of the block, no copy): the frame has a handful of blocks
@@ -651,6 +774,24 @@ class AggregationPlan:
         Raises LoweringError after the run for late events, NaT timestamps or NaN values."""
         specs = [(sources[sp.column], sp.kind, sp.ops, sp.period_ns, sp.windows_ns, [outs[o] for o in sp.outs]) for sp in self.specs]
         self.counters, self.stats = aggregate_host(keys, ts, specs, n)
+        self.check_counters()
+
+    def run_device(self, d_keys, d_ts, n, d_sources, d_outs, d_counters):
+        """one b2s_agg_run_device call over device addresses: sources {column: address}, outs {aggregate column: address of
+        float64 [n]}; the three counters accumulate at d_counters (zeroed) for the caller to read and `check_counters`"""
+        c_specs = (nat.AggSpec * len(self.specs))()
+        keep = []
+        for i, sp in enumerate(self.specs):
+            win = np.ascontiguousarray(sp.windows_ns, dtype=np.int64)
+            ptrs = (C.c_void_p * len(sp.outs))(*[d_outs[o] for o in sp.outs])
+            keep += [win, ptrs]
+            c_specs[i] = nat.AggSpec(d_sources[sp.column], sp.kind, sp.ops, sp.period_ns, len(win),
+                                     win.ctypes.data_as(C.POINTER(C.c_int64)), ptrs)
+        before = nat.launch_count()
+        nat.check(nat.load().b2s_agg_run_device(d_keys, d_ts, n, c_specs, len(self.specs), d_counters, None))
+        self.stats = {"rows": n, "kernels": nat.launch_count() - before}
+
+    def check_counters(self):
         late, nat_rows, nans = (int(c) for c in self.counters)
         if late:
             raise LoweringError(f"{late} rows have a timestamp below the previous row of their key: late and out-of-order events "
@@ -659,6 +800,12 @@ class AggregationPlan:
             raise LoweringError(f"{nat_rows} rows have a NaT timestamp: they belong to no window")
         if nans:
             raise LoweringError(f"{nans} aggregated values are NaN: impute them before the aggregation")
+
+
+def _convert(lib, ops, n, counters):
+    """one b2s_cols_convert_device launch on the library stream"""
+    arr = (nat.Convert * len(ops))(*ops)
+    nat.check(lib.b2s_cols_convert_device(arr, len(ops), n, counters.ptr, counters.shape[0], None))
 
 
 def aggregate_host(keys, ts, specs, n):
@@ -908,6 +1055,9 @@ class FeatureSet:
             raise LoweringError("targets are storage (out of scope): ingest returns the frame")
         from . import columnar
 
+        if columnar.is_columnar(source) and columnar.is_device_source(source):
+            batch = self._ingest_device(source, namespace, reference_dtypes)
+            return batch if return_df else None
         if columnar.is_columnar(source):
             # columnar sources (dict of arrays, Arrow table / record batch, DLPack producers): no DataFrame on either side;
             # entity columns are carried through untouched (they would be the frame's index)
@@ -945,6 +1095,68 @@ class FeatureSet:
         enc = self._encoded_keys(key_frame) if self._plan.agg is not None else None
         out = self._plan.run(df, reference_dtypes=reference_dtypes, keys=enc)
         return out if return_df else None
+
+    def _ingest_device(self, source, namespace, reference_dtypes):
+        """CUDA columns -> DeviceColumnBatch: the columnar path with the data kept in HBM.  Everything refused is refused
+        before any copy or launch."""
+        from . import columnar
+
+        if reference_dtypes:
+            raise LoweringError("reference_dtypes=True widens integer results to int64, which no offline step takes: CUDA "
+                                "columns are ingested with the device dtypes")
+        cols = columnar.device_columns(source)
+        keys = [e.name for e in self.entities if e.name in cols]
+        carried = {k: cols.pop(k) for k in keys}
+        ts_names = {self.timestamp_key} if self.timestamp_key else set()
+        if any(str(c.dtype) == "int64" and k not in ts_names for k, c in cols.items()):
+            for step in self._graph.steps.values():  # DateExtractor's timestamp_col, read off the graph as validate_steps does
+                obj = getattr(step, "_object", None)
+                cls = type(obj).__name__ if obj is not None else str(step.class_name or "").rsplit(".", 1)[-1]
+                if cls == "DateExtractor":
+                    col = getattr(obj, "timestamp_col", None) if obj is not None else (step.class_args or {}).get("timestamp_col")
+                    ts_names.add(col or "timestamp")
+        schema, dtypes = columnar.device_schema(cols, ts_names)
+        for k, c in cols.items():
+            c.dtype = dtypes[k]
+        agg_key = _aggregation_key(self._graph)
+        key_cols = None
+        if agg_key != "[]" and self.entities:  # an aggregation step by name: its keys are refused before the plan is lowered
+            key_cols = self._device_key_columns(carried)
+        key = ("columns", schema, agg_key)
+        if self._plan is None or not isinstance(self._plan_key[0], str) or self._plan_key != key:
+            self.validate_steps(namespace)
+            self._plan = self._lower(namespace, schema)
+            self._plan_key = key
+        if self._plan.agg is None:
+            key_cols = None
+        elif key_cols is None:  # the plan aggregates (whatever the step is called): the host path's check, at its place
+            key_cols = self._device_key_columns(carried)
+        held = list(cols.values()) + (key_cols or [])
+        try:
+            for c in held:
+                c.acquire()
+            batch = self._plan.run_device(cols, key_cols)
+        finally:
+            for c in held:
+                c.release()
+        batch.index = {k: c.obj for k, c in carried.items()}
+        return batch
+
+    def _device_key_columns(self, carried):
+        """the entity key columns of CUDA columns, refused as `_encoded_keys` refuses them, and string keys (no string column
+        lives on the device)"""
+        from .keys import _key_kind
+
+        names = [e.name for e in self.entities]
+        if not names or not all(k in carried for k in names):
+            raise LoweringError(f"the aggregation's entity columns {names} must all be in the ingested data")
+        what = f"feature set {self.name}"
+        for k in names:
+            if carried[k].dtype.kind in "OSU":
+                raise LoweringError(f"{what}: key {k!r} of dtype {carried[k].dtype} is a string key: there are no string "
+                                    "columns on the device (hash them on the host)")
+        _key_kind({k: np.empty(0, carried[k].dtype) for k in names}, names, what)
+        return [carried[k] for k in names]
 
     @property
     def plan(self):
