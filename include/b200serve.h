@@ -434,10 +434,16 @@ int b2s_hash_strings(const char* bytes, const int64_t* offsets, int64_t n, int64
  * timestamp is <= the entity row's (backward, exact matches allowed, no tolerance), NaN / NaT where there is none.
  * A b2s_pit index holds one feature set in HBM: its rows sorted by (64-bit key, int64 nanosecond timestamp), equal
  * pairs in input order, the feature columns as rows of 4-byte words, and each key's run in an open-addressing slot
- * array.  Built once from host columns (each 4 or 8 bytes wide; column c takes words [sum of earlier widths / 4, ...)). */
+ * array.  Built once from columns (each 4 or 8 bytes wide; column c takes words [sum of earlier widths / 4, ...)):
+ * host arrays for b2s_pit_index_create, which uploads them, or memory of the library's device for
+ * b2s_pit_index_create_device, which reads them where they are.  Both refuse n_rows <= 0 (and >= 2^31), more than 64
+ * columns and widths other than 4 / 8 with B2S_ERR_INVALID; _device also refuses, before any launch, keys, timestamps
+ * (8 bytes) or columns (their width) that are misaligned or not on the library's device.  The build makes 53 launches. */
 typedef struct b2s_pit_s* b2s_pit_t;
 int b2s_pit_index_create(const int64_t* keys, const int64_t* ts_ns, int64_t n_rows, const void* const* cols,
                          const int32_t* col_bytes, int32_t n_cols, b2s_pit_t* out);
+int b2s_pit_index_create_device(const int64_t* d_keys, const int64_t* d_ts, int64_t n_rows, const void* const* d_cols,
+                                const int32_t* col_bytes, int32_t n_cols, b2s_pit_t* out);
 int b2s_pit_index_destroy(b2s_pit_t index);
 /* longest_run 1: every key has one row, so the index can also serve exact-key joins */
 int b2s_pit_index_info(b2s_pit_t index, int64_t* n_rows, int64_t* n_keys, int64_t* longest_run, int32_t* row_words,
@@ -550,6 +556,13 @@ int b2s_pit_train_pack(const int64_t* ts, int64_t n, const b2s_pit_set* sets, in
                        int32_t n_cols, const b2s_pit_label* label, const b2s_pit_feat* feats, int32_t n_feats,
                        const b2s_pit_feat* label_vec, int32_t x_bytes, b2s_pit_tensors* out, float* phase_ms,
                        b2s_stats* stats);
+/* b2s_pit_train_pack with ts, each set's keys and each entity column's src in memory of the library's device: nothing is
+ * uploaded (stats->h2d_ms is 0), the launches are the same.  Also B2S_ERR_INVALID, before any launch, for such an input
+ * (n > 0) that is misaligned or not on the library's device. */
+int b2s_pit_train_pack_device(const int64_t* d_ts, int64_t n, const b2s_pit_set* sets, int32_t n_sets, const b2s_pit_col* cols,
+                              int32_t n_cols, const b2s_pit_label* label, const b2s_pit_feat* feats, int32_t n_feats,
+                              const b2s_pit_feat* label_vec, int32_t x_bytes, b2s_pit_tensors* out, float* phase_ms,
+                              b2s_stats* stats);
 
 /* ---- windowed aggregations at feature-set ingest ------------------------------------------------------------------
  * storey.AggregateByKey as FeatureSet.add_aggregation places it in a feature set's graph (feature_store/feature_set.py:
@@ -637,6 +650,11 @@ typedef struct b2s_key_col {
   int32_t is_signed;
 } b2s_key_col;
 int b2s_keys_encode_device(const b2s_key_col* cols, int32_t n_cols, int64_t n, int64_t* d_keys, void* stream);
+/* b2s_ts_profile_device: one launch over n int64 nanosecond timestamps in memory of the library's device; counts (host,
+ * 4) gets the NaT (INT64_MIN) values and the other values that are not whole multiples of 10^3, 10^6 and 10^9, in one
+ * small copy: the call returns when they are there.  n = 0: zeros, no launch.  B2S_ERR_INVALID before any launch for
+ * n < 0, a null counts, or d_ts null (n > 0), misaligned or not on the library's device. */
+int b2s_ts_profile_device(const int64_t* d_ts, int64_t n, int64_t* counts, void* stream);
 
 #ifdef __cplusplus
 }

@@ -192,6 +192,7 @@ SIGNATURES = {
     "b2s_hash_strings": (C.c_int, [C.c_char_p, C.POINTER(_i64), _i64, C.POINTER(_i64)]),
     # point-in-time (as-of) joins
     "b2s_pit_index_create": (C.c_int, [_vp, _vp, _i64, C.POINTER(_vp), _pi32, _i32, C.POINTER(_vp)]),
+    "b2s_pit_index_create_device": (C.c_int, [_vp, _vp, _i64, C.POINTER(_vp), _pi32, _i32, C.POINTER(_vp)]),
     "b2s_pit_index_destroy": (C.c_int, [_vp]),
     "b2s_pit_index_info": (C.c_int, [_vp, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_i64), _pi32, C.POINTER(_i64)]),
     "b2s_pit_join_device": (C.c_int, [_vp, _i64, C.POINTER(PitSet), _i32, C.POINTER(PitCol), _i32, _vp, _vp, _vp]),
@@ -203,6 +204,9 @@ SIGNATURES = {
     "b2s_pit_train_pack": (C.c_int, [_vp, _i64, C.POINTER(PitSet), _i32, C.POINTER(PitCol), _i32, C.POINTER(PitLabel),
                                      C.POINTER(PitFeat), _i32, C.POINTER(PitFeat), _i32, C.POINTER(PitTensors), _pf32,
                                      C.POINTER(Stats)]),
+    "b2s_pit_train_pack_device": (C.c_int, [_vp, _i64, C.POINTER(PitSet), _i32, C.POINTER(PitCol), _i32, C.POINTER(PitLabel),
+                                            C.POINTER(PitFeat), _i32, C.POINTER(PitFeat), _i32, C.POINTER(PitTensors), _pf32,
+                                            C.POINTER(Stats)]),
     # device arrays handed to the caller
     "b2s_darray_info": (C.c_int, [_vp, C.POINTER(_vp), C.POINTER(_i64)]),
     "b2s_darray_release": (C.c_int, [_vp]),
@@ -217,6 +221,7 @@ SIGNATURES = {
     "b2s_pointer_device": (C.c_int, [_vp, _pi32]),
     "b2s_cols_convert_device": (C.c_int, [C.POINTER(Convert), _i32, _i64, _vp, _i32, _vp]),
     "b2s_keys_encode_device": (C.c_int, [C.POINTER(KeyCol), _i32, _i64, _vp, _vp]),
+    "b2s_ts_profile_device": (C.c_int, [_vp, _i64, C.POINTER(_i64), _vp]),
     # windowed aggregations
     "b2s_agg_run_device": (C.c_int, [_vp, _vp, _i64, C.POINTER(AggSpec), _i32, _vp, _vp]),
     "b2s_agg_run_host": (C.c_int, [_vp, _vp, _i64, C.POINTER(AggSpec), _i32, _vp, C.POINTER(Stats)]),

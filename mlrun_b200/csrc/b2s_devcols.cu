@@ -1,7 +1,8 @@
 // b2s_devcols.cu -- device-resident feature-set ingest: what the host path does around the columns and aggregation kernels,
 // done on the device for columns that already live in HBM.  convert_kernel stages the caller's columns into the slot block
 // b2s_cols_run_device reads (copies, and widening of 1- and 2-byte ints), counts int32 values a float32 map output would
-// round, and gives result columns the dtypes the host path gives them; keys_kernel encodes entity keys as keys.py does.
+// round, and gives result columns the dtypes the host path gives them; keys_kernel encodes entity keys as keys.py does;
+// ts_profile_kernel counts what registration and the as-of join ask of a timestamp column (NaT, and its coarsest unit).
 #include <cuda_runtime.h>
 
 #include <cmath>
@@ -80,6 +81,27 @@ __global__ void __launch_bounds__(kThreads) keys_kernel(KeyCol hi, KeyCol lo, in
   for (int64_t i = (int64_t)blockIdx.x * kThreads + threadIdx.x; i < n; i += (int64_t)gridDim.x * kThreads) {
     const int64_t h = key_word(hi, i);
     keys[i] = pair ? (int64_t)(((uint64_t)h << 32) | ((uint64_t)key_word(lo, i) & 0xFFFFFFFFull)) : h;
+  }
+}
+
+// counts[0]: NaT (INT64_MIN) values; counts[1..3]: the other values that are not whole multiples of 10^3, 10^6, 10^9 ns.
+// A zero remainder means the same in C (truncated) and numpy (floored) division, so negative timestamps count alike.
+__global__ void __launch_bounds__(kThreads) ts_profile_kernel(const int64_t* __restrict__ ts, int64_t n, unsigned long long* __restrict__ counts) {
+  unsigned long long c[4] = {0, 0, 0, 0};
+  for (int64_t i = (int64_t)blockIdx.x * kThreads + threadIdx.x; i < n; i += (int64_t)gridDim.x * kThreads) {
+    const int64_t t = ts[i];
+    if (t == INT64_MIN) {
+      ++c[0];
+    } else {
+      c[1] += t % 1000ll != 0;
+      c[2] += t % 1000000ll != 0;
+      c[3] += t % 1000000000ll != 0;
+    }
+  }
+  for (int k = 0; k < 4; ++k) {
+    unsigned long long v = c[k];
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if ((threadIdx.x & 31) == 0 && v) atomicAdd(counts + k, v);
   }
 }
 
@@ -202,6 +224,37 @@ extern "C" int b2s_keys_encode_device(const b2s_key_col* cols, int32_t n_cols, i
     launches.add(1);
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return b2s_int_fail(B2S_ERR_CUDA, "keys launch failed: %s", cudaGetErrorString(e));
+    return B2S_OK;
+  } catch (const std::exception& e) {
+    return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
+  }
+}
+
+extern "C" int b2s_ts_profile_device(const int64_t* d_ts, int64_t n, int64_t* counts, void* stream) {
+  try {  // no C++ exception crosses the C boundary
+    if (n < 0 || !counts || (n && !d_ts)) return b2s_int_fail(B2S_ERR_INVALID, "n >= 0, non-null counts and (n > 0) timestamps");
+    if (misaligned(d_ts, 8)) return b2s_int_fail(B2S_ERR_INVALID, "d_ts must be 8-byte aligned");
+    for (int k = 0; k < 4; ++k) counts[k] = 0;
+    if (n == 0) return B2S_OK;
+    if (int rc = device_ready()) return rc;
+    int32_t dev = -1;
+    if (int rc = b2s_pointer_device(d_ts, &dev)) return rc;
+    if (dev != b2s_int_device()) return b2s_int_fail(B2S_ERR_INVALID, "d_ts is not memory of the library's device %d", b2s_int_device());
+    cudaStream_t st = stream ? (cudaStream_t)stream : b2s_int_stream();
+    Launches launches;
+    SyncOnExit done{st};
+    DeviceBlock blk(st);
+    unsigned long long* d_counts = nullptr;
+    blk.scratch(d_counts, 32);
+    if (int rc = blk.alloc()) return rc;
+    B2S_CUDA_TRY(cudaMemsetAsync(d_counts, 0, 32, st));
+    const int gx = (int)std::max<int64_t>(1, std::min<int64_t>((n + kThreads - 1) / kThreads, (int64_t)b2s_int_sm_count() * 8));
+    ts_profile_kernel<<<gx, kThreads, 0, st>>>(d_ts, n, d_counts);
+    launches.add(1);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return b2s_int_fail(B2S_ERR_CUDA, "ts profile launch failed: %s", cudaGetErrorString(e));
+    B2S_CUDA_TRY(cudaMemcpyAsync(counts, d_counts, 32, cudaMemcpyDeviceToHost, st));
+    B2S_CUDA_TRY(cudaStreamSynchronize(st));
     return B2S_OK;
   } catch (const std::exception& e) {
     return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());

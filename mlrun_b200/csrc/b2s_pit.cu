@@ -174,31 +174,27 @@ extern "C" int b2s_pit_index_destroy(b2s_pit_t ix) {
   }
 }
 
-static int index_build(b2s_pit_s* ix, const int64_t* keys, const int64_t* ts, int64_t n, const void* const* cols,
+// Builds the index from device arrays of n rows: keys, timestamps and the feature columns (4 or 8 bytes wide).  Both
+// entry points end here; the host one stages its arrays first.
+static int index_build(b2s_pit_s* ix, const int64_t* d_keys, const int64_t* d_ts_in, int64_t n, const void* const* d_cols,
                        const int32_t* col_bytes, int32_t n_cols, cudaStream_t st) {
   LayoutParams lp{};
   lp.n_cols = n_cols;
   for (int c = 0; c < n_cols; ++c) {
+    lp.cols[c] = d_cols[c];
     lp.words[c] = col_bytes[c] / 4;
     lp.row_words += lp.words[c];
   }
   ix->row_words = lp.row_words;
-  // the temporaries in one block: keys and timestamps in input order, the columns, the counters
   SyncOnExit done{st};
   DeviceBlock blk(st);
-  const int64_t* d_keys = nullptr;
-  const int64_t* d_ts_in = nullptr;
   unsigned long long* d_stat = nullptr;  // [0] runs, [1] longest run
-  blk.input(d_keys, keys, (size_t)n * 8);
-  blk.input(d_ts_in, ts, (size_t)n * 8);
   blk.scratch(d_stat, 16);
-  for (int c = 0; c < n_cols; ++c) blk.input(lp.cols[c], cols[c], (size_t)n * col_bytes[c]);
   SortBufs sb(st);
   if (int rc = sb.alloc(n)) return rc;
   if (int rc = blk.alloc()) return rc;
   B2S_CUDA_TRY(cudaMemsetAsync(d_stat, 0, 16, st));
-  if (int rc = blk.upload()) return rc;
-  B2S_CUDA_TRY(cudaMemcpyAsync(sb.k[0], ts, n * 8, cudaMemcpyHostToDevice, st));
+  B2S_CUDA_TRY(cudaMemcpyAsync(sb.k[0], d_ts_in, n * 8, cudaMemcpyDeviceToDevice, st));
   // by timestamp, then (stably) by key: rows ordered by (key, timestamp), equal pairs in input order
   Launches launches;
   if (int rc = radix_sort(sb, false, n, launches)) return rc;
@@ -231,23 +227,77 @@ static int index_build(b2s_pit_s* ix, const int64_t* keys, const int64_t* ts, in
   return B2S_OK;
 }
 
+// the host entry's first step: keys, timestamps and columns uploaded into one block, then the shared build
+static int index_build_host(b2s_pit_s* ix, const int64_t* keys, const int64_t* ts, int64_t n, const void* const* cols,
+                            const int32_t* col_bytes, int32_t n_cols, cudaStream_t st) {
+  SyncOnExit done{st};
+  DeviceBlock blk(st);
+  const int64_t* d_keys = nullptr;
+  const int64_t* d_ts = nullptr;
+  const void* d_cols[kMaxOuts] = {};
+  blk.input(d_keys, keys, (size_t)n * 8);
+  blk.input(d_ts, ts, (size_t)n * 8);
+  for (int c = 0; c < n_cols; ++c) blk.input(d_cols[c], cols[c], (size_t)n * col_bytes[c]);
+  if (int rc = blk.alloc()) return rc;
+  if (int rc = blk.upload()) return rc;
+  return index_build(ix, d_keys, d_ts, n, d_cols, col_bytes, n_cols, st);
+}
+
+static int check_index_args(const int64_t* keys, const int64_t* ts_ns, int64_t n_rows, const void* const* cols, const int32_t* col_bytes,
+                            int32_t n_cols, b2s_pit_t* out) {
+  if (!keys || !ts_ns || !out || n_rows <= 0 || n_rows > 0x7fffffffll || n_cols < 0 || n_cols > kMaxOuts || (n_cols && (!cols || !col_bytes)))
+    return b2s_int_fail(B2S_ERR_INVALID, "bad arguments");
+  for (int c = 0; c < n_cols; ++c)
+    if (!cols[c] || (col_bytes[c] != 4 && col_bytes[c] != 8)) return b2s_int_fail(B2S_ERR_INVALID, "column %d: null or not 4 / 8 bytes wide", c);
+  if (!b2s_int_inited()) return b2s_int_fail(B2S_ERR_STATE, "b2s_init was not called (no CUDA device: there is no CPU fallback)");
+  return B2S_OK;
+}
+
+// B2S_ERR_INVALID unless p is device memory of the library's device, aligned to `align` bytes
+static int check_on_device(const void* p, int align, const char* what, int i) {
+  if (misaligned(p, align)) return b2s_int_fail(B2S_ERR_INVALID, "%s %d: not %d-byte aligned", what, i, align);
+  int32_t dev = -1;
+  if (int rc = b2s_pointer_device(p, &dev)) return rc;
+  if (dev != b2s_int_device())
+    return b2s_int_fail(B2S_ERR_INVALID, "%s %d: %s, not memory of the library's device %d", what, i, dev < 0 ? "host memory" : "another device's memory",
+                        b2s_int_device());
+  return B2S_OK;
+}
+
+using IndexBuild = int (*)(b2s_pit_s*, const int64_t*, const int64_t*, int64_t, const void* const*, const int32_t*, int32_t, cudaStream_t);
+
+static int index_create(IndexBuild build, const int64_t* keys, const int64_t* ts_ns, int64_t n_rows, const void* const* cols,
+                        const int32_t* col_bytes, int32_t n_cols, b2s_pit_t* out) {
+  B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
+  auto* ix = new b2s_pit_s();
+  ix->n_rows = n_rows;
+  if (int rc = build(ix, keys, ts_ns, n_rows, cols, col_bytes, n_cols, b2s_int_stream())) {
+    b2s_pit_index_destroy(ix);
+    return rc;
+  }
+  *out = ix;
+  return B2S_OK;
+}
+
 extern "C" int b2s_pit_index_create(const int64_t* keys, const int64_t* ts_ns, int64_t n_rows, const void* const* cols,
                                     const int32_t* col_bytes, int32_t n_cols, b2s_pit_t* out) {
   try {  // no C++ exception crosses the C boundary
-    if (!keys || !ts_ns || !out || n_rows <= 0 || n_rows > 0x7fffffffll || n_cols < 0 || n_cols > kMaxOuts || (n_cols && (!cols || !col_bytes)))
-      return b2s_int_fail(B2S_ERR_INVALID, "bad arguments");
+    if (int rc = check_index_args(keys, ts_ns, n_rows, cols, col_bytes, n_cols, out)) return rc;
+    return index_create(index_build_host, keys, ts_ns, n_rows, cols, col_bytes, n_cols, out);
+  } catch (const std::exception& e) {
+    return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
+  }
+}
+
+extern "C" int b2s_pit_index_create_device(const int64_t* d_keys, const int64_t* d_ts, int64_t n_rows, const void* const* d_cols,
+                                           const int32_t* col_bytes, int32_t n_cols, b2s_pit_t* out) {
+  try {  // no C++ exception crosses the C boundary
+    if (int rc = check_index_args(d_keys, d_ts, n_rows, d_cols, col_bytes, n_cols, out)) return rc;
+    if (int rc = check_on_device(d_keys, 8, "keys", 0)) return rc;
+    if (int rc = check_on_device(d_ts, 8, "timestamps", 0)) return rc;
     for (int c = 0; c < n_cols; ++c)
-      if (!cols[c] || (col_bytes[c] != 4 && col_bytes[c] != 8)) return b2s_int_fail(B2S_ERR_INVALID, "column %d: null or not 4 / 8 bytes wide", c);
-    if (!b2s_int_inited()) return b2s_int_fail(B2S_ERR_STATE, "b2s_init was not called (no CUDA device: there is no CPU fallback)");
-    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
-    auto* ix = new b2s_pit_s();
-    ix->n_rows = n_rows;
-    if (int rc = index_build(ix, keys, ts_ns, n_rows, cols, col_bytes, n_cols, b2s_int_stream())) {
-      b2s_pit_index_destroy(ix);
-      return rc;
-    }
-    *out = ix;
-    return B2S_OK;
+      if (int rc = check_on_device(d_cols[c], col_bytes[c], "column", c)) return rc;
+    return index_create(index_build, d_keys, d_ts, n_rows, d_cols, col_bytes, n_cols, out);
   } catch (const std::exception& e) {
     return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
   }
@@ -1033,51 +1083,119 @@ int pack_empty(b2s_pit_tensors& out, bool label) {
   return label ? darray_new(out.label, 0) : B2S_OK;
 }
 
-// b2s_pit_train_pack over n > 0 rows: sets / cols are checked host descriptors whose destinations are stand-ins
-int pack_call(const int64_t* ts, int64_t n, b2s_pit_set* sets, int32_t n_sets, b2s_pit_col* cols, int32_t n_cols,
+// b2s_pit_train_pack over n > 0 rows: sets / cols are checked descriptors whose destinations are stand-ins and whose
+// inputs (d_ts, each set's keys, each column's source) are device memory.  Both entry points end here; the host one
+// stages its inputs first.
+int pack_call(const int64_t* d_ts, int64_t n, b2s_pit_set* sets, int32_t n_sets, b2s_pit_col* cols, int32_t n_cols,
               const b2s_pit_label* label, Pack pk, float* phase_ms, b2s_stats* stats) {
   cudaStream_t st = b2s_int_stream();
   Events ev;
-  if (int rc = ev.create(7)) return rc;
-  pk.ev = ev.data() + 5;
+  if (int rc = ev.create(6)) return rc;
+  pk.ev = ev.data() + 4;
   Launches launches;
   {
-    // one device block for the inputs and the counters: the outputs are train_run's scratch
+    // the counters: the outputs are train_run's scratch
     SyncOnExit done{st};
     DeviceBlock blk(st);
-    const int64_t* d_ts = nullptr;
-    if (ts) blk.input(d_ts, ts, (size_t)n * 8);
-    for (int s = 0; s < n_sets; ++s) blk.input(sets[s].keys, sets[s].keys, (size_t)n * 8);
-    for (int c = 0; c < n_cols; ++c) blk.input(cols[c].src, cols[c].src, (size_t)n * cols[c].bytes);
     unsigned long long* d_miss = nullptr;
     int64_t* d_kept = nullptr;
     blk.scratch(d_miss, 8 * (size_t)std::max(n_sets, 1));
     blk.scratch(d_kept, 8);
     if (int rc = blk.alloc()) return rc;
-    B2S_CUDA_TRY(cudaEventRecord(ev[0], st));
-    if (int rc = blk.upload()) return rc;
     if (int rc = train_run(d_ts, n, sets, n_sets, cols, n_cols, label, reinterpret_cast<int64_t*>(g_stand_in),
-                           d_miss, d_kept, st, ev.data() + 1, launches, &pk))
+                           d_miss, d_kept, st, ev.data(), launches, &pk))
       return rc;
   }
   B2S_CUDA_TRY(cudaStreamSynchronize(st));
   float keep_ms = 0.f, pack_ms = 0.f;
-  cudaEventElapsedTime(&keep_ms, ev[3], ev[4]);  // keep + scan
-  cudaEventElapsedTime(&pack_ms, ev[5], ev[6]);
+  cudaEventElapsedTime(&keep_ms, ev[2], ev[3]);  // keep + scan
+  cudaEventElapsedTime(&pack_ms, ev[4], ev[5]);
   if (phase_ms) {
-    cudaEventElapsedTime(&phase_ms[0], ev[1], ev[2]);  // sort
-    cudaEventElapsedTime(&phase_ms[1], ev[2], ev[3]);  // join
+    cudaEventElapsedTime(&phase_ms[0], ev[0], ev[1]);  // sort
+    cudaEventElapsedTime(&phase_ms[1], ev[1], ev[2]);  // join
     phase_ms[2] = keep_ms + pack_ms;                   // compaction (the host reads kept between the two)
     phase_ms[3] = pack_ms;
   }
   if (stats) {
     stats->rows = n;
-    cudaEventElapsedTime(&stats->h2d_ms, ev[0], ev[1]);
-    cudaEventElapsedTime(&stats->kernel_ms, ev[1], ev[4]);
+    cudaEventElapsedTime(&stats->kernel_ms, ev[0], ev[3]);
     stats->kernel_ms += pack_ms;
     stats->kernels = launches.n;
   }
   return B2S_OK;
+}
+
+// the host entry's first step: the timestamps, keys and entity columns uploaded into one block, then pack_call
+int pack_call_host(const int64_t* ts, int64_t n, b2s_pit_set* sets, int32_t n_sets, b2s_pit_col* cols, int32_t n_cols,
+                   const b2s_pit_label* label, Pack pk, float* phase_ms, b2s_stats* stats) {
+  cudaStream_t st = b2s_int_stream();
+  Events ev;
+  if (int rc = ev.create(2)) return rc;
+  SyncOnExit done{st};
+  DeviceBlock blk(st);
+  const int64_t* d_ts = nullptr;
+  if (ts) blk.input(d_ts, ts, (size_t)n * 8);
+  for (int s = 0; s < n_sets; ++s) blk.input(sets[s].keys, sets[s].keys, (size_t)n * 8);
+  for (int c = 0; c < n_cols; ++c) blk.input(cols[c].src, cols[c].src, (size_t)n * cols[c].bytes);
+  if (int rc = blk.alloc()) return rc;
+  B2S_CUDA_TRY(cudaEventRecord(ev[0], st));
+  if (int rc = blk.upload()) return rc;
+  B2S_CUDA_TRY(cudaEventRecord(ev[1], st));
+  if (int rc = pack_call(d_ts, n, sets, n_sets, cols, n_cols, label, pk, phase_ms, stats)) return rc;
+  if (stats) cudaEventElapsedTime(&stats->h2d_ms, ev[0], ev[1]);  // pack_call has synchronised the stream
+  return B2S_OK;
+}
+
+using PackRun = int (*)(const int64_t*, int64_t, b2s_pit_set*, int32_t, b2s_pit_col*, int32_t, const b2s_pit_label*, Pack, float*,
+                        b2s_stats*);
+
+// Both b2s_pit_train_pack entries: the checks, then `run` over n > 0 rows (on_device: ts, keys and sources must be memory
+// of the library's device).
+int train_pack(PackRun run, bool on_device, const int64_t* ts, int64_t n, const b2s_pit_set* sets, int32_t n_sets,
+               const b2s_pit_col* cols, int32_t n_cols, const b2s_pit_label* label, const b2s_pit_feat* feats, int32_t n_feats,
+               const b2s_pit_feat* label_vec, int32_t x_bytes, b2s_pit_tensors* out, float* phase_ms, b2s_stats* stats) {
+  if (!out || n_sets < 0 || n_cols < 0 || n_feats < 0 || (n_sets && !sets) || (n_cols && !cols) || (n_feats && !feats))
+    return b2s_int_fail(B2S_ERR_INVALID, "bad arguments");
+  if (x_bytes != 4 && x_bytes != 8) return b2s_int_fail(B2S_ERR_INVALID, "x_bytes %d: the matrix is float32 (4) or float64 (8)", x_bytes);
+  *out = b2s_pit_tensors{};
+  // every output, found flag and entity destination lives in scratch: the checks of b2s_pit_train_host run on copies
+  // whose destinations stand in for those regions
+  std::vector<b2s_pit_set> s2(sets, sets + n_sets);
+  std::vector<std::vector<b2s_pit_out>> o2(n_sets);
+  for (int s = 0; s < n_sets; ++s) {
+    if (s2[s].n_out < 0 || s2[s].n_out > kMaxOuts || (s2[s].n_out && !s2[s].outs))
+      return b2s_int_fail(B2S_ERR_INVALID, "set %d: null index / keys / outputs", s);
+    o2[s].assign(s2[s].outs, s2[s].outs + s2[s].n_out);
+    for (b2s_pit_out& o : o2[s]) o.out = g_stand_in;
+    s2[s].outs = o2[s].data();
+    s2[s].found = reinterpret_cast<uint8_t*>(g_stand_in);
+    s2[s].ts_out = nullptr;
+  }
+  std::vector<b2s_pit_col> c2(cols, cols + n_cols);
+  for (b2s_pit_col& c : c2) c.dst = g_stand_in;
+  int64_t counters[2];
+  if (int rc = check_train(s2.data(), n_sets, c2.data(), n_cols, ts, n, label, counters, counters + 1)) return rc;
+  for (int i = 0; i < n_feats; ++i)
+    if (int rc = check_feat(feats[i], s2.data(), n_sets, c2.data(), n_cols, "feature", i)) return rc;
+  if (label_vec)
+    if (int rc = check_feat(*label_vec, s2.data(), n_sets, c2.data(), n_cols, "label", 0)) return rc;
+  if (phase_ms) phase_ms[0] = phase_ms[1] = phase_ms[2] = phase_ms[3] = 0.f;
+  if (stats) memset(stats, 0, sizeof(*stats));
+  if (!b2s_int_inited()) return b2s_int_fail(B2S_ERR_STATE, "b2s_init was not called (no CUDA device: there is no CPU fallback)");
+  if (on_device && n) {
+    if (ts)
+      if (int rc = check_on_device(ts, 8, "timestamps", 0)) return rc;
+    for (int s = 0; s < n_sets; ++s)
+      if (int rc = check_on_device(s2[s].keys, 8, "keys of set", s)) return rc;
+    for (int c = 0; c < n_cols; ++c)
+      if (int rc = check_on_device(c2[c].src, c2[c].bytes, "entity column", c)) return rc;
+  }
+  B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
+  const int rc = n ? run(ts, n, s2.data(), n_sets, c2.data(), n_cols, label, Pack{feats, n_feats, label_vec, x_bytes, out, nullptr},
+                         phase_ms, stats)
+                   : pack_empty(*out, label_vec != nullptr);
+  if (rc) release_tensors(*out);
+  return rc;
 }
 
 }  // namespace
@@ -1180,40 +1298,21 @@ extern "C" int b2s_pit_train_pack(const int64_t* ts, int64_t n, const b2s_pit_se
                                   const b2s_pit_feat* label_vec, int32_t x_bytes, b2s_pit_tensors* out, float* phase_ms,
                                   b2s_stats* stats) {
   try {  // no C++ exception crosses the C boundary
-    if (!out || n_sets < 0 || n_cols < 0 || n_feats < 0 || (n_sets && !sets) || (n_cols && !cols) || (n_feats && !feats))
-      return b2s_int_fail(B2S_ERR_INVALID, "bad arguments");
-    if (x_bytes != 4 && x_bytes != 8) return b2s_int_fail(B2S_ERR_INVALID, "x_bytes %d: the matrix is float32 (4) or float64 (8)", x_bytes);
-    *out = b2s_pit_tensors{};
-    // every output, found flag and entity destination lives in scratch: the checks of b2s_pit_train_host run on copies
-    // whose destinations stand in for those regions
-    std::vector<b2s_pit_set> s2(sets, sets + n_sets);
-    std::vector<std::vector<b2s_pit_out>> o2(n_sets);
-    for (int s = 0; s < n_sets; ++s) {
-      if (s2[s].n_out < 0 || s2[s].n_out > kMaxOuts || (s2[s].n_out && !s2[s].outs))
-        return b2s_int_fail(B2S_ERR_INVALID, "set %d: null index / keys / outputs", s);
-      o2[s].assign(s2[s].outs, s2[s].outs + s2[s].n_out);
-      for (b2s_pit_out& o : o2[s]) o.out = g_stand_in;
-      s2[s].outs = o2[s].data();
-      s2[s].found = reinterpret_cast<uint8_t*>(g_stand_in);
-      s2[s].ts_out = nullptr;
-    }
-    std::vector<b2s_pit_col> c2(cols, cols + n_cols);
-    for (b2s_pit_col& c : c2) c.dst = g_stand_in;
-    int64_t counters[2];
-    if (int rc = check_train(s2.data(), n_sets, c2.data(), n_cols, ts, n, label, counters, counters + 1)) return rc;
-    for (int i = 0; i < n_feats; ++i)
-      if (int rc = check_feat(feats[i], s2.data(), n_sets, c2.data(), n_cols, "feature", i)) return rc;
-    if (label_vec)
-      if (int rc = check_feat(*label_vec, s2.data(), n_sets, c2.data(), n_cols, "label", 0)) return rc;
-    if (phase_ms) phase_ms[0] = phase_ms[1] = phase_ms[2] = phase_ms[3] = 0.f;
-    if (stats) memset(stats, 0, sizeof(*stats));
-    if (!b2s_int_inited()) return b2s_int_fail(B2S_ERR_STATE, "b2s_init was not called (no CUDA device: there is no CPU fallback)");
-    B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
-    const int rc = n ? pack_call(ts, n, s2.data(), n_sets, c2.data(), n_cols, label, Pack{feats, n_feats, label_vec, x_bytes, out, nullptr},
-                                 phase_ms, stats)
-                     : pack_empty(*out, label_vec != nullptr);
-    if (rc) release_tensors(*out);
-    return rc;
+    return train_pack(pack_call_host, false, ts, n, sets, n_sets, cols, n_cols, label, feats, n_feats, label_vec, x_bytes, out, phase_ms,
+                      stats);
+  } catch (const std::exception& e) {
+    if (out) release_tensors(*out);
+    return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
+  }
+}
+
+extern "C" int b2s_pit_train_pack_device(const int64_t* d_ts, int64_t n, const b2s_pit_set* sets, int32_t n_sets,
+                                         const b2s_pit_col* cols, int32_t n_cols, const b2s_pit_label* label, const b2s_pit_feat* feats,
+                                         int32_t n_feats, const b2s_pit_feat* label_vec, int32_t x_bytes, b2s_pit_tensors* out,
+                                         float* phase_ms, b2s_stats* stats) {
+  try {  // no C++ exception crosses the C boundary
+    return train_pack(pack_call, true, d_ts, n, sets, n_sets, cols, n_cols, label, feats, n_feats, label_vec, x_bytes, out, phase_ms,
+                      stats);
   } catch (const std::exception& e) {
     if (out) release_tensors(*out);
     return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());

@@ -21,6 +21,7 @@ import numpy as np
 from .. import _native as nat
 from ..lowering import LoweringError
 from ..serving.resolve import MLRunInvalidArgumentError
+from . import columnar
 from .ingest import _INT_DTYPES
 from .keys import _NAT, _UNIT_NS, _encode_keys, _key_kind, _ns
 
@@ -43,6 +44,22 @@ class PitIndex:
         self._h = C.c_void_p()
         nat.check(self._lib.b2s_pit_index_create(keys.ctypes.data, ts_ns.ctypes.data, len(keys), ptrs, nat._p(widths, C.c_int32),
                                                  len(cols), C.byref(self._h)))
+        self._info()
+
+    @classmethod
+    def device(cls, d_keys, d_ts, n, cols):
+        """the index of n rows whose keys, timestamps and columns [(address, 4 or 8 bytes)] are in device memory
+        (b2s_pit_index_create_device): nothing crosses to the host"""
+        self = cls.__new__(cls)
+        self._lib = nat.init()
+        ptrs = (C.c_void_p * max(len(cols), 1))(*[a for a, _w in cols])
+        widths = np.array([w for _a, w in cols] or [0], dtype=np.int32)
+        self._h = C.c_void_p()
+        nat.check(self._lib.b2s_pit_index_create_device(d_keys, d_ts, n, ptrs, nat._p(widths, C.c_int32), len(cols), C.byref(self._h)))
+        self._info()
+        return self
+
+    def _info(self):
         n_rows, n_keys, longest, cap = C.c_int64(), C.c_int64(), C.c_int64(), C.c_int64()
         words = C.c_int32()
         nat.check(self._lib.b2s_pit_index_info(self._h, C.byref(n_rows), C.byref(n_keys), C.byref(longest), C.byref(words),
@@ -134,26 +151,39 @@ def pit_train_pack(ts, sets, cols, label, feats, label_vec, dtype):
     bytes, nat.PIT_FEAT_*)] are the matrix columns, label_vec the label vector's source (or None), dtype float32 /
     float64 -> (features [kept, F], label [kept] or None, order [kept]: nat.DeviceArray, {sort_ms, join_ms, compact_ms,
     pack_ms, kept, **stats})"""
-    lib = nat.init()
     n = len(ts) if ts is not None else len(cols[0]) if cols else len(sets[0][1]) if sets else 0
     ts = None if ts is None else np.ascontiguousarray(ts, dtype=np.int64)
+    keys = [np.ascontiguousarray(k, dtype=np.int64) for _ix, k, _a, _o in sets]
+    srcs = [np.ascontiguousarray(c) for c in cols]
+    return _train_pack("b2s_pit_train_pack", None if ts is None else ts.ctypes.data, n,
+                       [(ix, k.ctypes.data, asof, outs) for (ix, _k, asof, outs), k in zip(sets, keys)],
+                       [(c.ctypes.data, c.dtype.itemsize) for c in srcs], label, feats, label_vec, dtype)
+
+
+def pit_train_pack_device(d_ts, n, sets, cols, label, feats, label_vec, dtype):
+    """pit_train_pack over inputs in device memory (b2s_pit_train_pack_device): d_ts an address or None, each set's keys
+    an address, cols [(address, bytes)]; nothing is uploaded"""
+    return _train_pack("b2s_pit_train_pack_device", d_ts, n, sets, cols, label, feats, label_vec, dtype)
+
+
+def _train_pack(entry, ts, n, sets, cols, label, feats, label_vec, dtype):
+    """one b2s_pit_train_pack* call: ts, keys and column sources are addresses the entry point reads"""
+    lib = nat.init()
     keep = []  # arrays the descriptors point into
     c_sets = (nat.PitSet * max(len(sets), 1))()
     for i, (index, keys, asof, outs) in enumerate(sets):
-        keys = np.ascontiguousarray(keys, dtype=np.int64)
         descs = (nat.PitOut * max(len(outs), 1))(*[nat.PitOut(w, np.dtype(dt).itemsize, m, None) for w, dt, m in outs])
-        keep += [keys, descs]
-        c_sets[i] = nat.PitSet(index._h, keys.ctypes.data, int(asof), len(outs), descs, None, None)
-    srcs = [np.ascontiguousarray(c) for c in cols]
-    c_cols = (nat.PitCol * max(len(cols), 1))(*[nat.PitCol(s.ctypes.data, None, s.dtype.itemsize) for s in srcs])
+        keep.append(descs)
+        c_sets[i] = nat.PitSet(index._h, keys, int(asof), len(outs), descs, None, None)
+    c_cols = (nat.PitCol * max(len(cols), 1))(*[nat.PitCol(a, None, w) for a, w in cols])
     c_label = None if label is None else C.byref(nat.PitLabel(*label))
     c_feats = (nat.PitFeat * max(len(feats), 1))(*[nat.PitFeat(*f) for f in feats])
     c_vec = None if label_vec is None else C.byref(nat.PitFeat(*label_vec))
     out = nat.PitTensors()
     phase = (C.c_float * 4)()
     stats = nat.Stats()
-    nat.check(lib.b2s_pit_train_pack(None if ts is None else ts.ctypes.data, n, c_sets, len(sets), c_cols, len(cols), c_label,
-                                     c_feats, len(feats), c_vec, np.dtype(dtype).itemsize, C.byref(out), phase, C.byref(stats)))
+    nat.check(getattr(lib, entry)(ts, n, c_sets, len(sets), c_cols, len(cols), c_label, c_feats, len(feats), c_vec,
+                                  np.dtype(dtype).itemsize, C.byref(out), phase, C.byref(stats)))
     k = out.kept
     features = nat.DeviceArray(out.features, (k, len(feats)), dtype)
     order = nat.DeviceArray(out.order, (k,), np.int64)
@@ -178,33 +208,165 @@ class TrainingTensors:
         self.columns, self.rows, self.stats = list(columns), rows, stats
 
 
+class _Columns:
+    """the columns of an entity frame or offline frame as the planner and the registration read them, filled from a pandas
+    frame or from CUDA columns: `columns` (names in order), `dtypes` {name: dtype}, `n`, and each column's data -- the
+    frame's (`frame`), or an acquirable `columnar.DeviceColumn` (`device`).  Keys are encoded and timestamps checked with
+    numpy on the host side and by the kernels on the device side; what is refused is refused alike."""
+
+    def __init__(self, columns, dtypes, n, frame=None, device=None):
+        self.columns, self.dtypes, self.n = list(columns), dict(dtypes), int(n)
+        self.frame, self.device = frame, device
+        self.keys = {}  # (names, kind) -> encoded keys of a device frame
+        self.profiles = {}  # name -> b2s_ts_profile_device counts of a device frame
+
+    @classmethod
+    def of_frame(cls, frame):
+        if frame.index.names[0]:
+            frame = frame.reset_index()
+        # dtypes by position: a name that appears twice is refused by the planner, not by a lookup here
+        return cls(frame.columns, dict(zip(frame.columns, frame.dtypes)), len(frame), frame=frame)
+
+    @classmethod
+    def of_device(cls, source, timestamp_names):
+        """CUDA columns (a mapping, or a DeviceColumnBatch whose index columns come first, as reset_index() puts them);
+        an int64 column named in `timestamp_names` is datetime64[ns].  Described, not acquired: nothing is read yet."""
+        cols = columnar.device_columns(source)
+        if len({c.n for c in cols.values()}) > 1:
+            raise ValueError("All arrays must be of the same length")
+        for name, c in cols.items():
+            if str(c.dtype) == "int64" and name in timestamp_names:
+                c.dtype = np.dtype("datetime64[ns]")
+        n = next(iter(cols.values())).n if cols else 0
+        return cls(cols, {k: c.dtype for k, c in cols.items()}, n, device=cols)
+
+    @staticmethod
+    def of(source, timestamp_names):
+        if columnar.is_columnar(source) and columnar.is_device_source(source):
+            return _Columns.of_device(source, timestamp_names)
+        return _Columns.of_frame(source)
+
+    def select(self, names, renamed):
+        """columns `names`, renamed `renamed`, in that order (the entity-less spine); a device frame keeps its encoded keys
+        under the new names (the set's own, made at registration).  Timestamps are profiled again by each query, as the
+        host path checks its frame's each time."""
+        if self.device is None:
+            frame = self.frame[names].copy(deep=False)
+            frame.columns = renamed
+            return _Columns.of_frame(frame.reset_index(drop=True))
+        new = dict(zip(names, renamed))
+        out = _Columns(renamed, {new[c]: self.dtypes[c] for c in names}, self.n, device={new[c]: self.device[c] for c in names})
+        out.keys = {(tuple(new[k] for k in ks), kind): v for (ks, kind), v in self.keys.items() if all(k in new for k in ks)}
+        return out
+
+    def to_host(self):
+        """the same columns on the host (one copy each): what `get_offline_features` assembles its frame from"""
+        if self.device is None:
+            return self
+        import pandas as pd
+
+        return _Columns.of_frame(pd.DataFrame({c: self.device[c].numpy().view(self.dtypes[c]) for c in self.columns}, copy=False))
+
+    def acquire(self, names):
+        """-> {name: device address} of the named device columns, the library stream ordered behind their producers"""
+        return {c: self.device[c].acquire().ptr for c in names}
+
+    def release(self):
+        if self.device is not None:
+            for c in self.device.values():
+                c.release()
+
+    def key_kind(self, names, what):
+        if self.device is not None:
+            for k in names:
+                if k in self.dtypes and self.dtypes[k].kind in "OSU":
+                    raise LoweringError(f"{what}: key {k!r} of dtype {self.dtypes[k]} is a string key: there are no string "
+                                        "columns on the device (hash them on the host)")
+            return _key_kind({k: np.empty(0, self.dtypes[k]) for k in names}, names, what)
+        return _key_kind(self.frame, names, what)
+
+    def encode_keys(self, names, kind, what):
+        """numpy int64 keys of a host frame; a DeviceArray of a device frame (b2s_keys_encode_device, once per key)"""
+        if self.device is None:
+            return _encode_keys(self.frame, names, kind, what)
+        at = (tuple(names), kind)
+        if at not in self.keys:
+            lib = nat.init()
+            keys = nat.DeviceArray(nat.darray_alloc(8 * self.n), (self.n,), np.int64)
+            if self.n:
+                ptrs = self.acquire(names)
+                kc = (nat.KeyCol * len(names))(*[nat.KeyCol(ptrs[k], self.dtypes[k].itemsize, int(self.dtypes[k].kind == "i"))
+                                                 for k in names])
+                nat.check(lib.b2s_keys_encode_device(kc, len(names), self.n, keys.ptr, None))
+            self.keys[at] = keys
+        return self.keys[at]
+
+    def timestamps(self, name, what, profile=True):
+        """-> (int64 nanoseconds: a host array, or a device address), unit, [NaT, not whole us, ms, s] counts (a host
+        frame without `profile`: [NaT] alone)"""
+        if self.device is None:
+            ts_ns, unit = _ns(self.frame[name], what)
+            if not profile:
+                return ts_ns, unit, [int((ts_ns == _NAT).sum())]
+            real = ts_ns[ts_ns != _NAT]
+            return ts_ns, unit, [len(ts_ns) - len(real)] + [int((real % f).any()) for f in (10**3, 10**6, 10**9)]
+        self.timestamp_dtype(name, what)
+        ptr = self.acquire([name])[name]
+        if name not in self.profiles:
+            counts = np.zeros(4, dtype=np.int64)
+            nat.check(nat.init().b2s_ts_profile_device(ptr, self.n, nat._p(counts, C.c_int64), None))
+            self.profiles[name] = [int(v) for v in counts]
+        return ptr, "ns", self.profiles[name]
+
+    def timestamp_dtype(self, name, what):
+        """CUDA timestamps are int64 nanoseconds (datetime64[ns]); any other dtype is refused as `keys._ns` refuses it"""
+        dt = self.dtypes[name]
+        if dt != np.dtype("datetime64[ns]"):
+            raise LoweringError(f"{what} has dtype {dt}: the as-of join takes tz-naive datetime64 timestamps")
+
+    def array(self, name):
+        """a column's data for the join: a numpy array, or a device address"""
+        return self.frame[name].to_numpy() if self.device is None else self.acquire([name])[name]
+
+
+def _ts_factor(counts):
+    """the coarsest unit every timestamp is a whole number of (10^9 when there are none): a query whose timestamps are
+    coarser would round them"""
+    return next((f for f, c in zip((10**9, 10**6, 10**3), counts[:0:-1]) if not c), 1)
+
+
 class OfflineSource:
-    """one feature set's offline frame, registered with its device index (built once)"""
+    """one feature set's offline rows, registered with its device index (built once): a pandas frame, or CUDA columns
+    that stay in HBM"""
 
     def __init__(self, featureset, frame):
         self.featureset = featureset
         self.name = featureset.name
         self.entities = [e.name for e in featureset.entities]
         self.timestamp_key = featureset.timestamp_key
-        if frame.index.names[0]:
-            frame = frame.reset_index()
-        missing = [k for k in self.entities + ([self.timestamp_key] if self.timestamp_key else []) if k not in frame.columns]
+        self.keys = None
+        rows = _Columns.of(frame, {self.timestamp_key} if self.timestamp_key else set())
+        missing = [k for k in self.entities + ([self.timestamp_key] if self.timestamp_key else []) if k not in rows.columns]
         if missing:
             raise MLRunInvalidArgumentError(f"feature set {self.name}: the offline frame has no column {missing[0]!r}")
         if not self.entities:
             raise LoweringError(f"feature set {self.name} has no entities: only keyed feature sets are joined on the device")
-        self.frame = frame
-        self.key_kind = _key_kind(frame, self.entities, f"feature set {self.name}")
-        keys = _encode_keys(frame, self.entities, self.key_kind, f"feature set {self.name}")
+        self.rows = rows
+        self.frame = rows.frame
+        what = f"feature set {self.name}"
+        self.key_kind = rows.key_kind(self.entities, what)
+        if rows.device is not None:
+            self._register_device(rows, what)
+            return
+        frame = rows.frame
+        keys = rows.encode_keys(self.entities, self.key_kind, what)
         if self.key_kind == "str":
             strings = frame[self.entities[0]].to_numpy()
             if len(np.unique(keys)) != len(set(strings.tolist())):
                 raise MLRunInvalidArgumentError(f"feature set {self.name}: two entity keys share a 64-bit hash")
         if self.timestamp_key:
-            ts_ns, _unit = _ns(frame[self.timestamp_key], f"feature set {self.name} timestamp {self.timestamp_key!r}")
-            self.has_nat = bool((ts_ns == _NAT).any())
-            # the coarsest unit every timestamp is a whole number of: a query whose timestamps are coarser would round them
-            self.ts_factor = max((f for f in _UNIT_NS.values() if not (ts_ns[ts_ns != _NAT] % f).any()), default=1)
+            ts_ns, _unit, counts = rows.timestamps(self.timestamp_key, f"{what} timestamp {self.timestamp_key!r}")
+            self.has_nat, self.ts_factor = counts[0] > 0, _ts_factor(counts)
         else:
             ts_ns, self.has_nat, self.ts_factor = np.zeros(len(frame), dtype=np.int64), False, 10**9
         self.features, cols, word = {}, [], 0
@@ -229,12 +391,87 @@ class OfflineSource:
             word += stored.dtype.itemsize // 4
         self.index = PitIndex(keys, ts_ns, cols)
 
+    def _register_device(self, rows, what):
+        """the index of CUDA columns, built where they are: keys encoded (kept as a library array, so that later writes to
+        the caller's entity columns do not change the set), the timestamps profiled, narrow ints and bool widened to int32
+        in temporaries; only counters come back"""
+        self.features, plan, word, widen = {}, [], 0, []
+        for name in rows.columns:
+            if name in self.entities or name == self.timestamp_key:
+                continue
+            dt = rows.dtypes[name]
+            s = str(dt)
+            if s == "float32":
+                width, miss = 4, _NAN32
+            elif s == "float64":
+                width, miss = 8, _NAN64
+            elif s in _INT_DTYPES:
+                width, miss = 4, 0
+                if s != "int32":
+                    widen.append(name)
+            elif dt.kind == "M":
+                width, miss = 8, _NAT
+            else:
+                self.features[name] = (None, s, None)  # refused when a vector selects it
+                continue
+            self.features[name] = (word, s, miss)
+            plan.append((name, width))
+            word += width // 4
+        if self.timestamp_key:
+            rows.timestamp_dtype(self.timestamp_key, f"{what} timestamp {self.timestamp_key!r}")  # refused before any call
+        lib = nat.init()
+        n = rows.n
+        try:
+            if self.timestamp_key:
+                d_ts, _unit, counts = rows.timestamps(self.timestamp_key, f"{what} timestamp {self.timestamp_key!r}")
+                self.has_nat, self.ts_factor = counts[0] > 0, _ts_factor(counts)
+                zeros = None
+            self.keys = rows.encode_keys(self.entities, self.key_kind, what)
+            if not self.timestamp_key:
+                zeros = nat.DeviceArray(nat.darray_alloc(8 * n, zero=True), (n,), np.int64)
+                d_ts, self.has_nat, self.ts_factor = zeros.ptr, False, 10**9
+            ptrs = rows.acquire([name for name, _w in plan])
+            # 1- and 2-byte ints and bool as int32, in one convert launch into one temporary block
+            pitch = (4 * n + 255) // 256 * 256
+            temp = nat.DeviceArray(nat.darray_alloc(max(pitch * len(widen), 8)), (max(pitch * len(widen), 8),), np.uint8) \
+                if widen else None
+            kinds = {"int8": nat.CONV_I8_I32, "uint8": nat.CONV_U8_I32, "bool": nat.CONV_U8_I32, "int16": nat.CONV_I16_I32,
+                     "uint16": nat.CONV_U16_I32}
+            ops = []
+            for j, name in enumerate(widen):
+                ops.append(nat.Convert(ptrs[name], temp.ptr + j * pitch, kinds[str(rows.dtypes[name])], 0))
+                ptrs[name] = temp.ptr + j * pitch
+            if ops and n:
+                nat.check(lib.b2s_cols_convert_device((nat.Convert * len(ops))(*ops), len(ops), n, None, 0, None))
+            self.index = PitIndex.device(self.keys.ptr if n else None, d_ts if n else None, n,
+                                         [(ptrs[name], width) for name, width in plan])
+            del temp, zeros  # the build has synchronised: the temporaries go back now
+        except BaseException:
+            if self.keys is not None:
+                self.keys.release()
+            raise
+        finally:
+            rows.release()
+
+    @property
+    def ts_dtype(self):
+        return self.rows.dtypes[self.timestamp_key]
+
     def close(self):
-        self.index.close()
+        index = getattr(self, "index", None)
+        if index is not None:
+            index.close()
+        if self.keys is not None:
+            self.keys.release()
+        self.rows.keys, self.rows.profiles = {}, {}
 
 
 def register_offline_frame(featureset, frame):
-    """hand over a feature set's offline rows (the frame its targets would hold); the device index is built here"""
+    """hand over a feature set's offline rows (the frame its targets would hold); the device index is built here.  `frame`
+    is a pandas frame, or CUDA columns: a `columnar.DeviceColumnBatch` (`FeatureSet.ingest`'s result; its `index` holds the
+    entity columns) or a mapping of CUDA columns, whose int64 `timestamp_key` column is nanoseconds.  The source registered
+    from CUDA columns behaves as the one registered from the equal pandas frame, and its columns stay in HBM: only counters
+    cross to the host."""
     old = _OFFLINE.pop(featureset.name, None)
     if old is not None:
         old.close()
@@ -323,9 +560,11 @@ class _Query:
 
 def _plan_query(vector, entity_rows=None, entity_timestamp_column=None, target=None, run_config=None, drop_columns=None,
                 start_time=None, end_time=None, with_indexes=False, update_stats=False, engine=None, engine_args=None, query=None,
-                order_by=None, spark_service=None, timestamp_for_filtering=None, additional_filters=None):
+                order_by=None, spark_service=None, timestamp_for_filtering=None, additional_filters=None, on_host=False):
     """the one planner of `get_offline_features` and `get_offline_tensors`: refusals, the parsed fields and label, the
-    entity-less spine, the join of each set, the entity timestamps and the device descriptors"""
+    entity-less spine, the join of each set, the entity timestamps and the device descriptors.  The entity frame is read
+    through `_Columns`, from a pandas frame or from CUDA columns (`q.device`: then the timestamps, keys and columns of
+    the device call are device addresses); `on_host` copies a spine registered from CUDA columns to the host first."""
     if entity_rows is None and entity_timestamp_column is not None:  # api.py:228-232
         raise MLRunInvalidArgumentError("entity_timestamp_column param can not be specified without entity_rows param")
     if engine not in (None, "local"):
@@ -360,22 +599,21 @@ def _plan_query(vector, entity_rows=None, entity_timestamp_column=None, target=N
                 raise LoweringError(f"feature set {name} is keyed by {_OFFLINE[name].entities}, the first set by {spine.entities}: "
                                     "relations between differently keyed feature sets are not lowered")
         head = spine.entities + ([spine.timestamp_key] if spine.timestamp_key else [])
-        entity_rows = spine.frame[head + [f for f, _a in fields[spine_name]]].copy(deep=False)
         spine_features = [f"{f}_{spine_name}" for f, _a in fields[spine_name]]
-        entity_rows.columns = head + spine_features
-        entity_rows = entity_rows.reset_index(drop=True)
+        entity_rows = spine.rows.select(head + [f for f, _a in fields[spine_name]], head + spine_features)
         entity_timestamp_column = spine.timestamp_key
         spine_alias = dict(([(c, c) for c in head] if not drop_indexes else []) +
                            [(f"{f}_{spine_name}", a or f) for f, a in fields.pop(spine_name)])
         index_columns = list(spine.entities)
     else:
         index_columns = []
-        if entity_rows.index.names[0]:
-            entity_rows = entity_rows.reset_index()
-    n = len(entity_rows)
+        entity_rows = _Columns.of(entity_rows, {entity_timestamp_column} if entity_timestamp_column else set())
     names = [str(c) for c in entity_rows.columns]
     if len(set(names)) != len(names):
         raise LoweringError("duplicate column names in the entity frame")
+    if entity_less and on_host:
+        entity_rows = entity_rows.to_host()
+    n = entity_rows.n
 
     # the join of each set (base.py:430-460): as-of when it has a timestamp key and an entity timestamp column is known
     entity_ts = entity_timestamp_column
@@ -396,12 +634,8 @@ def _plan_query(vector, entity_rows=None, entity_timestamp_column=None, target=N
         ts_col = ts_col or src.timestamp_key
     any_asof = any(a for _n, _s, a in plan)
     ts_ns = unit = None
-    if any_asof:
-        if entity_ts not in entity_rows.columns:
-            raise KeyError(entity_ts)
-        ts_ns, unit = _ns(entity_rows[entity_ts], f"entity timestamp {entity_ts!r}")
-        if (ts_ns == _NAT).any():
-            raise ValueError("Merge keys contain null values on left side")
+
+    def set_refusals(unit):
         for name, src, asof in plan:
             if asof and src.has_nat:
                 raise ValueError("Merge keys contain null values on right side")
@@ -409,22 +643,44 @@ def _plan_query(vector, entity_rows=None, entity_timestamp_column=None, target=N
                 raise LoweringError(f"feature set {name}: timestamps finer than the entity column's unit {unit!r} would be "
                                     "rounded by the reference's cast: not lowered")
 
+    # CUDA columns: every refusal is raised before the first launch (the timestamp profile, a key encode), in the host's
+    # order.  The one refusal that reads data, NaT on the left side, cannot come first: a key-kind refusal wins over it.
+    key_error = None
+    if entity_rows.device is not None:
+        try:
+            for name, src, _asof in plan:
+                _entity_key_kind(entity_rows, name, src)
+        except LoweringError as err:
+            key_error = err
+    if any_asof:
+        if entity_ts not in entity_rows.columns:
+            raise KeyError(entity_ts)
+        if key_error is not None:
+            entity_rows.timestamp_dtype(entity_ts, f"entity timestamp {entity_ts!r}")
+            set_refusals("ns")
+            raise key_error
+        ts_ns, unit, counts = entity_rows.timestamps(entity_ts, f"entity timestamp {entity_ts!r}", profile=False)
+        if counts[0]:
+            raise ValueError("Merge keys contain null values on left side")
+        set_refusals(unit)
+    if key_error is not None:
+        raise key_error
+
     # device call: every set's selected words, its timestamps and found flags; numeric entity columns permuted alongside
     sets = []
     for name, src, asof in plan:
-        kind = _key_kind(entity_rows, src.entities, f"entity keys of {name}")
-        if kind != src.key_kind:
-            raise LoweringError(f"feature set {name}: entity keys are {kind}, the set's are {src.key_kind}")
-        keys = _encode_keys(entity_rows, src.entities, kind, f"entity keys of {name}")
+        kind = _entity_key_kind(entity_rows, name, src)
+        keys = entity_rows.encode_keys(src.entities, kind, f"entity keys of {name}")
         outs = []
         for f, _a in fields[name]:
             word, s, miss = src.features[f]
             outs.append((word, np.int64 if s.startswith("datetime64") else np.float64 if s == "float64" else np.float32 if s == "float32"
                          else np.int32, miss))
-        sets.append((src.index, keys, asof, outs))
-    dev_cols = [c for c in entity_rows.columns if entity_rows[c].dtype.kind in "iufMb" and getattr(entity_rows[c].dtype, "tz", None) is None
-                and isinstance(entity_rows[c].dtype, np.dtype)]
-    arrays = [entity_rows[c].to_numpy() for c in dev_cols]
+        sets.append((src.index, keys.ptr if entity_rows.device is not None else keys, asof, outs))
+    dtypes = entity_rows.dtypes
+    dev_cols = [c for c in entity_rows.columns if dtypes[c].kind in "iufMb" and getattr(dtypes[c], "tz", None) is None
+                and isinstance(dtypes[c], np.dtype)]
+    arrays = [entity_rows.array(c) for c in dev_cols]
     dev_label = None
     if label is not None:  # the label's place on the device: an output of its set, or the spine's own column
         lname, lfeat = label
@@ -442,7 +698,15 @@ def _plan_query(vector, entity_rows=None, entity_timestamp_column=None, target=N
     q.dev_cols, q.arrays, q.spine_alias, q.spine_features = dev_cols, arrays, spine_alias, spine_features
     q.index_columns, q.entity_less, q.drop_indexes = index_columns, entity_less, drop_indexes
     q.train = label is not None or entity_less
+    q.device = entity_rows.device is not None
     return q
+
+
+def _entity_key_kind(entity_rows, name, src):
+    kind = entity_rows.key_kind(src.entities, f"entity keys of {name}")
+    if kind != src.key_kind:
+        raise LoweringError(f"feature set {name}: entity keys are {kind}, the set's are {src.key_kind}")
+    return kind
 
 
 def _layout(q):
@@ -508,12 +772,18 @@ def get_offline_features(feature_vector, entity_rows=None, entity_timestamp_colu
                          engine_args=None, query=None, order_by=None, spark_service=None, timestamp_for_filtering=None,
                          additional_filters=None):
     """feature_store/api.py:99 on the local engine: the training frame of `feature_vector` for `entity_rows`, point-in-time
-    correct per feature set.  What the device does not run is refused with LoweringError (there is no pandas fallback)."""
+    correct per feature set.  What the device does not run is refused with LoweringError (there is no pandas fallback).
+    Feature sets registered from CUDA columns are joined where their indexes are; without entity rows, a spine registered
+    from CUDA columns has the columns the frame uses copied to the host once per call, since the result is a host frame.
+    CUDA `entity_rows` are refused: `get_offline_tensors` builds the training set from them without leaving the device."""
+    if entity_rows is not None and columnar.is_columnar(entity_rows) and columnar.is_device_source(entity_rows):
+        raise LoweringError("entity_rows are CUDA columns: get_offline_features returns a host frame; use get_offline_tensors, "
+                            "which builds the training set from them in device memory")
     q = _plan_query(feature_vector, entity_rows, entity_timestamp_column, target=target, run_config=run_config,
                     drop_columns=drop_columns, start_time=start_time, end_time=end_time, with_indexes=with_indexes,
                     update_stats=update_stats, engine=engine, engine_args=engine_args, query=query, order_by=order_by,
                     spark_service=spark_service, timestamp_for_filtering=timestamp_for_filtering,
-                    additional_filters=additional_filters)
+                    additional_filters=additional_filters, on_host=True)
     sets, arrays = q.sets, q.arrays
     if not q.n:
         order, joined, permuted, miss = (
@@ -539,14 +809,14 @@ def get_offline_features(feature_vector, entity_rows=None, entity_timestamp_colu
             c = source[1]
             if c in moved:
                 v = moved[c]
-                v = v.view(q.entity_rows[c].dtype) if v.dtype != q.entity_rows[c].dtype else v
+                v = v.view(q.entity_rows.dtypes[c]) if v.dtype != q.entity_rows.dtypes[c] else v
             else:  # strings, categories, objects: permuted on the host in the device's order
-                v = q.entity_rows[c].take(order).reset_index(drop=True).array
+                v = q.entity_rows.frame[c].take(order).reset_index(drop=True).array
         elif source[0] == "ts":
             name, src, asof = q.plan[source[1]]
             ts_out = joined[source[1]][1]
             # as-of: cast to the entity column's unit (base.py:389-410); exact: the set's own unit
-            tdt = np.dtype(f"datetime64[{q.unit}]") if asof else src.frame[src.timestamp_key].dtype
+            tdt = np.dtype(f"datetime64[{q.unit}]") if asof else src.ts_dtype
             v = np.where(ts_out == _NAT, _NAT, ts_out // _UNIT_NS[np.datetime_data(tdt)[0]]).view(tdt)
         else:
             s_i, j = source[1], source[2]
@@ -569,11 +839,23 @@ def get_offline_tensors(feature_vector, entity_rows=None, entity_timestamp_colum
     device memory: row i of `features`, `label` and `order` is row i of that call's `to_dataframe()`; the features are its
     columns without the label, the entity frame's own columns, the keys and the timestamps, converted as
     `to_numpy(dtype)` converts them (a missing value is NaN, bool 0 / 1).  Refuses what `get_offline_features` refuses,
-    with the same messages, and datetime features, which a matrix of numbers cannot hold."""
+    with the same messages, and datetime features, which a matrix of numbers cannot hold.
+
+    Entity rows may be CUDA columns (a mapping or a `columnar.DeviceColumnBatch`; `entity_timestamp_column` then names an
+    int64 / datetime64[ns] column of nanoseconds), and without entity rows the spine may be a set registered from CUDA
+    columns: the timestamps, keys and spine columns are then read where they are in HBM, and nothing is uploaded."""
     if np.dtype(dtype) not in (np.float32, np.float64):
         raise ValueError(f"dtype {dtype!r}: the feature matrix is float32 or float64")
     dtype = np.dtype(dtype)
     q = _plan_query(feature_vector, entity_rows, entity_timestamp_column, **options)
+    try:
+        return _tensors(q, dtype)
+    finally:
+        q.entity_rows.release()
+
+
+def _tensors(q, dtype):
+    """get_offline_tensors' pack of a planned query"""
     layout, _index_columns = _layout(q)
     label_source = None
     if q.dev_label is not None:
@@ -597,11 +879,11 @@ def get_offline_tensors(feature_vector, entity_rows=None, entity_timestamp_colum
                                     "the vector)")
             width, kind = _feat_kind(stored if stored in ("float32", "float64") else np.int32)
             return (s_i, j, width, nat.PIT_FEAT_BOOL if stored == "bool" else kind)
-        col = q.entity_rows[source[1]]
-        if col.dtype.kind == "M":
-            raise LoweringError(f"{what} {name!r} is a {col.dtype} column: a matrix of numbers has no place for it (drop it from "
+        col_dtype = q.entity_rows.dtypes[source[1]]
+        if col_dtype.kind == "M":
+            raise LoweringError(f"{what} {name!r} is a {col_dtype} column: a matrix of numbers has no place for it (drop it from "
                                 "the vector)")
-        return (-1, used.index(source[1])) + _feat_kind(col.dtype)
+        return (-1, used.index(source[1])) + _feat_kind(col_dtype)
 
     feats = [device_source(name, source, "feature") for name, source in picked]
     label_vec = None
@@ -610,5 +892,10 @@ def get_offline_tensors(feature_vector, entity_rows=None, entity_timestamp_colum
     dev_label = q.dev_label
     if dev_label is not None and dev_label[0] < 0:
         dev_label = (-1, used.index(label_source[1]), dev_label[2])
-    features, label, order, stats = pit_train_pack(q.ts_ns, q.sets, arrays, dev_label, feats, label_vec, dtype)
+    if q.device:
+        widths = [q.entity_rows.dtypes[c].itemsize for c in used]
+        features, label, order, stats = pit_train_pack_device(q.ts_ns, q.n, q.sets, list(zip(arrays, widths)), dev_label, feats,
+                                                              label_vec, dtype)
+    else:
+        features, label, order, stats = pit_train_pack(q.ts_ns, q.sets, arrays, dev_label, feats, label_vec, dtype)
     return TrainingTensors(features, label, order, [name for name, _s in picked], stats["kept"], stats)

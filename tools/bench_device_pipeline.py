@@ -4,8 +4,8 @@ add_aggregation.  The two paths alternate; each iteration checks that the device
 
 Prints one JSON line: each path's ingest times (the frame path from a pandas frame to a result frame; the device path from
 torch CUDA columns to a DeviceColumnBatch in HBM, synchronised), the device path's launches, staged and converted bytes, and
-the card and power limit the numbers were taken on.  Registration and training tensors from device sets are not part of
-this benchmark: those steps still take host frames.
+the card and power limit the numbers were taken on.  Registration and training tensors from device sets are measured by
+tools/bench_device_chain.py, which times the whole chain from CUDA columns to a training matrix.
 
     python tools/bench_device_pipeline.py [--rows 16777216] [--keys 1048576] [--iters 3]
 """
