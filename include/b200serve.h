@@ -248,8 +248,9 @@ int b2s_ring_bench(b2s_plan_t plan, const void* rows, int64_t n_src_rows, int64_
  * serving/routers.py:797-810).  The only exchange is the merge of every shard's votes into the full
  * response.  Instead of a separate all-gather, a plan can be given the output buffers of all ranks
  * (peer-mapped over NVLink with the IPC calls below); its kernels then store each output row into every
- * target at row `row_offset + row` straight from the epilogue (b2s_run_device only: b2s_run_host and the ring refuse
- * the plan).  n_peers = 0 restores local output. */
+ * target at row `row_offset + row` straight from the epilogue, the same words the plan writes locally (b2s_run_device
+ * only: b2s_run_host, the ring and b2s_table_enrich_host / _device refuse the plan with B2S_ERR_UNSUPPORTED).  At most 8
+ * targets; row_offset >= 0 needs no alignment.  n_peers = 0 restores local output. */
 int b2s_plan_set_merge_targets(b2s_plan_t plan, void* const* peer_out, int32_t n_peers, int64_t row_offset);
 int b2s_ipc_export(void* dptr, void* handle64 /* 64 bytes out */);
 int b2s_ipc_open(const void* handle64, void** dptr_out);
@@ -260,8 +261,10 @@ int b2s_ipc_close(void* dptr);
  * that can all-gather 64 bytes per rank (torch.distributed, MPI, a file, a socket ...):
  *     b2s_comm_create(rank, world, max_rows_per_rank, out_cols, &c);  b2s_comm_handle(c, mine);
  *     <all-gather the 64-byte handles>;  b2s_comm_connect(c, all);  b2s_plan_attach_comm(plan, c);
- * Every b2s_run_device launch of an attached plan (the host entry points refuse it) is then one STEP (epoch e = 1, 2,
- * ...) of the ensemble-merge (serving/routers.py:414-455 fans the event out to the routes, :789-810 reduces them; here the rows are
+ * Every b2s_run_device launch of an attached plan (the host and enrichment entry points refuse it) is then one STEP (epoch
+ * e = 1, 2, ...), a launch of 0 rows included: an empty shard stores nothing, but one small kernel still publishes its flag
+ * (and runs the fused wait), so that every rank takes every step.  A step is one ensemble-merge
+ * (serving/routers.py:414-455 fans the event out to the routes, :789-810 reduces them; here the rows are
  * sharded and the votes merged): the kernels store this rank's votes into slot e & 3 of EVERY rank's merged rows at row
  * block `rank`, and the launch's last CTA publishes e in every rank's flag array (st.release.sys).  b2s_comm_wait enqueues
  * a one-warp kernel that acquires all `world` flags of THIS rank at the current epoch, so work enqueued behind it (a D2H copy,
@@ -417,6 +420,8 @@ int b2s_table_lookup_host(b2s_table_t table, const int64_t* keys, int64_t n, flo
  * fetches the row from there (one TMA bulk copy per row), so the gathered rows never travel to HBM and back; the table's
  * impute policy folds into the kernel's Imputer operands.  B2S_ERR_UNSUPPORTED for plans the loader does not cover (tree
  * ensembles, MapValues, one-hot sources under an impute policy): use b2s_table_lookup_device + b2s_run_device then.
+ * Both enrichment calls refuse a plan with merge targets or an attached communicator (B2S_ERR_UNSUPPORTED, before anything
+ * is enqueued and without a step of the communicator): its kernels would store the votes there, not into `out`.
  * B2S_ERR_INVALID, before any launch, when d_keys is not 8-byte aligned or d_out / d_status is not 4-byte aligned. */
 int b2s_table_enrich_device(b2s_table_t table, b2s_plan_t plan, const int64_t* d_keys, int64_t n, void* d_out,
                             int32_t* d_status, void* stream);

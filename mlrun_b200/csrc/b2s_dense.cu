@@ -278,26 +278,27 @@ __global__ void __launch_bounds__(kDenseThreads, 1) dense_head_kernel(const __gr
         for (int k = 0; k < NP; ++k) sc[k] = sc_stage[rr * (NP + 1) + k];
         const int64_t row = t * kDM + wg * kWgRows + rr;
         if (row < p.n_rows) {
-          if (p.epi != DENSE_EPI_GENERIC && kp.n_peers == 0) {
-            // ---- fast epilogues: float32 registers only (compile-time indices; the intercepts are constant-bank operands)
+          if (p.epi != DENSE_EPI_GENERIC) {
+            // ---- fast epilogues: float32 registers only (compile-time indices; the intercepts are constant-bank operands).
+            // Merged rows take the same arithmetic as local ones: only the store differs (store_word, one word per target)
 #pragma unroll
             for (int k = 0; k < NP; ++k) sc[k] += p.biasf[k];
             if (p.epi == DENSE_EPI_SCORES) {  // out_cols == n_scores consecutive floats per row
-              float* o = kp.out + row * kp.out_cols;
-              if ((kp.out_cols & 3) == 0) {
+              if (kp.n_peers == 0 && (kp.out_cols & 3) == 0) {
+                float* o = kp.out + row * kp.out_cols;
 #pragma unroll
                 for (int k = 0; k < NP; k += 4)
                   if (k < p.n_scores) *reinterpret_cast<float4*>(o + k) = make_float4(sc[k], sc[k + 1], sc[k + 2], sc[k + 3]);
               } else {
 #pragma unroll
                 for (int k = 0; k < NP; ++k)
-                  if (k < p.n_scores) o[k] = sc[k];
+                  if (k < p.n_scores) store_word(kp, row, k, __float_as_uint(sc[k]));
               }
             } else if (p.epi == DENSE_EPI_MEAN) {  // VotingEnsemble._mean_vote: sum_m w[m] * pred[m], model order
               float v = 0.f;
 #pragma unroll
               for (int k = 0; k < NP; ++k) v = fmaf(p.votewf[k], sc[k], v);  // the padding has zero weight
-              kp.out[row] = v;
+              store_word(kp, row, 0, __float_as_uint(v));
             } else {  // one multi-class linear classifier: np.argmax (first maximum), then classes_[index]
               int best = 0;
               float bv = sc[0];
@@ -310,7 +311,7 @@ __global__ void __launch_bounds__(kDenseThreads, 1) dense_head_kernel(const __gr
               int lab = p.labels[0];
 #pragma unroll
               for (int k = 1; k < NP; ++k) lab = best == k ? p.labels[k] : lab;
-              reinterpret_cast<int32_t*>(kp.out)[row] = lab;
+              store_word(kp, row, 0, (uint32_t)lab);
             }
             if (kp.status) kp.status[row] = (int32_t)st;
           } else {

@@ -33,6 +33,8 @@ static inline int grid_for(int64_t n, int threads) {
 struct b2s_plan_s;
 B2S_HIDDEN int b2s_int_plan_shape(b2s_plan_s* plan, int* n_in, int* out_cols);  // B2S_ERR_STATE unless finalized
 B2S_HIDDEN int b2s_int_plan_kernels(const b2s_plan_s* plan);  // launches of one batch of a finalized plan (trees3: 3)
+// the plan's kernels store their votes to merge targets or an attached communicator, not into the caller's output
+B2S_HIDDEN bool b2s_int_plan_merges(const b2s_plan_s* plan);
 
 // the online table as the scoring kernel's gather loader sees it (b2s_table.cu fills it in)
 struct B2SGather {

@@ -278,6 +278,7 @@ struct b2s_plan_s {
 };
 
 int b2s_int_plan_kernels(const b2s_plan_s* p) { return p->kernels_per_batch; }
+bool b2s_int_plan_merges(const b2s_plan_s* p) { return p && (!p->peers.empty() || p->comm); }
 
 int b2s_int_plan_shape(b2s_plan_s* p, int* n_in, int* out_cols) {
   if (!p || !p->finalized) return fail(B2S_ERR_STATE, "plan not finalized");
@@ -1733,7 +1734,7 @@ struct NvtxRange {  // one range per plan launch, named after the kernel family 
 
 static int launch_on(b2s_plan_t p, const void* d_rows, int64_t n_rows, int64_t stride, void* d_out, int32_t* d_status,
                      cudaStream_t st, bool host_rows = false) {
-  if (n_rows == 0) return B2S_OK;
+  if (n_rows == 0 && !p->comm) return B2S_OK;
   NvtxRange nvtx(p->dense_ok ? "b2s:dense_head" : p->t3_ok ? "b2s:trees3 (prep+walk+vote)"
                  : p->rt_ok ? "b2s:rowthread" : p->mode == MODE_STORE ? "b2s:rows_store" : "b2s:rows_kernel");
   KParams k = p->kp;
@@ -1772,6 +1773,12 @@ static int launch_on(b2s_plan_t p, const void* d_rows, int64_t n_rows, int64_t s
       k.sig.timeout_flag = c->timeout_flag();
       k.sig.timeout_ns = fused_timeout_ns;
       c->fused_epoch = k.sig.wait_epoch;
+    }
+    if (n_rows == 0) {  // an empty shard is still a step: publish this rank's flag
+      G.launches.fetch_add(1, std::memory_order_relaxed);
+      cudaError_t e = merge_step_launch(k.sig, st);
+      if (e != cudaSuccess) return fail(B2S_ERR_CUDA, "merge step launch failed: %s", cudaGetErrorString(e));
+      return B2S_OK;
     }
   }
   if (p->t3_ok) {

@@ -291,6 +291,13 @@ extern "C" int b2s_table_lookup_host(b2s_table_t t, const int64_t* keys, int64_t
   }
 }
 
+// A plan with merge targets or an attached communicator stores its votes there and never into the enrichment's output,
+// which would then hand out memory no kernel wrote: both entry points refuse it before anything is enqueued.
+static int refuse_merging(b2s_plan_t plan) {
+  if (!b2s_int_plan_merges(plan)) return B2S_OK;
+  return b2s_int_fail(B2S_ERR_UNSUPPORTED, "the plan stores its votes to merge targets or a communicator: enrich without them");
+}
+
 static int launch_fused(b2s_table_t t, b2s_plan_t plan, const int64_t* d_keys, int64_t n, void* d_out, int32_t* d_status, cudaStream_t st) {
   B2SGather g{};
   g.d_keys = reinterpret_cast<const long long*>(d_keys);
@@ -310,6 +317,7 @@ extern "C" int b2s_table_enrich_device(b2s_table_t t, b2s_plan_t plan, const int
     if (!t || !plan || !d_keys || !d_out || n < 0) return b2s_int_fail(B2S_ERR_INVALID, "bad arguments");
     if (misaligned(d_keys, 8) || misaligned(d_out, 4) || misaligned(d_status, 4))
       return b2s_int_fail(B2S_ERR_INVALID, "keys must be 8-byte aligned, out and status 4-byte aligned");
+    if (int rc = refuse_merging(plan)) return rc;
     if (n == 0) return B2S_OK;
     B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
     return launch_fused(t, plan, d_keys, n, d_out, d_status, stream ? (cudaStream_t)stream : b2s_int_stream());
@@ -333,6 +341,7 @@ extern "C" int b2s_table_enrich_host(b2s_table_t t, b2s_plan_t plan, const int64
     if (int rc = b2s_int_plan_shape(plan, &n_in, &out_cols)) return rc;
     if (n_in != t->n_feat) return b2s_int_fail(B2S_ERR_INVALID, "the table has %d features, the plan takes %d", t->n_feat, n_in);
     if (out_bytes < n * out_cols * 4) return b2s_int_fail(B2S_ERR_INVALID, "out buffer too small");
+    if (int rc = refuse_merging(plan)) return rc;
     if (n == 0) return B2S_OK;
     std::lock_guard<std::mutex> lk(t->mu);
     B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));

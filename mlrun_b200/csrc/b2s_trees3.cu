@@ -55,4 +55,13 @@ cudaError_t t3_launch_vote(const KParams& k, const double* partial, int64_t col_
   return cudaGetLastError();
 }
 
+// an empty shard stores nothing, but the rank still publishes its flag, so that its peers' waits see the step and its
+// epochs stay those of the other ranks (one CTA: it is the launch's last)
+__global__ void merge_step_kernel(const __grid_constant__ MergeSig sig) { merge_signal(sig); }
+
+cudaError_t merge_step_launch(const MergeSig& sig, cudaStream_t st) {
+  merge_step_kernel<<<1, 32, 0, st>>>(sig);
+  return cudaGetLastError();
+}
+
 }  // namespace b2s

@@ -95,6 +95,10 @@ cudaError_t t3_launch_prep(const T3Prep& pr, const CUtensorMap& tmap, bool miss,
 cudaError_t t3_launch_walk(const T3Params& t, int depth, bool miss, bool cat, int grid, int block, int smem, int smem_optin, cudaStream_t st);
 cudaError_t t3_launch_vote(const KParams& k, const double* partial, int64_t col_stride, const int32_t* col_score,
                            const int32_t* col_order, const int32_t* model_cols, const int32_t* row_bad, int grid, cudaStream_t st);
+// the step of an attached communicator whose shard has no rows (launch_on): one CTA publishes the step's flag and runs its
+// fused wait.  Compiled beside the vote kernel: a kernel more in the split-compiled b2s_runtime.cu changes what ptxas emits
+// for some row-thread instantiations
+cudaError_t merge_step_launch(const MergeSig& sig, cudaStream_t st);
 
 #ifdef B2S_T3_KERNELS
 // explicit shared-window loads (32-bit addresses: no generic->shared conversion in the address arithmetic)

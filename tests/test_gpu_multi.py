@@ -125,7 +125,8 @@ def check_one(server, names, batches, label, full, max_rows, fused):
 wl = flow3_workload(n_rows=10001, n_num=56, n_cat=8, seed=7, n_models=4)
 server = wl.build_server(api, engine="sync")
 rng = np.random.default_rng(5)
-check(server, wl.names, [wl.X, wl.X[rng.permutation(len(wl.X))[:7777]]], "flow3")
+# the 1-row batch leaves rank 1 an empty shard: it stores nothing but still takes the step
+check(server, wl.names, [wl.X, wl.X[rng.permutation(len(wl.X))[:7777]], wl.X[:1]], "flow3")
 
 # (b) BASELINE configs[3]: a router of 8 mixed linear / tree scorers over 64 raw features (tree parts kernel + vote kernel)
 from sklearn.ensemble import GradientBoostingRegressor
@@ -140,13 +141,49 @@ for i in range(8):
     graph.add_route(f"m{i}", class_name="SKLearnModelServer", model=m, model_path="")
 server8 = fn.to_mock_server(namespace={"SKLearnModelServer": api.SKLearnModelServer})
 X8 = frng.normal(size=(65536, 64)).astype(np.float32)
-check(server8, [f"f{i}" for i in range(64)], [X8, X8[:30011]], "router8")
+check(server8, [f"f{i}" for i in range(64)], [X8, X8[:30011], X8[:1]], "router8")
+
+# (c) the dense head (wgmma): one 16-class LogisticRegression, argmax in the epilogue's float32 fast path
+from sklearn.linear_model import LogisticRegression
+from mlrun_b200 import packing
+from mlrun_b200.lowering import ColumnProgram
+
+
+class PlanServer:
+    """a compiled plan behind the two calls ShardedGraphServer makes of a server; its single-GPU answer is b2s_run_device
+    on device rows (the kernel the shards run, whatever the batch size)"""
+
+    def __init__(self, plan):
+        self.plan = plan
+
+    def compile(self, names=None):
+        return self
+
+    def run_batch(self, X, names=None):
+        X = np.ascontiguousarray(X, dtype=np.float32)
+        d_in = nat.DeviceBuffer(X.nbytes).upload(X)
+        d_out = nat.DeviceBuffer(len(X) * self.plan.out_cols * 4)
+        self.plan.run_device(d_in.ptr, len(X), X.shape[1] * 4, d_out.ptr)
+        assert self.plan.last_kernel == "dense", self.plan.last_kernel
+        return d_out.download(self.plan.out_dtype, (len(X), self.plan.out_cols))
+
+
+drng = np.random.default_rng(3)
+centres = drng.normal(size=(16, 64)) * 1.5
+yd = drng.integers(0, 16, size=6000)
+logit = LogisticRegression(max_iter=300).fit((centres[yd] + drng.normal(size=(6000, 64))).astype(np.float32), yd * 3 + 5)
+dplan = ColumnProgram([f"f{i}" for i in range(64)]).build_plan([packing.pack_model(logit)])
+assert "dense_head_kernel" in dplan.kernel, dplan.kernel
+Xd = (centres[drng.integers(0, 16, size=20001)] + drng.normal(size=(20001, 64))).astype(np.float32)
+check(PlanServer(dplan), None, [Xd, Xd[:4321], Xd[:1]], "dense")
 dist.destroy_process_group()
 '''
 
 
 def test_sharded_graph_server_with_completion_flags(tmp_path):
-    """the product API of the sharded router: no barrier, no collective -- readers wait on the per-rank completion flags"""
+    """the product API of the sharded router: no barrier, no collective -- readers wait on the per-rank completion flags.
+    The row-thread, trees3 and dense-head plans, merged rows bit-equal to the single-GPU answer, a 1-row batch among
+    them (rank 1's shard empty)"""
     import torch
 
     if torch.cuda.device_count() < 2:
@@ -158,6 +195,6 @@ def test_sharded_graph_server_with_completion_flags(tmp_path):
          "--master-port", "29622", str(script)],
         capture_output=True, text=True, env=dict(os.environ, REPO_ROOT=ROOT), timeout=600)
     assert out.returncode == 0, out.stdout[-3000:] + out.stderr[-3000:]
-    for label in ("flow3", "router8"):
+    for label in ("flow3", "router8", "dense"):
         for r in range(2):
             assert f"[{label} ok on rank {r}]" in out.stdout, out.stdout[-2000:]

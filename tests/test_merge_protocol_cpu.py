@@ -8,13 +8,20 @@ as a randomly scheduled model: N ranks, every rank's stream is a sequence of
 
 The checks are the two claims DESIGN.md section 7 makes for four slots and lag <= 1: every read sees every rank's block of
 exactly its step (no rank is ever more than SLOTS - 1 steps ahead of a reader), and the schedule never deadlocks.  With two
-slots the same schedule does let a fast rank overwrite a block a slow reader has not read: the model must catch that."""
+slots the same schedule does let a fast rank overwrite a block a slow reader has not read: the model must catch that.
+
+A rank whose shard of a step is empty (a batch of fewer rows than ranks, mlrun_b200.sharding.shard_bounds) stores nothing
+but still publishes the step's flag: its block of that step is not part of the response, and nobody waits for rows."""
 import random
 
 import pytest
 
+from mlrun_b200.sharding import shard_bounds
 
-def simulate(world, steps, slots, lag, seed):
+
+def simulate(world, steps, slots, lag, seed, empty=frozenset(), skip=False):
+    """empty: the (rank, step) pairs whose shard has no rows.  Such a rank stores nothing in that step and publishes its
+    flag; skip=True instead lets it take no step at all (no flag, and every later launch of it one epoch lower)"""
     rnd = random.Random(seed)
     flags = [[0] * world for _ in range(world)]           # flags[target][source]
     merged = [[[0] * world for _ in range(slots)] for _ in range(world)]  # merged[target][slot][source] = step stored
@@ -22,14 +29,19 @@ def simulate(world, steps, slots, lag, seed):
     prog = []
     for me in range(world):
         ops = []
-        for e in range(1, steps + 1):
+        e = 0  # this rank's epoch
+        for step in range(1, steps + 1):
+            if skip and (me, step) in empty:
+                continue
+            e += 1
             targets = [(me + 1 + g) % world for g in range(world)]  # right-hand neighbour first, as the launch wiring does
-            ops += [("store", t, e) for t in targets]
+            if (me, step) not in empty:
+                ops += [("store", t, e) for t in targets]
             ops += [("flag", t, e) for t in targets]
             if e > lag:
                 ops.append(("wait", e - lag))
                 ops.append(("read", e - lag))
-        for w in range(max(steps - lag + 1, 1), steps + 1):  # drain: the last `lag` steps
+        for w in range(max(e - lag + 1, 1), e + 1):  # drain: the last `lag` steps
             ops.append(("wait", w))
             ops.append(("read", w))
         prog.append(ops)
@@ -56,7 +68,7 @@ def simulate(world, steps, slots, lag, seed):
                     break  # still polling
             else:  # read
                 got = merged[r][op[1] % slots]
-                if any(v != op[1] for v in got):
+                if any(v != op[1] for src, v in enumerate(got) if (src, op[1]) not in empty):
                     torn.append((r, op[1], list(got)))
             pc[r] += 1
             progressed = True
@@ -85,3 +97,34 @@ def test_the_model_catches_too_few_slots(slots):
         caught += bool(torn)
         assert not simulate(8, steps=24, slots=slots, lag=0, seed=seed)[1]
     assert caught == 20
+
+
+def empty_shards(world, steps, seed):
+    """(rank, step) pairs left empty by shard_bounds when about a third of the batches have fewer rows than ranks"""
+    rnd = random.Random(seed)
+    empty = set()
+    for step in range(1, steps + 1):
+        n = rnd.randrange(world) if rnd.random() < 0.35 else rnd.randrange(world, 4 * world)
+        empty |= {(r, step) for r in range(world) if shard_bounds(n, r, world)[0] == shard_bounds(n, r, world)[1]}
+    return empty
+
+
+@pytest.mark.parametrize("world", [2, 4, 8])
+@pytest.mark.parametrize("lag", [0, 1])
+def test_empty_shards_publish_their_flags_and_never_tear_or_deadlock(world, lag):
+    """batches of fewer rows than ranks (0 rows included) among ordinary ones: every rank still takes every step"""
+    for seed in range(40):
+        empty = empty_shards(world, 24, seed)
+        assert any(r == world - 1 for r, _ in empty)
+        state, torn = simulate(world, steps=24, slots=4, lag=lag, seed=seed, empty=empty)
+        assert state == "done" and not torn, (seed, state, torn[:2])
+
+
+@pytest.mark.parametrize("world", [2, 4, 8])
+@pytest.mark.parametrize("lag", [0, 1])
+def test_a_rank_that_skips_its_empty_step_deadlocks_the_schedule(world, lag):
+    """a rank that launches nothing for an empty shard publishes no flag for it, and its later epochs lag one behind the
+    other ranks': they wait for its last step for ever (on the device, until B2S_COMM_TIMEOUT_MS)"""
+    for seed in range(3):
+        state, _ = simulate(world, steps=24, slots=4, lag=lag, seed=seed, empty={(world - 1, 5)}, skip=True)
+        assert state == "deadlock", seed
