@@ -432,6 +432,34 @@ int b2s_table_time_device(b2s_table_t table, const int64_t* const* d_keys, int32
 /* 64-bit FNV-1a of each string of a packed buffer (string i = bytes[offsets[i] .. offsets[i+1])): the key of a
  * string-valued entity.  Host code. */
 int b2s_hash_strings(const char* bytes, const int64_t* offsets, int64_t n, int64_t* keys_out);
+/* The online table built from columns in memory of the library's device; nothing but the counters and the key of a
+ * duplicate crosses to the host.  b2s_table_create_device builds what b2s_table_create builds from the same keys and the
+ * same values as float32 (the same capacity, the NaN row, the padded impute vector), so every lookup and enrichment call
+ * serves it alike; slot positions may differ, since keys are inserted concurrently.  Feature column c is n_keys values of
+ * cols[c] (FLOAT 4 / 8 bytes, INT and UINT 1 / 2 / 4 / 8, BOOL 1), converted as numpy's astype(float32) converts them:
+ * round to nearest even, overflow to +-inf, bool to 0 / 1.  Three launches: pack the rows, insert the keys (atomicCAS on
+ * the slot's row word), check for duplicates.  A repeated key is B2S_ERR_INVALID with b2s_table_create's message (the
+ * key, the first row that repeats an earlier key, and that row).  B2S_ERR_INVALID before any launch for n_keys outside
+ * 1 .. 2^31 - 1, a bad kind or width, or keys / columns that are null, misaligned or not on the library's device. */
+enum { B2S_TCOL_FLOAT = 0, B2S_TCOL_INT = 1, B2S_TCOL_UINT = 2, B2S_TCOL_BOOL = 3 };
+typedef struct b2s_table_col {
+  const void* src;
+  int32_t bytes;
+  int32_t kind; /* B2S_TCOL_* */
+} b2s_table_col;
+int b2s_table_create_device(const int64_t* d_keys, int64_t n_keys, const b2s_table_col* cols, int32_t n_features,
+                            const float* impute, b2s_table_t* out);
+/* Feature statistics of n rows of such columns (as float32), over the finite values: stats_out (host, [5][n_features]
+ * float32) gets mean, min, max, std (ddof 1) and count, accumulated in float64 and rounded to float32; NaN where a column
+ * has no finite value (std: fewer than two).  Three launches; returns when stats_out is filled. */
+int b2s_table_stats_device(const b2s_table_col* cols, int32_t n_features, int64_t n, float* stats_out, void* stream);
+/* The keys of the rows whose label is truthy (not NaN and not zero), compacted on the device and copied to keys_out
+ * (host, room for n) in no particular order; *n_out gets their number.  One launch; returns when they are there. */
+int b2s_table_label_keys_device(const int64_t* d_keys, int64_t n, const b2s_table_col* label, int64_t* keys_out, int64_t* n_out,
+                                void* stream);
+/* status[i] |= B2S_ROW_UNKNOWN_KEY where found[i] is 0: b2s_table_lookup_device + b2s_run_device + this give the status
+ * words b2s_table_enrich_device gives.  One launch, asynchronous. */
+int b2s_table_mark_unknown_device(const int32_t* d_found, int32_t* d_status, int64_t n, void* stream);
 
 /* ---- point-in-time training sets: as-of joins of entity rows onto feature-set indexes ---------------------------
  * get_offline_features on the local engine (feature_store/retrieval/base.py:412-468, local_merger.py:29-81) merges
@@ -655,6 +683,11 @@ typedef struct b2s_key_col {
   int32_t is_signed;
 } b2s_key_col;
 int b2s_keys_encode_device(const b2s_key_col* cols, int32_t n_cols, int64_t n, int64_t* d_keys, void* stream);
+/* b2s_keys_hash_decimal_device: the online table's key of a composite entity, in one launch: FNV-1a (b2s_hash_strings) of
+ * the decimal text of each row's values joined by '.', as Python's ".".join(str(v) for v in row), without materialising
+ * the text.  1 .. 16 signed int columns of 1, 2, 4 or 8 bytes.  B2S_ERR_INVALID before any launch for other columns, or
+ * columns / d_keys that are null (n > 0), misaligned or not on the library's device. */
+int b2s_keys_hash_decimal_device(const b2s_key_col* cols, int32_t n_cols, int64_t n, int64_t* d_keys, void* stream);
 /* b2s_ts_profile_device: one launch over n int64 nanosecond timestamps in memory of the library's device; counts (host,
  * 4) gets the NaT (INT64_MIN) values and the other values that are not whole multiples of 10^3, 10^6 and 10^9, in one
  * small copy: the call returns when they are there.  n = 0: zeros, no launch.  B2S_ERR_INVALID before any launch for

@@ -110,6 +110,14 @@ class KeyCol(C.Structure):
     _fields_ = [("src", _vp), ("bytes", _i32), ("is_signed", _i32)]
 
 
+# B2S_TCOL_* kinds of b2s_table_col
+TCOL_FLOAT, TCOL_INT, TCOL_UINT, TCOL_BOOL = 0, 1, 2, 3
+
+
+class TableCol(C.Structure):
+    _fields_ = [("src", _vp), ("bytes", _i32), ("kind", _i32)]
+
+
 # name -> (restype, argtypes); the single source of truth for the exported surface
 SIGNATURES = {
     "b2s_version": (C.c_int, []),
@@ -190,6 +198,10 @@ SIGNATURES = {
     "b2s_table_enrich_host": (C.c_int, [_vp, _vp, C.POINTER(_i64), _i64, _vp, _i64, _pi32, C.POINTER(Stats)]),
     "b2s_table_time_device": (C.c_int, [_vp, C.POINTER(_vp), _i32, _i64, _vp, _i64, _vp, _i32, _pf32]),
     "b2s_hash_strings": (C.c_int, [C.c_char_p, C.POINTER(_i64), _i64, C.POINTER(_i64)]),
+    "b2s_table_create_device": (C.c_int, [_vp, _i64, C.POINTER(TableCol), _i32, _pf32, C.POINTER(_vp)]),
+    "b2s_table_stats_device": (C.c_int, [C.POINTER(TableCol), _i32, _i64, _pf32, _vp]),
+    "b2s_table_label_keys_device": (C.c_int, [_vp, _i64, C.POINTER(TableCol), C.POINTER(_i64), C.POINTER(_i64), _vp]),
+    "b2s_table_mark_unknown_device": (C.c_int, [_vp, _vp, _i64, _vp]),
     # point-in-time (as-of) joins
     "b2s_pit_index_create": (C.c_int, [_vp, _vp, _i64, C.POINTER(_vp), _pi32, _i32, C.POINTER(_vp)]),
     "b2s_pit_index_create_device": (C.c_int, [_vp, _vp, _i64, C.POINTER(_vp), _pi32, _i32, C.POINTER(_vp)]),
@@ -221,6 +233,7 @@ SIGNATURES = {
     "b2s_pointer_device": (C.c_int, [_vp, _pi32]),
     "b2s_cols_convert_device": (C.c_int, [C.POINTER(Convert), _i32, _i64, _vp, _i32, _vp]),
     "b2s_keys_encode_device": (C.c_int, [C.POINTER(KeyCol), _i32, _i64, _vp, _vp]),
+    "b2s_keys_hash_decimal_device": (C.c_int, [C.POINTER(KeyCol), _i32, _i64, _vp, _vp]),
     "b2s_ts_profile_device": (C.c_int, [_vp, _i64, C.POINTER(_i64), _vp]),
     # windowed aggregations
     "b2s_agg_run_device": (C.c_int, [_vp, _vp, _i64, C.POINTER(AggSpec), _i32, _vp, _vp]),

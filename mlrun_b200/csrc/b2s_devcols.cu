@@ -84,6 +84,46 @@ __global__ void __launch_bounds__(kThreads) keys_kernel(KeyCol hi, KeyCol lo, in
   }
 }
 
+constexpr int kMaxDecimalCols = 16;
+
+struct DecimalCols {
+  KeyCol c[kMaxDecimalCols];
+  int n;
+};
+
+__device__ __forceinline__ uint64_t fnv_byte(uint64_t h, unsigned b) { return (h ^ b) * 1099511628211ULL; }
+
+// FNV-1a folded over the decimal text of v, most significant digit first.  The magnitude is taken in uint64 (2^63 for
+// INT64_MIN, which has no int64 negation); it has at most 19 digits, so p never passes 10^18.
+__device__ __forceinline__ uint64_t fnv_decimal(uint64_t h, int64_t v) {
+  uint64_t u = (uint64_t)v;
+  if (v < 0) {
+    h = fnv_byte(h, '-');
+    u = 0ull - u;
+  }
+  uint64_t p = 1;
+  while (u / p >= 10) p *= 10;
+  for (;;) {
+    const uint64_t d = u / p;
+    h = fnv_byte(h, (unsigned)('0' + d));
+    u -= d * p;
+    if (p == 1) return h;
+    p /= 10;
+  }
+}
+
+// online.py _encode_keys of a composite key: FNV-1a of ".".join(str(v) for v in row)
+__global__ void __launch_bounds__(kThreads) keys_decimal_kernel(const __grid_constant__ DecimalCols cols, int64_t n, int64_t* __restrict__ keys) {
+  for (int64_t i = (int64_t)blockIdx.x * kThreads + threadIdx.x; i < n; i += (int64_t)gridDim.x * kThreads) {
+    uint64_t h = 1469598103934665603ULL;
+    for (int c = 0; c < cols.n; ++c) {
+      if (c) h = fnv_byte(h, '.');
+      h = fnv_decimal(h, key_word(cols.c[c], i));
+    }
+    keys[i] = (int64_t)h;
+  }
+}
+
 // counts[0]: NaT (INT64_MIN) values; counts[1..3]: the other values that are not whole multiples of 10^3, 10^6, 10^9 ns.
 // A zero remainder means the same in C (truncated) and numpy (floored) division, so negative timestamps count alike.
 __global__ void __launch_bounds__(kThreads) ts_profile_kernel(const int64_t* __restrict__ ts, int64_t n, unsigned long long* __restrict__ counts) {
@@ -224,6 +264,37 @@ extern "C" int b2s_keys_encode_device(const b2s_key_col* cols, int32_t n_cols, i
     launches.add(1);
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return b2s_int_fail(B2S_ERR_CUDA, "keys launch failed: %s", cudaGetErrorString(e));
+    return B2S_OK;
+  } catch (const std::exception& e) {
+    return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
+  }
+}
+
+extern "C" int b2s_keys_hash_decimal_device(const b2s_key_col* cols, int32_t n_cols, int64_t n, int64_t* d_keys, void* stream) {
+  try {  // no C++ exception crosses the C boundary
+    if (n < 0 || !cols || n_cols < 1 || n_cols > kMaxDecimalCols)
+      return b2s_int_fail(B2S_ERR_INVALID, "n >= 0 and 1 .. %d key columns", kMaxDecimalCols);
+    DecimalCols dc{};
+    dc.n = n_cols;
+    for (int c = 0; c < n_cols; ++c) {
+      const b2s_key_col& k = cols[c];
+      if (!k.is_signed || (k.bytes != 1 && k.bytes != 2 && k.bytes != 4 && k.bytes != 8))
+        return b2s_int_fail(B2S_ERR_INVALID, "key column %d: %d bytes %s is not a signed int column", c, k.bytes, k.is_signed ? "signed" : "unsigned");
+      if (n && !k.src) return b2s_int_fail(B2S_ERR_INVALID, "key column %d: null", c);
+      dc.c[c] = KeyCol{k.src, k.bytes, 1};
+    }
+    if (n && !d_keys) return b2s_int_fail(B2S_ERR_INVALID, "d_keys: null");
+    if (n == 0) return B2S_OK;
+    if (int rc = device_ready()) return rc;
+    for (int c = 0; c < n_cols; ++c)
+      if (int rc = check_on_device(cols[c].src, cols[c].bytes, "key column", c)) return rc;
+    if (int rc = check_on_device(d_keys, 8, "d_keys", 0)) return rc;
+    cudaStream_t st = stream ? (cudaStream_t)stream : b2s_int_stream();
+    Launches launches;
+    keys_decimal_kernel<<<grid_for(n, kThreads), kThreads, 0, st>>>(dc, n, d_keys);
+    launches.add(1);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return b2s_int_fail(B2S_ERR_CUDA, "decimal keys launch failed: %s", cudaGetErrorString(e));
     return B2S_OK;
   } catch (const std::exception& e) {
     return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());

@@ -253,17 +253,6 @@ static int check_index_args(const int64_t* keys, const int64_t* ts_ns, int64_t n
   return B2S_OK;
 }
 
-// B2S_ERR_INVALID unless p is device memory of the library's device, aligned to `align` bytes
-static int check_on_device(const void* p, int align, const char* what, int i) {
-  if (misaligned(p, align)) return b2s_int_fail(B2S_ERR_INVALID, "%s %d: not %d-byte aligned", what, i, align);
-  int32_t dev = -1;
-  if (int rc = b2s_pointer_device(p, &dev)) return rc;
-  if (dev != b2s_int_device())
-    return b2s_int_fail(B2S_ERR_INVALID, "%s %d: %s, not memory of the library's device %d", what, i, dev < 0 ? "host memory" : "another device's memory",
-                        b2s_int_device());
-  return B2S_OK;
-}
-
 using IndexBuild = int (*)(b2s_pit_s*, const int64_t*, const int64_t*, int64_t, const void* const*, const int32_t*, int32_t, cudaStream_t);
 
 static int index_create(IndexBuild build, const int64_t* keys, const int64_t* ts_ns, int64_t n_rows, const void* const* cols,

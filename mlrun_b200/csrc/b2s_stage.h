@@ -31,6 +31,17 @@ struct SyncOnExit {
   ~SyncOnExit() { cudaStreamSynchronize(st); }
 };
 
+// B2S_ERR_INVALID unless p is device memory of the library's device, aligned to `align` bytes
+inline int check_on_device(const void* p, int align, const char* what, int i) {
+  if (misaligned(p, align)) return b2s_int_fail(B2S_ERR_INVALID, "%s %d: not %d-byte aligned", what, i, align);
+  int32_t dev = -1;
+  if (int rc = b2s_pointer_device(p, &dev)) return rc;
+  if (dev != b2s_int_device())
+    return b2s_int_fail(B2S_ERR_INVALID, "%s %d: %s, not memory of the library's device %d", what, i, dev < 0 ? "host memory" : "another device's memory",
+                        b2s_int_device());
+  return B2S_OK;
+}
+
 // CUDA events, destroyed when the array leaves scope.
 class Events {
  public:

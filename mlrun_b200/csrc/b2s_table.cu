@@ -24,6 +24,7 @@
 #include "../../include/b200serve.h"
 #include "b2s_internal.h"
 #include "b2s_hash.cuh"
+#include "b2s_stage.h"
 
 namespace {
 
@@ -154,6 +155,26 @@ struct b2s_table_s {
   char* h_pin = nullptr;
 };
 
+// what both builds do once the slots and values are in place: the padded impute vector (NaN: keep the stored value),
+// the lookup grid and the events of the host calls
+static int table_finish(b2s_table_s* t, const float* impute) {
+  const int n_features = t->n_feat;
+  std::vector<float> imp(((size_t)n_features + 3) / 4 * 4, NAN);
+  if (impute)
+    for (int c = 0; c < n_features; ++c) {
+      imp[c] = impute[c];
+      if (impute[c] == impute[c]) t->any_impute = 1;
+    }
+  t->h_impute = imp;
+  B2S_CUDA_TRY(cudaMalloc(&t->d_impute, imp.size() * 4));
+  B2S_CUDA_TRY(cudaMemcpy(t->d_impute, imp.data(), imp.size() * 4, cudaMemcpyHostToDevice));
+  int occ = 0;
+  B2S_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, table_lookup_kernel, 256, 0));
+  t->grid = b2s_int_sm_count() * std::max(occ, 1);
+  for (int i = 0; i < 4; ++i) B2S_CUDA_TRY(cudaEventCreate(&t->ev[i]));
+  return B2S_OK;
+}
+
 extern "C" int b2s_table_create(const int64_t* keys, int64_t n_keys, const float* values, int32_t n_features, const float* impute,
                                 b2s_table_t* out) {
   try {  // no C++ exception crosses the C boundary
@@ -184,19 +205,7 @@ extern "C" int b2s_table_create(const int64_t* keys, int64_t n_keys, const float
       const std::vector<float> nan_row((size_t)n_features, NAN);
       B2S_CUDA_TRY(cudaMemcpy(t->d_values + (size_t)n_keys * n_features, nan_row.data(), (size_t)n_features * 4, cudaMemcpyHostToDevice));
     }
-    std::vector<float> imp(((size_t)n_features + 3) / 4 * 4, NAN);
-    if (impute)
-      for (int c = 0; c < n_features; ++c) {
-        imp[c] = impute[c];
-        if (impute[c] == impute[c]) t->any_impute = 1;
-      }
-    t->h_impute = imp;
-    B2S_CUDA_TRY(cudaMalloc(&t->d_impute, imp.size() * 4));
-    B2S_CUDA_TRY(cudaMemcpy(t->d_impute, imp.data(), imp.size() * 4, cudaMemcpyHostToDevice));
-    int occ = 0;
-    B2S_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, table_lookup_kernel, 256, 0));
-    t->grid = b2s_int_sm_count() * std::max(occ, 1);
-    for (int i = 0; i < 4; ++i) B2S_CUDA_TRY(cudaEventCreate(&t->ev[i]));
+    if (int rc = table_finish(t, impute)) return rc;
     *out = t;
     return B2S_OK;
   } catch (const std::exception& e) {
@@ -484,6 +493,436 @@ extern "C" int b2s_hash_strings(const char* bytes, const int64_t* offsets, int64
       keys_out[i] = (int64_t)h;
     }
     return B2S_OK;
+  } catch (const std::exception& e) {
+    return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
+  }
+}
+
+// ---- the online table built from device columns --------------------------------------------------------------------------
+// A vector's online rows that already live in HBM (CUDA columns, a device ingest's result) become a table without a host
+// round trip: table_pack_kernel writes the row-major float32 values, table_insert_kernel claims one slot per key,
+// table_check_kernel finds repeated keys; the statistics of the impute policy and the keys of truthy labels are reduced and
+// compacted where the columns are.
+namespace {
+
+struct TCol {
+  const void* src;
+  int32_t bytes;
+  int32_t kind;
+};
+
+constexpr int kTableThreads = 256;
+constexpr unsigned kNaN32 = 0x7fc00000u;  // the NaN numpy writes
+
+// the value of row i as numpy's astype(float32) gives it (round to nearest even, overflow to +-inf, bool to 0 / 1; a
+// float64 NaN keeps its sign and the top of its payload, quieted, as x86's conversion keeps them)
+__device__ __forceinline__ float col_f32(const TCol& c, int64_t i) {
+  switch (c.kind) {
+    case B2S_TCOL_FLOAT:
+      if (c.bytes == 4) return static_cast<const float*>(c.src)[i];
+      {
+        const double d = static_cast<const double*>(c.src)[i];
+        if (d != d) {
+          const unsigned long long b = (unsigned long long)__double_as_longlong(d);
+          return __uint_as_float((unsigned)(b >> 32 & 0x80000000u) | kNaN32 | (unsigned)(b >> 29 & 0x3fffffu));
+        }
+        return __double2float_rn(d);
+      }
+    case B2S_TCOL_INT:
+      switch (c.bytes) {
+        case 1: return (float)static_cast<const int8_t*>(c.src)[i];
+        case 2: return (float)static_cast<const int16_t*>(c.src)[i];
+        case 4: return __int2float_rn(static_cast<const int32_t*>(c.src)[i]);
+        default: return __ll2float_rn(static_cast<const long long*>(c.src)[i]);
+      }
+    case B2S_TCOL_UINT:
+      switch (c.bytes) {
+        case 1: return (float)static_cast<const uint8_t*>(c.src)[i];
+        case 2: return (float)static_cast<const uint16_t*>(c.src)[i];
+        case 4: return __uint2float_rn(static_cast<const uint32_t*>(c.src)[i]);
+        default: return __ull2float_rn(static_cast<const unsigned long long*>(c.src)[i]);
+      }
+    default: return static_cast<const uint8_t*>(c.src)[i] ? 1.f : 0.f;
+  }
+}
+
+// values[r][c] = column c at row r, through a 32 x 32 shared tile: loads run down each column, stores along each row.
+// blockIdx.y is the tile of 32 columns; the blocks of x = 0 also write row n, all NaN (the unknown key's row).
+__global__ void __launch_bounds__(kTableThreads) table_pack_kernel(const TCol* __restrict__ cols, int32_t n_feat, int64_t n,
+                                                                    float* __restrict__ values) {
+  __shared__ float tile[32][33];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int c0 = blockIdx.y * 32;
+  const int cw = min(32, n_feat - c0);
+  if (blockIdx.x == 0 && (int)threadIdx.x < cw) values[n * n_feat + c0 + threadIdx.x] = __uint_as_float(kNaN32);
+  for (int64_t r0 = (int64_t)blockIdx.x * 32; r0 < n; r0 += (int64_t)gridDim.x * 32) {
+    for (int c = warp; c < cw; c += kTableThreads / 32) {
+      const TCol col = cols[c0 + c];
+      if (r0 + lane < n) tile[c][lane] = col_f32(col, r0 + lane);
+    }
+    __syncthreads();
+    for (int r = warp; r < 32 && r0 + r < n; r += kTableThreads / 32)
+      if (lane < cw) values[(r0 + r) * n_feat + c0 + lane] = tile[lane][r];
+    __syncthreads();
+  }
+}
+
+// one thread per key claims the first free slot of its walk (the row word goes from -1 to the row, then the key is
+// stored): a repeated key takes a slot of its own, which table_check_kernel finds
+__global__ void __launch_bounds__(kTableThreads) table_insert_kernel(const int64_t* __restrict__ keys, int64_t n, Slot* slots, uint64_t mask) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const long long k = keys[i];
+    uint64_t h = mix64((uint64_t)k) & mask;
+    for (;;) {
+      unsigned long long* rw = reinterpret_cast<unsigned long long*>(&slots[h].row);
+      if (atomicCAS(rw, ~0ull, (unsigned long long)i) == ~0ull) {
+        slots[h].key = k;
+        break;
+      }
+      h = (h + 1) & mask;
+    }
+  }
+}
+
+// Every row of a key lies on that key's walk, before its first empty slot.  Row i repeats an earlier row when the walk
+// shows the key at a smaller row; *dup = min over such i of (i << 32 | the key's first row): b2s_table_create stops at
+// the first row that repeats a key and names the row it repeats, the key's first.
+__global__ void __launch_bounds__(kTableThreads) table_check_kernel(const int64_t* __restrict__ keys, int64_t n, const Slot* __restrict__ slots,
+                                                                     uint64_t mask, unsigned long long* __restrict__ dup) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const long long k = keys[i];
+    uint64_t h = mix64((uint64_t)k) & mask;
+    long long first = i;
+    for (;;) {
+      const longlong2 s = __ldg(reinterpret_cast<const longlong2*>(slots) + h);
+      if (s.y < 0) break;
+      if (s.x == k && s.y < first) first = s.y;
+      h = (h + 1) & mask;
+    }
+    if (first < i) atomicMin(dup, ((unsigned long long)i << 32) | (unsigned long long)first);
+  }
+}
+
+struct StatPart {
+  double sum;
+  long long count;
+  float min, max;
+};
+
+// the block's sum of v (fixed order: lanes by shuffle, then warps by thread 0); valid in thread 0
+template <class T, class Op>
+__device__ __forceinline__ T block_reduce(T v, Op op, T* smem) {
+  for (int o = 16; o; o >>= 1) v = op(v, __shfl_down_sync(0xffffffffu, v, o));
+  if ((threadIdx.x & 31) == 0) smem[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x == 0)
+    for (int w = 1; w < kTableThreads / 32; ++w) v = op(v, smem[w]);
+  __syncthreads();
+  return v;
+}
+
+__device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
+
+// pass 1, blockIdx.y the column: count, sum (float64), min and max of the finite values, one partial per block
+__global__ void __launch_bounds__(kTableThreads) table_stats_sum_kernel(const TCol* __restrict__ cols, int64_t n, StatPart* __restrict__ part) {
+  __shared__ double s_d[kTableThreads / 32];
+  __shared__ long long s_c[kTableThreads / 32];
+  __shared__ float s_f[kTableThreads / 32];
+  const TCol col = cols[blockIdx.y];
+  double sum = 0.0;
+  long long count = 0;
+  float mn = INFINITY, mx = -INFINITY;
+  for (int64_t i = (int64_t)blockIdx.x * kTableThreads + threadIdx.x; i < n; i += (int64_t)gridDim.x * kTableThreads) {
+    const float v = col_f32(col, i);
+    if (fabsf(v) <= 3.402823466e38f) {
+      sum = __dadd_rn(sum, (double)v);
+      ++count;
+      mn = fminf(mn, v);
+      mx = fmaxf(mx, v);
+    }
+  }
+  sum = block_reduce(sum, dadd, s_d);
+  count = block_reduce(count, [](long long a, long long b) { return a + b; }, s_c);
+  mn = block_reduce(mn, [](float a, float b) { return fminf(a, b); }, s_f);
+  mx = block_reduce(mx, [](float a, float b) { return fmaxf(a, b); }, s_f);
+  if (threadIdx.x == 0) part[(int64_t)blockIdx.y * gridDim.x + blockIdx.x] = StatPart{sum, count, mn, mx};
+}
+
+// the column's mean from its pass-1 partials, summed in block order (every caller gets the same bits)
+__device__ __forceinline__ double column_mean(const StatPart* part, int nb, int c) {
+  double sum = 0.0;
+  long long count = 0;
+  for (int b = 0; b < nb; ++b) {
+    sum = __dadd_rn(sum, part[(int64_t)c * nb + b].sum);
+    count += part[(int64_t)c * nb + b].count;
+  }
+  return __ddiv_rn(sum, (double)count);
+}
+
+// pass 2: the sum of squared deviations from the mean, one partial per block (numpy's nanvar: subtract, multiply, sum)
+__global__ void __launch_bounds__(kTableThreads) table_stats_sq_kernel(const TCol* __restrict__ cols, int64_t n, const StatPart* __restrict__ part,
+                                                                        double* __restrict__ sq) {
+  __shared__ double s_d[kTableThreads / 32];
+  __shared__ double s_mean;
+  if (threadIdx.x == 0) s_mean = column_mean(part, gridDim.x, blockIdx.y);
+  __syncthreads();
+  const double mean = s_mean;
+  const TCol col = cols[blockIdx.y];
+  double ss = 0.0;
+  for (int64_t i = (int64_t)blockIdx.x * kTableThreads + threadIdx.x; i < n; i += (int64_t)gridDim.x * kTableThreads) {
+    const float v = col_f32(col, i);
+    if (fabsf(v) <= 3.402823466e38f) {
+      const double d = __dsub_rn((double)v, mean);
+      ss = __dadd_rn(ss, __dmul_rn(d, d));
+    }
+  }
+  ss = block_reduce(ss, dadd, s_d);
+  if (threadIdx.x == 0) sq[(int64_t)blockIdx.y * gridDim.x + blockIdx.x] = ss;
+}
+
+// one thread per column: out[5][n_feat] = mean, min, max, std (ddof 1), count, rounded to float32
+__global__ void table_stats_finish_kernel(const StatPart* __restrict__ part, const double* __restrict__ sq, int nb, int32_t n_feat,
+                                          float* __restrict__ out) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= n_feat) return;
+  long long count = 0;
+  float mn = INFINITY, mx = -INFINITY;
+  double ss = 0.0;
+  for (int b = 0; b < nb; ++b) {
+    const StatPart p = part[(int64_t)c * nb + b];
+    count += p.count;
+    mn = fminf(mn, p.min);
+    mx = fmaxf(mx, p.max);
+    ss = __dadd_rn(ss, sq[(int64_t)c * nb + b]);
+  }
+  const float nan = __uint_as_float(kNaN32);
+  out[c] = count ? __double2float_rn(column_mean(part, nb, c)) : nan;
+  out[n_feat + c] = count ? mn : nan;
+  out[2 * n_feat + c] = count ? mx : nan;
+  out[3 * n_feat + c] = count > 1 ? __double2float_rn(__dsqrt_rn(__ddiv_rn(ss, (double)(count - 1)))) : nan;
+  out[4 * n_feat + c] = (float)count;
+}
+
+// `notna(label) & bool(label)`
+__device__ __forceinline__ bool truthy(const TCol& c, int64_t i) {
+  if (c.kind == B2S_TCOL_FLOAT) {
+    const double v = c.bytes == 4 ? (double)static_cast<const float*>(c.src)[i] : static_cast<const double*>(c.src)[i];
+    return v == v && v != 0.0;
+  }
+  switch (c.bytes) {
+    case 1: return static_cast<const uint8_t*>(c.src)[i] != 0;
+    case 2: return static_cast<const uint16_t*>(c.src)[i] != 0;
+    case 4: return static_cast<const uint32_t*>(c.src)[i] != 0;
+    default: return static_cast<const unsigned long long*>(c.src)[i] != 0;
+  }
+}
+
+// keys of the truthy rows, appended warp by warp (one atomicAdd per warp)
+__global__ void __launch_bounds__(kTableThreads) table_label_keys_kernel(const int64_t* __restrict__ keys, int64_t n, const TCol label,
+                                                                          int64_t* __restrict__ out, unsigned long long* __restrict__ count) {
+  const int lane = threadIdx.x & 31;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i - lane < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const bool t = i < n && truthy(label, i);
+    const unsigned m = __ballot_sync(0xffffffffu, t);
+    unsigned long long base = 0;
+    if (lane == 0 && m) base = atomicAdd(count, (unsigned long long)__popc(m));
+    base = __shfl_sync(0xffffffffu, base, 0);
+    if (t) out[base + __popc(m & ((1u << lane) - 1u))] = keys[i];
+  }
+}
+
+int check_tcols(const b2s_table_col* cols, int32_t n_cols, int64_t n, std::vector<TCol>& dev) {
+  dev.resize(n_cols);
+  for (int c = 0; c < n_cols; ++c) {
+    const b2s_table_col& k = cols[c];
+    const bool ok = k.kind == B2S_TCOL_FLOAT ? (k.bytes == 4 || k.bytes == 8)
+                    : k.kind == B2S_TCOL_BOOL ? k.bytes == 1
+                    : (k.kind == B2S_TCOL_INT || k.kind == B2S_TCOL_UINT) && (k.bytes == 1 || k.bytes == 2 || k.bytes == 4 || k.bytes == 8);
+    if (!ok) return b2s_int_fail(B2S_ERR_INVALID, "column %d: kind %d of %d bytes is not a column kind", c, k.kind, k.bytes);
+    if (n && !k.src) return b2s_int_fail(B2S_ERR_INVALID, "column %d: null", c);
+    dev[c] = TCol{k.src, k.bytes, k.kind};
+  }
+  return B2S_OK;
+}
+
+int check_tcols_on_device(const std::vector<TCol>& cols) {
+  for (size_t c = 0; c < cols.size(); ++c)
+    if (int rc = check_on_device(cols[c].src, cols[c].bytes, "column", (int)c)) return rc;
+  return B2S_OK;
+}
+
+int table_device_ready() {
+  if (!b2s_int_inited()) return b2s_int_fail(B2S_ERR_STATE, "b2s_init was not called (no CUDA device: there is no CPU fallback)");
+  B2S_CUDA_TRY(cudaSetDevice(b2s_int_device()));
+  return B2S_OK;
+}
+
+int launched(const char* what) {
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return b2s_int_fail(B2S_ERR_CUDA, "%s launch failed: %s", what, cudaGetErrorString(e));
+  return B2S_OK;
+}
+
+// the pack, insert and check launches into t (slots and values allocated here), then the host build's refusal of a repeat
+int table_build_device(b2s_table_s* t, const int64_t* d_keys, const std::vector<TCol>& cols, cudaStream_t st) {
+  const int64_t n = t->n_keys;
+  const int32_t F = t->n_feat;
+  SyncOnExit done{st};
+  DeviceBlock blk(st);
+  const TCol* d_cols = nullptr;
+  unsigned long long* d_dup = nullptr;
+  blk.input(d_cols, cols.data(), sizeof(TCol) * cols.size());
+  blk.scratch(d_dup, 8);
+  if (int rc = blk.alloc()) return rc;
+  if (int rc = blk.upload()) return rc;
+  B2S_CUDA_TRY(cudaMalloc(&t->d_slots, t->cap * sizeof(Slot)));
+  B2S_CUDA_TRY(cudaMalloc(&t->d_values, ((size_t)n + 1) * F * 4));
+  B2S_CUDA_TRY(cudaMemsetAsync(t->d_slots, 0xff, t->cap * sizeof(Slot), st));  // row -1: empty
+  B2S_CUDA_TRY(cudaMemsetAsync(d_dup, 0xff, 8, st));
+  Launches launches;
+  const int gy = (F + 31) / 32;
+  const int gx = (int)std::max<int64_t>(1, std::min<int64_t>((n + 31) / 32, ((int64_t)b2s_int_sm_count() * 8 + gy - 1) / gy));
+  table_pack_kernel<<<dim3(gx, gy), kTableThreads, 0, st>>>(d_cols, F, n, t->d_values);
+  launches.add(1);
+  if (int rc = launched("table pack")) return rc;
+  const int g = grid_for(n, kTableThreads);
+  table_insert_kernel<<<g, kTableThreads, 0, st>>>(d_keys, n, t->d_slots, t->cap - 1);
+  launches.add(1);
+  if (int rc = launched("table insert")) return rc;
+  table_check_kernel<<<g, kTableThreads, 0, st>>>(d_keys, n, t->d_slots, t->cap - 1, d_dup);
+  launches.add(1);
+  if (int rc = launched("table check")) return rc;
+  unsigned long long dup = 0;
+  B2S_CUDA_TRY(cudaMemcpyAsync(&dup, d_dup, 8, cudaMemcpyDeviceToHost, st));
+  B2S_CUDA_TRY(cudaStreamSynchronize(st));
+  if (dup != ~0ull) {
+    const long long row = (long long)(dup >> 32), first = (long long)(dup & 0xffffffffull);
+    long long key = 0;
+    B2S_CUDA_TRY(cudaMemcpy(&key, d_keys + row, 8, cudaMemcpyDeviceToHost));
+    return b2s_int_fail(B2S_ERR_INVALID, "duplicate entity key %lld (rows %lld and %lld)", key, first, row);
+  }
+  return B2S_OK;
+}
+
+}  // namespace
+
+extern "C" int b2s_table_create_device(const int64_t* d_keys, int64_t n_keys, const b2s_table_col* cols, int32_t n_features,
+                                       const float* impute, b2s_table_t* out) {
+  try {  // no C++ exception crosses the C boundary
+    if (!d_keys || !cols || !out || n_keys <= 0 || n_keys > 0x7fffffffll || n_features <= 0 || n_features > 65535 * 32)
+      return b2s_int_fail(B2S_ERR_INVALID, "bad arguments");
+    std::vector<TCol> dev;
+    if (int rc = check_tcols(cols, n_features, n_keys, dev)) return rc;
+    if (int rc = table_device_ready()) return rc;
+    if (int rc = check_on_device(d_keys, 8, "keys", 0)) return rc;
+    if (int rc = check_tcols_on_device(dev)) return rc;
+    uint64_t cap = 16;
+    while (cap < (uint64_t)n_keys * 2) cap <<= 1;  // b2s_table_create's capacity: load factor <= 0.5
+    auto* t = new b2s_table_s();
+    t->n_keys = n_keys;
+    t->n_feat = n_features;
+    t->cap = cap;
+    int rc = table_build_device(t, d_keys, dev, b2s_int_stream());
+    if (!rc) rc = table_finish(t, impute);
+    if (rc) {
+      b2s_table_destroy(t);
+      return rc;
+    }
+    *out = t;
+    return B2S_OK;
+  } catch (const std::exception& e) {
+    return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
+  }
+}
+
+extern "C" int b2s_table_stats_device(const b2s_table_col* cols, int32_t n_features, int64_t n, float* stats_out, void* stream) {
+  try {  // no C++ exception crosses the C boundary
+    if (!cols || !stats_out || n < 0 || n_features <= 0 || n_features > 65535) return b2s_int_fail(B2S_ERR_INVALID, "bad arguments");
+    std::vector<TCol> dev;
+    if (int rc = check_tcols(cols, n_features, n, dev)) return rc;
+    if (int rc = table_device_ready()) return rc;
+    if (n)
+      if (int rc = check_tcols_on_device(dev)) return rc;
+    cudaStream_t st = stream ? (cudaStream_t)stream : b2s_int_stream();
+    const int nb = (int)std::max<int64_t>(1, std::min<int64_t>((n + kTableThreads - 1) / kTableThreads,
+                                                               ((int64_t)b2s_int_sm_count() * 8 + n_features - 1) / n_features));
+    SyncOnExit done{st};
+    DeviceBlock blk(st);
+    const TCol* d_cols = nullptr;
+    StatPart* d_part = nullptr;
+    double* d_sq = nullptr;
+    float* d_out = nullptr;
+    blk.input(d_cols, dev.data(), sizeof(TCol) * dev.size());
+    blk.scratch(d_part, sizeof(StatPart) * (size_t)nb * n_features);
+    blk.scratch(d_sq, sizeof(double) * (size_t)nb * n_features);
+    blk.output(d_out, stats_out, sizeof(float) * 5, n_features);
+    if (int rc = blk.alloc()) return rc;
+    if (int rc = blk.upload()) return rc;
+    Launches launches;
+    table_stats_sum_kernel<<<dim3(nb, n_features), kTableThreads, 0, st>>>(d_cols, n, d_part);
+    launches.add(1);
+    if (int rc = launched("table stats")) return rc;
+    table_stats_sq_kernel<<<dim3(nb, n_features), kTableThreads, 0, st>>>(d_cols, n, d_part, d_sq);
+    launches.add(1);
+    if (int rc = launched("table stats")) return rc;
+    table_stats_finish_kernel<<<(n_features + 127) / 128, 128, 0, st>>>(d_part, d_sq, nb, n_features, d_out);
+    launches.add(1);
+    if (int rc = launched("table stats")) return rc;
+    B2S_CUDA_TRY(cudaMemcpyAsync(stats_out, d_out, sizeof(float) * 5 * n_features, cudaMemcpyDeviceToHost, st));
+    B2S_CUDA_TRY(cudaStreamSynchronize(st));
+    return B2S_OK;
+  } catch (const std::exception& e) {
+    return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
+  }
+}
+
+extern "C" int b2s_table_label_keys_device(const int64_t* d_keys, int64_t n, const b2s_table_col* label, int64_t* keys_out, int64_t* n_out,
+                                           void* stream) {
+  try {  // no C++ exception crosses the C boundary
+    if (!label || !n_out || n < 0 || (n && (!d_keys || !keys_out))) return b2s_int_fail(B2S_ERR_INVALID, "bad arguments");
+    std::vector<TCol> dev;
+    if (int rc = check_tcols(label, 1, n, dev)) return rc;
+    *n_out = 0;
+    if (n == 0) return B2S_OK;
+    if (int rc = table_device_ready()) return rc;
+    if (int rc = check_on_device(d_keys, 8, "keys", 0)) return rc;
+    if (int rc = check_tcols_on_device(dev)) return rc;
+    cudaStream_t st = stream ? (cudaStream_t)stream : b2s_int_stream();
+    SyncOnExit done{st};
+    DeviceBlock blk(st);
+    unsigned long long* d_count = nullptr;
+    int64_t* d_out = nullptr;
+    blk.scratch(d_count, 8);
+    blk.scratch(d_out, (size_t)n * 8);
+    if (int rc = blk.alloc()) return rc;
+    B2S_CUDA_TRY(cudaMemsetAsync(d_count, 0, 8, st));
+    Launches launches;
+    table_label_keys_kernel<<<grid_for(n, kTableThreads), kTableThreads, 0, st>>>(d_keys, n, dev[0], d_out, d_count);
+    launches.add(1);
+    if (int rc = launched("label keys")) return rc;
+    unsigned long long count = 0;
+    B2S_CUDA_TRY(cudaMemcpyAsync(&count, d_count, 8, cudaMemcpyDeviceToHost, st));
+    B2S_CUDA_TRY(cudaStreamSynchronize(st));
+    if (count) B2S_CUDA_TRY(cudaMemcpyAsync(keys_out, d_out, count * 8, cudaMemcpyDeviceToHost, st));
+    B2S_CUDA_TRY(cudaStreamSynchronize(st));
+    *n_out = (int64_t)count;
+    return B2S_OK;
+  } catch (const std::exception& e) {
+    return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
+  }
+}
+
+extern "C" int b2s_table_mark_unknown_device(const int32_t* d_found, int32_t* d_status, int64_t n, void* stream) {
+  try {  // no C++ exception crosses the C boundary
+    if (n < 0 || (n && (!d_found || !d_status))) return b2s_int_fail(B2S_ERR_INVALID, "bad arguments");
+    if (n == 0) return B2S_OK;
+    if (int rc = table_device_ready()) return rc;
+    if (int rc = check_on_device(d_found, 4, "found", 0)) return rc;
+    if (int rc = check_on_device(d_status, 4, "status", 0)) return rc;
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(4 * b2s_int_sm_count(), (n + 255) / 256));
+    b2s_int_count_launches(1);
+    mark_unknown_kernel<<<grid, 256, 0, stream ? (cudaStream_t)stream : b2s_int_stream()>>>(d_found, d_status, n);
+    return launched("mark_unknown");
   } catch (const std::exception& e) {
     return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
   }

@@ -5,7 +5,10 @@ Plugin-API mirror of the parts of mlrun.feature_store the enrichment routers tou
 (mlrun/feature_store/feature_vector.py:903-1067).  The reference reads the online (NoSQL) store once per entity row
 through a storey graph; here the vector's online rows live in HBM (`b2s_table_*`, include/b200serve.h) and a batch of
 keys is resolved by one kernel launch.  The feature-store control plane (vector definition, targets, stats
-calculation jobs) is out of scope: a `FeatureVector` is built from an in-memory frame and registered by uri.
+calculation jobs) is out of scope: a `FeatureVector` is built from an in-memory frame, or from CUDA columns (a
+`columnar.DeviceColumnBatch` or a mapping), and registered by uri.  A vector of CUDA columns builds its table, its
+statistics and its label set on the device (b2s_table_create_device and friends): only counters, the 5 x F statistics
+and the keys of rows with a truthy label cross to the host, and the service equals the one built from the equal frame.
 
 Values are float32 on the device; impute values (constants or "$mean"-style statistics) are rounded to float32 when the
 service is initialised, and the stats table computed here is float32-valued, so `get()` returns the same numbers on
@@ -18,7 +21,9 @@ import ctypes as C
 import numpy as np
 
 from .. import _native as nat
+from ..lowering import LoweringError
 from ..serving.resolve import MLRunInvalidArgumentError
+from . import columnar
 
 _REGISTRY = {}
 
@@ -58,6 +63,47 @@ class DeviceTable:
         self._h = C.c_void_p()
         nat.check(self._lib.b2s_table_create(keys.ctypes.data_as(C.POINTER(C.c_int64)), len(keys), nat._p(values, C.c_float),
                                              self.n_feat, nat._p(imp, C.c_float), C.byref(self._h)))
+
+    @classmethod
+    def device(cls, d_keys, n_keys, cols, impute=None):
+        """the table of n_keys rows whose keys (an int64 address) and feature columns ([nat.TableCol]) are in device memory
+        (b2s_table_create_device): the same table b2s_table_create builds from the same values as float32"""
+        self = cls.__new__(cls)
+        self._lib = nat.init()
+        self.n_keys, self.n_feat = int(n_keys), len(cols)
+        imp = None if impute is None else np.ascontiguousarray(impute, dtype=np.float32)
+        self._h = C.c_void_p()
+        nat.check(self._lib.b2s_table_create_device(d_keys, self.n_keys, (nat.TableCol * len(cols))(*cols), self.n_feat,
+                                                    nat._p(imp, C.c_float), C.byref(self._h)))
+        return self
+
+    def lookup_arrays(self, d_keys):
+        """device keys (a DeviceArray of int64) -> ((n, F) float32 imputed rows, (n,) int32 found flags) as DeviceArrays,
+        ready when returned"""
+        n = d_keys.shape[0]
+        rows = nat.DeviceArray(nat.darray_alloc(max(n * self.n_feat * 4, 4)), (n, self.n_feat), np.float32)
+        found = nat.DeviceArray(nat.darray_alloc(max(n * 4, 4)), (n,), np.int32)
+        if n:
+            self.lookup_device(d_keys.ptr, n, rows.ptr, self.n_feat * 4, found.ptr)
+            nat.check(self._lib.b2s_device_sync())
+        return rows, found
+
+    def enrich_arrays(self, plan, d_keys):
+        """device keys -> (outputs, status) of `plan` as DeviceArrays, ready when returned: one fused launch
+        (b2s_table_enrich_device), or for plans the gather loader does not cover the gather, the plan's launches and the
+        unknown-key bits, as b2s_table_enrich_host runs them"""
+        n = d_keys.shape[0]
+        out = nat.DeviceArray(nat.darray_alloc(max(n * plan.out_cols * 4, 4)), (n, plan.out_cols), plan.out_dtype)
+        status = nat.DeviceArray(nat.darray_alloc(max(n * 4, 4)), (n,), np.int32)
+        if n:
+            if not self.enrich_device(plan, d_keys.ptr, n, out.ptr, status.ptr):
+                if b"merge targets" in (self._lib.b2s_last_error() or b""):
+                    nat.check(-6)  # the plan stores its votes elsewhere: refused, as b2s_table_enrich_host refuses it
+                rows, found = self.lookup_arrays(d_keys)
+                plan.run_device(rows.ptr, n, self.n_feat * 4, out.ptr, status.ptr)
+                nat.check(self._lib.b2s_table_mark_unknown_device(found.ptr, status.ptr, n, None))
+            nat.check(self._lib.b2s_device_sync())
+        return out, status
 
     def lookup(self, keys, with_stats=False):
         keys = np.ascontiguousarray(keys, dtype=np.int64)
@@ -120,8 +166,11 @@ class DeviceTable:
 
 
 class FeatureVector:
-    """name, requested features, index (entity) keys, label column, and the online rows as a frame whose index (or
-    `index_keys` columns) holds the entity keys"""
+    """name, requested features, index (entity) keys, label column, and the online rows: a frame whose index (or
+    `index_keys` columns) holds the entity keys, or CUDA columns -- a `columnar.DeviceColumnBatch` (its `index` holds the
+    entity columns, unless `index_keys` name result columns) or a mapping that holds the `index_keys` columns.  CUDA
+    columns are described here and read when the service is built; the service equals the one built from the equal frame
+    (`batch.to_host().to_pandas()`, or the mapping's columns indexed by `index_keys`)."""
 
     def __init__(self, name, features, index_keys, frame, stats=None, label_column=None, with_indexes=False):
         self.name = name
@@ -129,26 +178,35 @@ class FeatureVector:
         self.index_keys = list(index_keys)
         self.label_column = label_column
         self.with_indexes = with_indexes
-        if all(k in frame.columns for k in self.index_keys):
+        self.device = None
+        if columnar.is_columnar(frame) and columnar.is_device_source(frame):
+            self.device = _DeviceRows(frame, self.index_keys)
+            frame = None
+        elif all(k in frame.columns for k in self.index_keys):
             frame = frame.set_index(self.index_keys)
         self.frame = frame
         self._stats = stats
 
     def get_stats_table(self):
-        """feature statistics (mean / min / max / std / count per feature), float32-valued"""
+        """feature statistics (mean / min / max / std / count per feature), float32-valued.  Of CUDA columns: one
+        reduction on the device (b2s_table_stats_device); count, min and max equal the frame's, mean and std are within one
+        float32 ulp of them (bit-equal where every float64 partial sum is exact: the frame sums sequentially)"""
         if self._stats is None:
             import pandas as pd
 
             cols = [f for f in self.features if f != self.label_column]
-            vals = self.frame[cols].to_numpy(dtype=np.float32).copy()
-            vals[~np.isfinite(vals)] = np.nan  # statistics of the finite observations
-            with np.errstate(all="ignore"):
-                stats = {
-                    "mean": np.nanmean(vals.astype(np.float64), axis=0).astype(np.float32),
-                    "min": np.nanmin(vals, axis=0), "max": np.nanmax(vals, axis=0),
-                    "std": np.nanstd(vals.astype(np.float64), axis=0, ddof=1).astype(np.float32),
-                    "count": np.sum(~np.isnan(vals), axis=0).astype(np.float32),
-                }
+            if self.device is not None:
+                stats = dict(zip(("mean", "min", "max", "std", "count"), self.device.stats(cols)))
+            else:
+                vals = self.frame[cols].to_numpy(dtype=np.float32).copy()
+                vals[~np.isfinite(vals)] = np.nan  # statistics of the finite observations
+                with np.errstate(all="ignore"):
+                    stats = {
+                        "mean": np.nanmean(vals.astype(np.float64), axis=0).astype(np.float32),
+                        "min": np.nanmin(vals, axis=0), "max": np.nanmax(vals, axis=0),
+                        "std": np.nanstd(vals.astype(np.float64), axis=0, ddof=1).astype(np.float32),
+                        "count": np.sum(~np.isnan(vals), axis=0).astype(np.float32),
+                    }
             self._stats = pd.DataFrame({k: [float(x) for x in v] for k, v in stats.items()}, index=cols)
         return self._stats
 
@@ -185,6 +243,8 @@ class OnlineVectorService:
     def initialize(self):
         """impute values (feature_vector.py:935-968), then the online rows go to the device"""
         self._impute_values = self._resolve_policy(dict(self.impute_policy)) if self.impute_policy else {}
+        if self.vector.device is not None:
+            return self._initialize_device(self.vector.device)
         frame = self.vector.frame
         values = frame[self._columns].to_numpy(dtype=np.float32)
         keys = self._encode_keys(frame.index, build=True)
@@ -198,12 +258,64 @@ class OnlineVectorService:
         impute = np.array([self._impute_values.get(c, np.nan) for c in self._columns], dtype=np.float32)
         self.table = DeviceTable(keys, values, impute if self._impute_values else None)
 
+    def _initialize_device(self, rows):
+        """the table, its keys and the truthy-label keys built where the CUDA columns are"""
+        feats = rows.table_cols(self._columns, "feature")
+        label = self.vector.label_column
+        label_col = rows.table_cols([label], "label")[0] if label and label in rows.columns else None
+        impute = np.array([self._impute_values.get(c, np.nan) for c in self._columns], dtype=np.float32)
+        self._string_keys = len(rows.keys) > 1
+        self._label_alive = None
+        try:
+            keys = _encode_device_keys(rows.keys, self._string_keys)
+            cols = [nat.TableCol(c.acquire().ptr, dt.itemsize, kind) for c, dt, kind in feats]
+            try:
+                self.table = DeviceTable.device(keys.ptr, rows.n, cols, impute if self._impute_values else None)
+            except nat.NativeError as err:  # the frame path hashes composite keys first and refuses a repeat there
+                if self._string_keys and "duplicate entity key" in str(err):
+                    raise MLRunInvalidArgumentError("two entity keys share a 64-bit hash (or a key is duplicated)") from None
+                raise
+            if label_col is not None:
+                c, dt, kind = label_col
+                alive, count = np.empty(rows.n, dtype=np.int64), C.c_int64()
+                nat.check(nat.load().b2s_table_label_keys_device(keys.ptr, rows.n, C.byref(nat.TableCol(c.acquire().ptr, dt.itemsize, kind)),
+                                                                 nat._p(alive, C.c_int64), C.byref(count), None))
+                self._label_alive = np.sort(alive[:count.value])
+            keys.release()
+        finally:
+            rows.release()
+
+    def _device_keys(self, keys):
+        """CUDA entity keys -> a library int64 array encoded as `_encode_keys` encodes the equal host keys; None for host
+        keys.  One CUDA int column for a single entity, or a mapping holding the `index_keys` columns."""
+        if isinstance(keys, dict) and keys and columnar.is_device_source(keys):
+            cols = columnar.device_columns(keys)
+            missing = [k for k in self._index_columns if k not in cols]
+            if missing:
+                raise LoweringError(f"the CUDA keys have no entity column {missing[0]!r}")
+            cols = [cols[k] for k in self._index_columns]
+        elif columnar.is_device_column(keys):
+            cols = [columnar.DeviceColumn(keys, self._index_columns[0] if self._index_columns else "key")]
+        else:
+            return None
+        _check_key_columns(cols)
+        if len(cols) > 1 and not self._string_keys:
+            raise MLRunInvalidArgumentError("the online table has integer entity keys")
+        try:
+            return _encode_device_keys(cols, self._string_keys)
+        finally:
+            for c in cols:
+                c.release()
+
     def _resolve_policy(self, policy):
         """{feature | "*": constant | "$stat"} -> {feature: float32 value held on the device} (feature_vector.py:935-968)"""
-        stats = self.vector.get_stats_table()
+        if self.vector.device is None:
+            self.vector.get_stats_table()
+        else:  # the refusals of the features come first, as there; the statistics are reduced when a "$" value needs them
+            self.vector.device.table_cols(self._columns, "feature")
 
         def value_of(feature, spec):
-            v = stats.loc[feature, spec[1:]] if isinstance(spec, str) and spec.startswith("$") else spec
+            v = self.vector.get_stats_table().loc[feature, spec[1:]] if isinstance(spec, str) and spec.startswith("$") else spec
             v = float(np.float32(v))
             if not np.isfinite(v):
                 raise MLRunInvalidArgumentError(f"impute value of feature {feature} is not finite ({v}): not held on the device")
@@ -250,8 +362,16 @@ class OnlineVectorService:
 
     # ---- batched engine surface --------------------------------------------------------------------
     def get_matrix(self, keys):
-        """entity keys (one per row; tuples for composite keys) -> ((B, F) float32 imputed rows, found mask)"""
-        return self.table.lookup(self._encode_keys(keys))
+        """entity keys (one per row; tuples for composite keys) -> ((B, F) float32 imputed rows, found mask).  CUDA keys
+        (one int column, or a mapping of the `index_keys` int columns) give `_native.DeviceArray`s instead: the rows and
+        int32 found flags, ready when returned."""
+        d_keys = self._device_keys(keys)
+        if d_keys is None:
+            return self.table.lookup(self._encode_keys(keys))
+        try:
+            return self.table.lookup_arrays(d_keys)
+        finally:
+            d_keys.release()
 
     # ---- the reference's call ---------------------------------------------------------------------------
     def get(self, entity_rows, as_list=False):
@@ -297,3 +417,91 @@ class OnlineVectorService:
         if self.table is not None:
             self.table.close()
             self.table = None
+
+
+# ------------------------------------------------------------------------------------------------ online rows in HBM
+_TCOL_KINDS = {"f": nat.TCOL_FLOAT, "i": nat.TCOL_INT, "u": nat.TCOL_UINT, "b": nat.TCOL_BOOL}
+
+
+def _check_key_columns(cols):
+    """entity columns of CUDA keys: signed ints of one length (the frame path hashes str() of other values, and a device
+    has no strings)"""
+    for c in cols:
+        if c.dtype.kind != "i":
+            raise LoweringError(f"entity key {c.name!r} has dtype {c.dtype}: CUDA entity keys are signed int columns (the "
+                                "frame path hashes str() of other values)")
+    if len({c.n for c in cols}) > 1:
+        raise ValueError("All arrays must be of the same length")
+
+
+def _encode_device_keys(cols, strings):
+    """-> a DeviceArray of int64 keys: one column widened (b2s_keys_encode_device), or the FNV-1a hash of the row's
+    decimal text joined by "." (b2s_keys_hash_decimal_device), as `_encode_keys` encodes ints and tuples"""
+    lib = nat.init()
+    n = cols[0].n
+    keys = nat.DeviceArray(nat.darray_alloc(max(8 * n, 8)), (n,), np.int64)
+    if n:
+        kc = (nat.KeyCol * len(cols))(*[nat.KeyCol(c.acquire().ptr, c.dtype.itemsize, 1) for c in cols])
+        fn = lib.b2s_keys_hash_decimal_device if strings else lib.b2s_keys_encode_device
+        nat.check(fn(kc, len(cols), n, keys.ptr, None))
+    return keys
+
+
+class _DeviceRows:
+    """a vector's online rows as CUDA columns: `keys` (the entity columns in order) and `columns` {name: DeviceColumn},
+    described when the vector is made, acquired by each call that reads them"""
+
+    def __init__(self, source, index_keys):
+        cols = columnar.device_columns(source)
+        if len({c.n for c in cols.values()}) > 1:
+            raise ValueError("All arrays must be of the same length")
+        data = list(source.columns) if isinstance(source, columnar.DeviceColumnBatch) else list(cols)
+        if isinstance(source, columnar.DeviceColumnBatch) and not all(k in source.columns for k in index_keys):
+            names = list(source.index)  # the frame keeps the batch's index
+            if not names:
+                raise LoweringError("the DeviceColumnBatch has no entity columns (index) and no index_keys columns")
+        else:
+            names = list(index_keys)
+            missing = [k for k in names if k not in cols]
+            if not names or missing:
+                raise LoweringError(f"the online rows have no entity column {(missing or [None])[0]!r}: CUDA columns hold their "
+                                    "keys in the index_keys columns")
+        self.keys = [cols[k] for k in names]
+        _check_key_columns(self.keys)
+        self.columns = {k: cols[k] for k in data if k not in names}
+        self.n = self.keys[0].n
+
+    def table_cols(self, names, what):
+        """-> [(DeviceColumn, dtype, nat.TCOL_*)] of the named columns; a missing name is pandas' KeyError"""
+        missing = [f for f in names if f not in self.columns]
+        if missing:
+            import pandas as pd
+
+            pd.DataFrame(columns=list(self.columns))[names]  # raises the frame path's KeyError
+        out = []
+        for f in names:
+            c = self.columns[f]
+            kind = _TCOL_KINDS.get(c.dtype.kind)
+            if kind is None or (c.dtype.kind == "f" and c.dtype.itemsize not in (4, 8)):
+                raise LoweringError(f"{what} {f!r} has dtype {c.dtype}: the online table takes float32, float64, (u)int8/16/32/64 "
+                                    "and bool columns")
+            out.append((c, c.dtype, kind))
+        return out
+
+    def stats(self, names):
+        """the frame path's statistics of the named features as a (5, F) float32 array: mean, min, max, std, count"""
+        feats = self.table_cols(names, "feature")
+        out = np.empty((5, len(names)), dtype=np.float32)
+        if not names:
+            return out
+        try:
+            lib = nat.init()
+            cols = [nat.TableCol(c.acquire().ptr, dt.itemsize, kind) for c, dt, kind in feats]
+            nat.check(lib.b2s_table_stats_device((nat.TableCol * len(cols))(*cols), len(cols), self.n, nat._p(out, C.c_float), None))
+        finally:
+            self.release()
+        return out
+
+    def release(self):
+        for c in self.keys + list(self.columns.values()):
+            c.release()

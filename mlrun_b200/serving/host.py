@@ -320,7 +320,9 @@ class GraphServer(Serde):
         """batched enrichment + predict for a graph whose root is an Enrichment router: entity keys -> outputs with the
         online-table gather feeding the fused scoring plan on the device (`b2s_table_enrich_host`: keys in, votes and status
         words out, nothing else crosses PCIe); replaces EnrichmentVotingEnsemble.preprocess + the per-model predicts,
-        serving/routers.py:1335-1342.  Unknown keys come back with status bit 4 (ROW_UNKNOWN_KEY)."""
+        serving/routers.py:1335-1342.  Unknown keys come back with status bit 4 (ROW_UNKNOWN_KEY).  CUDA keys (one int column,
+        or a mapping of the vector's `index_keys` int columns) stay in HBM: the outputs and status words come back as
+        `_native.DeviceArray`s, ready when returned."""
         from ..lowering import LoweringError
 
         compiled = self.compile()
@@ -331,7 +333,14 @@ class GraphServer(Serde):
         plan = compiled.plan
         if plan.n_in != svc.table.n_feat:
             raise LoweringError(f"the feature vector has {svc.table.n_feat} features, the models take {plan.n_in}")
-        out, status = svc.table.enrich(plan, svc._encode_keys(keys))
+        d_keys = svc._device_keys(keys)
+        if d_keys is None:
+            out, status = svc.table.enrich(plan, svc._encode_keys(keys))
+        else:
+            try:
+                out, status = svc.table.enrich_arrays(plan, d_keys)
+            finally:
+                d_keys.release()
         return (out, status) if with_status else out
 
     def run_binary(self, body):
