@@ -461,6 +461,22 @@ int b2s_table_label_keys_device(const int64_t* d_keys, int64_t n, const b2s_tabl
  * words b2s_table_enrich_device gives.  One launch, asynchronous. */
 int b2s_table_mark_unknown_device(const int32_t* d_found, int32_t* d_status, int64_t n, void* stream);
 
+/* Scoring rows held as device columns (a device ingest's result, a mapping of CUDA columns): n_rows rows whose input column
+ * c is cols[c] (n_cols must be the plan's n_in; kinds and widths as for b2s_table_create_device, each value converted as
+ * numpy's astype(float32) converts it) -> d_out (n_rows x out_cols words) and d_status (may be NULL), as b2s_run_device
+ * gives them for the same rows as a contiguous float32 matrix.  The columns are packed into row-major float32 rows at a
+ * stride of 4 * n_in bytes in library scratch, then scored by the plan's own launches, so the plan serves them with the
+ * kernel it picks for a contiguous host matrix of that width (b2s_plan_last_kernel).  The work runs in ranges of at most
+ * 2^20 rows that reuse one scratch buffer of min(n_rows, 2^20) * 4 * n_in bytes, freed on every return; range k's outputs
+ * go to d_out + k * 2^20 * out_cols words.  Asynchronous on `stream` (NULL = the library's stream).  stats (may be NULL)
+ * gets rows and kernels: per range, 1 pack launch plus the plan's launches; n_rows = 0 launches nothing.
+ * B2S_ERR_INVALID, before any launch, for n_cols other than n_in, a bad kind or width, a column that is null, not aligned
+ * to its width or not on the library's device, d_out / d_status not 4-byte aligned, a plan that is not finalized and
+ * n_rows < 0.  B2S_ERR_UNSUPPORTED, before anything is enqueued, for a plan with merge targets or an attached communicator
+ * (each range would be a step of its own). */
+int b2s_run_columns_device(b2s_plan_t plan, const b2s_table_col* cols, int32_t n_cols, int64_t n_rows, void* d_out,
+                           int32_t* d_status, b2s_stats* stats, void* stream);
+
 /* ---- point-in-time training sets: as-of joins of entity rows onto feature-set indexes ---------------------------
  * get_offline_features on the local engine (feature_store/retrieval/base.py:412-468, local_merger.py:29-81) merges
  * each feature set of a vector onto the entity frame with pandas.merge_asof: equal keys, the set's last row whose

@@ -146,6 +146,7 @@ SIGNATURES = {
     "b2s_plan_kernel": (C.c_char_p, [_vp]),
     "b2s_plan_last_kernel": (_i32, [_vp]),
     "b2s_run_device": (C.c_int, [_vp, _vp, _i64, _i64, _vp, _vp, _vp]),
+    "b2s_run_columns_device": (C.c_int, [_vp, C.POINTER(TableCol), _i32, _i64, _vp, _vp, C.POINTER(Stats), _vp]),
     "b2s_run_host": (C.c_int, [_vp, _vp, _i64, _i64, _vp, _i64, _vp, C.POINTER(Stats)]),
     "b2s_submit": (C.c_int, [_vp, _vp, _i64, _i64, C.POINTER(_u64)]),
     "b2s_wait": (C.c_int, [_vp, _u64, _vp, _i64, _vp, C.POINTER(Stats)]),

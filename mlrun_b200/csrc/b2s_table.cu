@@ -567,6 +567,26 @@ __global__ void __launch_bounds__(kTableThreads) table_pack_kernel(const TCol* _
   }
 }
 
+// one range of b2s_run_columns_device: rows[r][c] = column c at row first + r for r < n, the same tile transpose and
+// conversion as table_pack_kernel without its NaN row (kept apart so that table_pack_kernel's code stays as it is)
+__global__ void __launch_bounds__(kTableThreads) rows_pack_kernel(const TCol* __restrict__ cols, int32_t n_feat, int64_t first,
+                                                                   int64_t n, float* __restrict__ rows) {
+  __shared__ float tile[32][33];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int c0 = blockIdx.y * 32;
+  const int cw = min(32, n_feat - c0);
+  for (int64_t r0 = (int64_t)blockIdx.x * 32; r0 < n; r0 += (int64_t)gridDim.x * 32) {
+    for (int c = warp; c < cw; c += kTableThreads / 32) {
+      const TCol col = cols[c0 + c];
+      if (r0 + lane < n) tile[c][lane] = col_f32(col, first + r0 + lane);
+    }
+    __syncthreads();
+    for (int r = warp; r < 32 && r0 + r < n; r += kTableThreads / 32)
+      if (lane < cw) rows[(r0 + r) * n_feat + c0 + lane] = tile[lane][r];
+    __syncthreads();
+  }
+}
+
 // one thread per key claims the first free slot of its walk (the row word goes from -1 to the row, then the key is
 // stored): a repeated key takes a slot of its own, which table_check_kernel finds
 __global__ void __launch_bounds__(kTableThreads) table_insert_kernel(const int64_t* __restrict__ keys, int64_t n, Slot* slots, uint64_t mask) {
@@ -923,6 +943,62 @@ extern "C" int b2s_table_mark_unknown_device(const int32_t* d_found, int32_t* d_
     b2s_int_count_launches(1);
     mark_unknown_kernel<<<grid, 256, 0, stream ? (cudaStream_t)stream : b2s_int_stream()>>>(d_found, d_status, n);
     return launched("mark_unknown");
+  } catch (const std::exception& e) {
+    return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
+  }
+}
+
+// ---- scoring rows held as device columns ---------------------------------------------------------------------------------
+// Columns in HBM (a device ingest's result, a mapping of CUDA columns) are packed into float32 rows at the stride a
+// contiguous host matrix has, so the plan picks the kernel it picks for b2s_run_host rows of that width, then scored by the
+// plan's own launches.  Ranges of kColumnRangeRows rows share one scratch buffer (stream order keeps a range's pack behind
+// the previous range's scoring), so a batch of any size needs at most 4 * n_in MiB of staging.
+namespace {
+constexpr int64_t kColumnRangeRows = 1 << 20;
+}
+
+extern "C" int b2s_run_columns_device(b2s_plan_t plan, const b2s_table_col* cols, int32_t n_cols, int64_t n_rows, void* d_out,
+                                      int32_t* d_status, b2s_stats* stats, void* stream) {
+  try {  // no C++ exception crosses the C boundary
+    if (stats) memset(stats, 0, sizeof(*stats));
+    if (!plan || !cols || n_rows < 0 || (n_rows && !d_out)) return b2s_int_fail(B2S_ERR_INVALID, "bad arguments");
+    int n_in = 0, out_cols = 0;
+    if (b2s_int_plan_shape(plan, &n_in, &out_cols)) return b2s_int_fail(B2S_ERR_INVALID, "plan not finalized");
+    if (n_cols != n_in) return b2s_int_fail(B2S_ERR_INVALID, "%d columns, the plan takes %d", n_cols, n_in);
+    std::vector<TCol> dev;
+    if (int rc = check_tcols(cols, n_cols, n_rows, dev)) return rc;
+    if (misaligned(d_out, 4) || misaligned(d_status, 4)) return b2s_int_fail(B2S_ERR_INVALID, "out and status must be 4-byte aligned");
+    if (int rc = refuse_merging(plan)) return rc;  // a range per communicator step would split one call into several
+    if (n_rows == 0) return B2S_OK;
+    if (int rc = table_device_ready()) return rc;
+    if (int rc = check_tcols_on_device(dev)) return rc;
+    cudaStream_t st = stream ? (cudaStream_t)stream : b2s_int_stream();
+    const int64_t row_bytes = (int64_t)n_in * 4, out_bytes = (int64_t)out_cols * 4;
+    DeviceBlock blk(st);  // freed in stream order on every return
+    const TCol* d_cols = nullptr;
+    float* d_rows = nullptr;
+    blk.input(d_cols, dev.data(), sizeof(TCol) * dev.size());
+    blk.scratch(d_rows, (size_t)std::min(n_rows, kColumnRangeRows) * row_bytes);
+    if (int rc = blk.alloc()) return rc;
+    if (int rc = blk.upload()) return rc;
+    Launches launches;
+    const int gy = (n_in + 31) / 32;
+    for (int64_t r0 = 0; r0 < n_rows; r0 += kColumnRangeRows) {
+      const int64_t n = std::min(kColumnRangeRows, n_rows - r0);
+      const int gx = (int)std::max<int64_t>(1, std::min<int64_t>((n + 31) / 32, ((int64_t)b2s_int_sm_count() * 8 + gy - 1) / gy));
+      rows_pack_kernel<<<dim3(gx, gy), kTableThreads, 0, st>>>(d_cols, n_in, r0, n, d_rows);
+      launches.add(1);
+      if (int rc = launched("rows pack")) return rc;
+      if (int rc = b2s_run_device(plan, d_rows, n, row_bytes, static_cast<char*>(d_out) + r0 * out_bytes,
+                                  d_status ? d_status + r0 : nullptr, st))
+        return rc;
+      launches.n += b2s_int_plan_kernels(plan);  // b2s_run_device adds them to the library's count itself
+    }
+    if (stats) {
+      stats->rows = n_rows;
+      stats->kernels = launches.n;
+    }
+    return B2S_OK;
   } catch (const std::exception& e) {
     return b2s_int_fail(B2S_ERR_INVALID, "%s: %s", __func__, e.what());
   }

@@ -186,10 +186,13 @@ class DeviceColumn:
     states (shape, strides, dtype, device) without touching the library: from the CUDA array interface, or else from a
     DLPack capsule taken with stream=-1 (no synchronisation) and dropped at once.  `acquire` orders the library stream
     behind the producer (DLPack: the producer makes the stream it is given wait; CUDA array interface v3: the library stream
-    waits for `stream`) and holds a DLPack capsule until `release`."""
+    waits for `stream`) and holds a DLPack capsule until `release`.
 
-    def __init__(self, obj, name):
-        self.obj, self.name = obj, name
+    With matrix=True the object is any array instead: `shape`, `ndim` and byte `strides` are recorded as the producer states
+    them and the caller judges them (a row matrix: `plan.check_rows`)."""
+
+    def __init__(self, obj, name, matrix=False):
+        self.obj, self.name, self.matrix = obj, name, matrix
         self.ptr = None
         self._capsule = None
         self._cai = None
@@ -219,6 +222,15 @@ class DeviceColumn:
             return self.obj.__dlpack__()
 
     def _shape(self, shape, strides, dtype, byte_strides):
+        if self.matrix:
+            self.dtype, self.shape = dtype, tuple(int(d) for d in shape)
+            if strides is None:  # C order
+                strides = [dtype.itemsize * int(np.prod(self.shape[i + 1:])) for i in range(len(self.shape))]
+            elif not byte_strides:
+                strides = [s * dtype.itemsize for s in strides]
+            self.strides, self.ndim = tuple(int(s) for s in strides), len(self.shape)
+            self.n = self.shape[0] if self.shape else 1
+            return
         if len(shape) != 1:
             raise ValueError(f"column {self.name!r}: expected a 1-D column, got shape {shape}")
         step = dtype.itemsize if byte_strides else 1

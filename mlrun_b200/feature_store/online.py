@@ -447,6 +447,25 @@ def _encode_device_keys(cols, strings):
     return keys
 
 
+def table_cols(columns, names, what):
+    """-> [(DeviceColumn, dtype, nat.TCOL_*)] of the named columns of {name: DeviceColumn}; a missing name is pandas'
+    KeyError"""
+    missing = [f for f in names if f not in columns]
+    if missing:
+        import pandas as pd
+
+        pd.DataFrame(columns=list(columns))[names]  # raises the frame path's KeyError
+    out = []
+    for f in names:
+        c = columns[f]
+        kind = _TCOL_KINDS.get(c.dtype.kind)
+        if kind is None or (c.dtype.kind == "f" and c.dtype.itemsize not in (4, 8)):
+            raise LoweringError(f"{what} {f!r} has dtype {c.dtype}: the online table takes float32, float64, (u)int8/16/32/64 "
+                                "and bool columns")
+        out.append((c, c.dtype, kind))
+    return out
+
+
 class _DeviceRows:
     """a vector's online rows as CUDA columns: `keys` (the entity columns in order) and `columns` {name: DeviceColumn},
     described when the vector is made, acquired by each call that reads them"""
@@ -472,21 +491,7 @@ class _DeviceRows:
         self.n = self.keys[0].n
 
     def table_cols(self, names, what):
-        """-> [(DeviceColumn, dtype, nat.TCOL_*)] of the named columns; a missing name is pandas' KeyError"""
-        missing = [f for f in names if f not in self.columns]
-        if missing:
-            import pandas as pd
-
-            pd.DataFrame(columns=list(self.columns))[names]  # raises the frame path's KeyError
-        out = []
-        for f in names:
-            c = self.columns[f]
-            kind = _TCOL_KINDS.get(c.dtype.kind)
-            if kind is None or (c.dtype.kind == "f" and c.dtype.itemsize not in (4, 8)):
-                raise LoweringError(f"{what} {f!r} has dtype {c.dtype}: the online table takes float32, float64, (u)int8/16/32/64 "
-                                    "and bool columns")
-            out.append((c, c.dtype, kind))
-        return out
+        return table_cols(self.columns, names, what)
 
     def stats(self, names):
         """the frame path's statistics of the named features as a (5, F) float32 array: mean, min, max, std, count"""

@@ -24,6 +24,22 @@ def _f64(a):
     return np.ascontiguousarray(a, dtype=np.float64)
 
 
+def check_rows(X, n_in):
+    """X (a numpy array, or anything with its dtype / ndim / shape / byte strides) as rows a plan of n_in columns reads"""
+    if X.dtype != np.float32 or X.ndim != 2 or X.shape[1] != n_in or (X.shape[0] and X.strides[1] != 4):
+        raise ValueError(f"rows must be a float32 (B, {n_in}) array with unit inner stride")
+    return X
+
+
+# b2s_run_columns_device packs and scores at most this many rows at a time, in one scratch buffer of that many rows
+RANGE_ROWS = 1 << 20
+
+
+def column_ranges(n, out_row_bytes):
+    """[(first row, rows, byte offset of the range's outputs)] of b2s_run_columns_device over n rows"""
+    return [(r0, min(RANGE_ROWS, n - r0), r0 * out_row_bytes) for r0 in range(0, n, RANGE_ROWS)]
+
+
 class PackedTrees:
     """SoA tree ensemble in the layout b2s_plan_add_tree_model takes (children are tree-relative)"""
 
@@ -173,9 +189,7 @@ class DevicePlan:
 
     # ---- execution ---------------------------------------------------------------------------
     def _check_rows(self, X):
-        if X.dtype != np.float32 or X.ndim != 2 or X.shape[1] != self.n_in or (X.shape[0] and X.strides[1] != 4):
-            raise ValueError(f"rows must be a float32 (B, {self.n_in}) array with unit inner stride")
-        return X
+        return check_rows(X, self.n_in)
 
     def _stride(self, X):
         return X.strides[0] if X.shape[0] else self.n_in * 4  # an empty array reports no usable strides
@@ -243,6 +257,15 @@ class DevicePlan:
 
     def run_device(self, d_rows, n_rows, row_stride, d_out, d_status=None, stream=None):
         nat.check(self._lib.b2s_run_device(self._h, d_rows, n_rows, row_stride, d_out, d_status, stream))
+
+    def run_columns_device(self, cols, n, d_out, d_status=None, stream=None):
+        """n rows of `n_in` device columns ([nat.TableCol], one per input column) -> outputs (+ status) in HBM
+        (b2s_run_columns_device): packed into float32 rows range by range (`column_ranges`), each range then scored by
+        the plan's own launches.  Returns the call's stats (its `kernels`: per range, the pack and the plan's launches)."""
+        arr = (nat.TableCol * max(len(cols), 1))(*cols)
+        stats = nat.Stats()
+        nat.check(self._lib.b2s_run_columns_device(self._h, arr, len(cols), int(n), d_out, d_status, C.byref(stats), stream))
+        return stats.as_dict()
 
     def set_merge_targets(self, peer_ptrs, row_offset):
         """fused ensemble-merge: every output row is stored into each peer buffer at row_offset + row"""

@@ -295,9 +295,85 @@ class GraphServer(Serde):
 
     def run_batch(self, X, names=None, with_status=False):
         """(B, F) float32 rows, columns named `names` (default f0..fF-1 or the compiled schema) ->
-        (B, out_cols) outputs from one fused launch.  Semantics: row i is the event {names[j]: X[i, j]}."""
+        (B, out_cols) outputs from one fused launch.  Semantics: row i is the event {names[j]: X[i, j]}.
+
+        Rows already in HBM are scored there; the outputs (and status words) then come back as `_native.DeviceArray`s,
+        ready when returned, and the producer's queued writes are awaited first:
+          - a CUDA matrix (a torch tensor, any DLPack or CUDA-array-interface producer, a DeviceArray such as
+            `get_offline_tensors(...).features` with names=t.columns): float32, unit inner stride, a row stride that is a
+            multiple of 4 bytes; read in place at its own row stride, without a copy.  Equals run_batch(X.cpu().numpy()).
+          - a `columnar.DeviceColumnBatch` (its result and index columns) or a mapping of CUDA columns: `names` (default: the
+            compiled schema) picks the plan's input columns in order; float32/64, (u)int8/16/32/64 and bool columns are
+            packed into float32 rows on the device, each converted as `astype(np.float32)` converts it.  Equals, bit for bit,
+            run_batch(np.stack([np.asarray(c).astype(np.float32) for c in picked], axis=1), names).  That can differ from
+            `frame[names].to_numpy(np.float32)` of a mixed frame, which goes through float64 and so rounds an int64 above
+            2**53 twice."""
+        from ..feature_store import columnar
+
+        if columnar.is_device_column(X):
+            return self._run_device_matrix(X, names, with_status)
+        if isinstance(X, (dict, columnar.DeviceColumnBatch)) and columnar.is_device_source(X):
+            return self._run_device_columns(X, names, with_status)
         compiled = self.compile(names)
         return compiled.plan.run(np.ascontiguousarray(X, dtype=np.float32), with_status=with_status)
+
+    def _run_device_matrix(self, X, names, with_status):
+        """run_batch of a CUDA matrix: b2s_run_device over the rows where they are"""
+        from ..feature_store.columnar import DeviceColumn
+        from ..lowering import LoweringError
+        from ..plan import check_rows
+
+        m = DeviceColumn(X, "X", matrix=True)
+        if m.dtype != np.float32:
+            raise LoweringError(f"the CUDA matrix has dtype {m.dtype}: the plan reads float32 rows (build it with "
+                                'get_offline_tensors(..., dtype="float32"))')
+        if names is not None:
+            check_rows(m, len(names))
+        plan = self.compile(names).plan
+        check_rows(m, plan.n_in)
+        n = m.shape[0]
+        stride = m.strides[0] if n > 1 else plan.n_in * 4  # one row: any stated stride reads the same words
+        if stride % 4:
+            raise ValueError(f"the CUDA matrix's row stride of {stride} bytes is not a multiple of 4")
+        out, status = _device_results(plan, n, with_status)
+        try:
+            m.acquire()
+            if m.ptr % 4:
+                raise ValueError("the CUDA matrix does not start on a 4-byte boundary")
+            if n:
+                plan.run_device(m.ptr, n, stride, out.ptr, status.ptr if status is not None else None)
+                _device_sync()
+        finally:
+            m.release()
+        return (out, status) if with_status else out
+
+    def _run_device_columns(self, X, names, with_status):
+        """run_batch of CUDA columns: b2s_run_columns_device packs the picked columns into rows and scores them"""
+        from .. import _native as nat
+        from ..feature_store import columnar
+        from ..feature_store.online import table_cols
+        from ..lowering import LoweringError
+
+        cols = columnar.device_columns(X)
+        if len({c.n for c in cols.values()}) > 1:
+            raise ValueError("All arrays must be of the same length")
+        names = list(self.compile().in_names if names is None else names)
+        for name in names:
+            if name in cols and cols[name].dtype.kind == "M":
+                raise LoweringError(f"feature {name!r} is a {cols[name].dtype} column: a matrix of numbers has no place for it "
+                                    "(drop it from names)")
+        picked = table_cols(cols, names, "feature")
+        plan = self.compile(names).plan
+        n = next(iter(cols.values())).n if cols else len(X)
+        out, status = _device_results(plan, n, with_status)
+        try:
+            tcols = [nat.TableCol(c.acquire().ptr, dt.itemsize, kind) for c, dt, kind in picked]
+            plan.run_columns_device(tcols, n, out.ptr, status.ptr if status is not None else None)
+            _device_sync()
+        finally:
+            for c in cols.values():
+                c.release()
+        return (out, status) if with_status else out
 
     def run_events(self, bodies, path=None):
         """feature-dict event bodies -> per-event responses through the fused plan.  Rows flagged by the
@@ -388,6 +464,21 @@ class GraphServer(Serde):
                                         lambda j: {**response, "outputs": vals.tolist()}, _tracked_op(compiled.tracker))
         text = codec.format_outputs(out[:, 0] if out.shape[1] == 1 else out)
         return self.context.Response(body=codec.dumps_with_outputs(response, text), content_type="application/json", status_code=200)
+
+
+def _device_results(plan, n, with_status):
+    """the outputs (and, with_status, the status words) of n rows as DeviceArrays"""
+    from .. import _native as nat
+
+    out = nat.DeviceArray(nat.darray_alloc(max(n * plan.out_cols * 4, 4)), (n, plan.out_cols), plan.out_dtype)
+    status = nat.DeviceArray(nat.darray_alloc(max(n * 4, 4)), (n,), np.int32) if with_status else None
+    return out, status
+
+
+def _device_sync():
+    from .. import _native as nat
+
+    nat.check(nat.load().b2s_device_sync())
 
 
 def _tracked_op(tracker):
