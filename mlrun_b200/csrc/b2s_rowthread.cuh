@@ -13,7 +13,8 @@
 //   The TPR partial sums of a row are combined in shared memory in a fixed order (deterministic fp64);
 //   bias, link, vote and the coalesced 4-byte store are done by the row's q = 0 thread.  A non-finite
 //   model input surfaces as a non-finite score (NaN/Inf survive fma even with a zero weight), which is
-//   what the per-row status tests.
+//   what the per-row status tests.  A plan whose mean vote is folded into one linear model (RTParams::folded) runs
+//   the same loop with one accumulator: one DFMA per value.
 #pragma once
 #include <cuda.h>  // CUtensorMap (type only; the encoder is resolved at run time by the host)
 #include <type_traits>
@@ -76,7 +77,8 @@ struct RTParams {
     int32_t cnt;      // number of categories
     int32_t woff_b;   // byte offset of the first category's weight row in s_wcat
     float fill;       // Imputer value of the column (NaN: not imputed)
-    int32_t pad[2];
+    int32_t woff_fb;  // byte offset of the first category's folded weight in s_wcatf (folded plans)
+    int32_t pad;
   };
   CatFast catf[kRTMaxCatCols];
   int32_t cats_fast;   // 1: catf describes every categorical column
@@ -89,6 +91,13 @@ struct RTParams {
   uint64_t g_mask;
   const float* g_values;       // [n_keys + 1][n_in]; row n_keys is all NaN and stands for an unknown key
   long long g_missing_row;
+  // mean vote of identity scorers folded into one linear model (rt_build): sum_k v_k (b_k + w_k . x) = wf . x + bias_f.
+  // The per-model tables above stay: a row whose folded score is not finite is re-scored from them (rt_unfolded_vote).
+  int32_t folded;
+  int32_t zero_woff_fb;        // byte offset of the zero row in s_wcatf
+  const double* wcat_f;        // [n_cat] (global; copied to shared memory after the per-model rows, plus a zero row)
+  double bias_f;
+  double wf[NCH * 4];          // constant-bank operands
 };
 
 // how a thread finds the 16-byte chunks of its row inside the shared-memory tile
@@ -112,11 +121,14 @@ struct RowSwizzled {  // 2-D TMA boxes of 32 floats x TR rows, SWIZZLE_128B: chu
   }
 };
 
-// dot products of the chunks [CH0, CH1) of a row with all NS weight columns (the weights, fills and limits
-// are constant-bank / uniform-register operands).  The row is an array of RPT = 1 rows: this form compiles to the
-// same code as the kernel has always had; a scalar row changes its register allocation and stack frame.
-template <int NCH, int NS, int CH0, int CH1, typename Row>
-__device__ __forceinline__ void rt_slice(const RTParams<NCH, NS>& p, const Row (&xr)[1], double (&acc)[1][NS]) {
+// dot products of the chunks [CH0, CH1) of a row with NA weight columns (the weights, fills and limits are
+// constant-bank / uniform-register operands): NA = NS scores the plan's score slots, NA = 1 < NS the folded model (wf).
+// The row is an array of RPT = 1 rows: this form compiles to the same code as the kernel has always had; a scalar row
+// changes its register allocation and stack frame.
+template <int NCH, int NS, int NA, int CH0, int CH1, typename Row>
+__device__ __forceinline__ void rt_slice(const RTParams<NCH, NS>& p, const Row (&xr)[1], double (&acc)[1][NA]) {
+  static_assert(NA == NS || NA == 1, "score slots or the folded model");
+  constexpr bool F = NA != NS;
   constexpr int RPT = 1;
   constexpr int BATCH = 4;  // chunks converted before their DFMAs are issued (ILP)
 #pragma unroll
@@ -148,9 +160,9 @@ __device__ __forceinline__ void rt_slice(const RTParams<NCH, NS>& p, const Row (
         for (int u = 0; u < 4; ++u) {
           const int c = ch * 4 + u;
 #pragma unroll
-          for (int k = 0; k < NS; ++k)
+          for (int k = 0; k < NA; ++k)
 #pragma unroll
-            for (int i = 0; i < RPT; ++i) acc[i][k] = fma(p.w[c][k], xd[i][cb * 4 + u], acc[i][k]);
+            for (int i = 0; i < RPT; ++i) acc[i][k] = fma(F ? p.wf[c] : p.w[c][k], xd[i][cb * 4 + u], acc[i][k]);
         }
       }
     }
@@ -171,14 +183,16 @@ __device__ __noinline__ int rt_cat_search(const RTParams<NCH, NS>& p, int cc, fl
   return j;
 }
 
-// one-hot columns Q0, Q0+TPR, ... of one row: "onehot(x) . w" is a gather from the shared-memory weight rows.
+// one-hot columns Q0, Q0+TPR, ... of one row: "onehot(x) . w" is a gather from the shared-memory weight rows
+// (s_wcat: rows of NA doubles, the per-model rows or, NA = 1 < NS, the folded ones).
 // Fully unrolled with literal column slots (the caller's branch on the slice index is warp-uniform), so every
 // table entry is a constant-bank operand and the address arithmetic stays in the uniform datapath.
-template <int NCH, int NS, int Q0, int TPR, typename Row>
+template <int NCH, int NS, int NA, int Q0, int TPR, typename Row>
 __device__ __forceinline__ void rt_cats(const RTParams<NCH, NS>& p, const Row (&xr)[1], const double* __restrict__ s_wcat,
-                                        double (&acc)[1][NS]) {
+                                        double (&acc)[1][NA]) {
   constexpr int RPT = 1;
   constexpr int ITERS = (kRTMaxCatCols - Q0 + TPR - 1) / TPR;
+  constexpr bool F = NA != NS;
   if (p.cats_fast) {  // integer codes first .. first + cnt - 1 in every column: no search, no per-column branch
     const char* wb = reinterpret_cast<const char*>(s_wcat);
 #pragma unroll
@@ -193,10 +207,10 @@ __device__ __forceinline__ void rt_cats(const RTParams<NCH, NS>& p, const Row (&
         const int v = __float2int_rz(x);  // saturating; NaN -> 0 and fails the equality below
         const unsigned jj = (unsigned)(v - cf.first);
         const bool miss = ((float)v != x) | (jj >= (unsigned)cf.cnt);
-        const int a = miss ? p.zero_woff_b : cf.woff_b + (int)jj * (NS * 8);
-        if constexpr (NS % 2 == 0) {  // weight rows are 16-byte aligned: LDS.128
+        const int a = miss ? (F ? p.zero_woff_fb : p.zero_woff_b) : (F ? cf.woff_fb : cf.woff_b) + (int)jj * (NA * 8);
+        if constexpr (NA % 2 == 0) {  // weight rows are 16-byte aligned: LDS.128
 #pragma unroll
-          for (int k = 0; k < NS; k += 2) {
+          for (int k = 0; k < NA; k += 2) {
             const double2 w2 = *reinterpret_cast<const double2*>(wb + a + k * 8);
             acc[i][k] += w2.x;
             acc[i][k + 1] += w2.y;
@@ -204,7 +218,7 @@ __device__ __forceinline__ void rt_cats(const RTParams<NCH, NS>& p, const Row (&
         } else {
           const double* wc = reinterpret_cast<const double*>(wb + a);
 #pragma unroll
-          for (int k = 0; k < NS; ++k) acc[i][k] += wc[k];
+          for (int k = 0; k < NA; ++k) acc[i][k] += wc[k];
         }
       }
     }
@@ -226,9 +240,9 @@ __device__ __forceinline__ void rt_cats(const RTParams<NCH, NS>& p, const Row (&
       } else {
         j = rt_cat_search(p, cc, x);
       }
-      const double* wc = s_wcat + (size_t)j * NS;
+      const double* wc = s_wcat + (size_t)j * NA;
 #pragma unroll
-      for (int k = 0; k < NS; ++k) acc[i][k] += wc[k];
+      for (int k = 0; k < NA; ++k) acc[i][k] += wc[k];
     }
   }
 }
@@ -236,24 +250,61 @@ __device__ __forceinline__ void rt_cats(const RTParams<NCH, NS>& p, const Row (&
 // slice q of a row: the dot products over its share of the LIVE leading chunks + its share of the one-hot columns.
 // The slice index is warp-uniform; each case has compile-time column indices (constant operands); the row's one-hot
 // columns are dealt round-robin to its threads.
-template <int NCH, int NS, int TPR, int LIVE, typename Row>
+template <int NCH, int NS, int NA, int TPR, int LIVE, typename Row>
 __device__ __forceinline__ void rt_row_slices(const RTParams<NCH, NS>& p, int q, const Row (&xr)[1], const double* __restrict__ s_wcat,
-                                              double (&acc)[1][NS]) {
+                                              double (&acc)[1][NA]) {
   static_assert(LIVE % TPR == 0, "live chunks must split evenly over the row's threads");
   constexpr int CPT = LIVE / TPR;
   if (TPR == 1 || q == 0) {
-    rt_slice<NCH, NS, 0, CPT>(p, xr, acc);
-    rt_cats<NCH, NS, 0, TPR>(p, xr, s_wcat, acc);
+    rt_slice<NCH, NS, NA, 0, CPT>(p, xr, acc);
+    rt_cats<NCH, NS, NA, 0, TPR>(p, xr, s_wcat, acc);
   } else if (q == 1) {
-    rt_slice<NCH, NS, (TPR > 1 ? CPT : 0), (TPR > 1 ? 2 * CPT : 0)>(p, xr, acc);
-    rt_cats<NCH, NS, (TPR > 1 ? 1 : 0), TPR>(p, xr, s_wcat, acc);
+    rt_slice<NCH, NS, NA, (TPR > 1 ? CPT : 0), (TPR > 1 ? 2 * CPT : 0)>(p, xr, acc);
+    rt_cats<NCH, NS, NA, (TPR > 1 ? 1 : 0), TPR>(p, xr, s_wcat, acc);
   } else if (q == 2) {
-    rt_slice<NCH, NS, (TPR > 2 ? 2 * CPT : 0), (TPR > 2 ? 3 * CPT : 0)>(p, xr, acc);
-    rt_cats<NCH, NS, (TPR > 2 ? 2 : 0), TPR>(p, xr, s_wcat, acc);
+    rt_slice<NCH, NS, NA, (TPR > 2 ? 2 * CPT : 0), (TPR > 2 ? 3 * CPT : 0)>(p, xr, acc);
+    rt_cats<NCH, NS, NA, (TPR > 2 ? 2 : 0), TPR>(p, xr, s_wcat, acc);
   } else {
-    rt_slice<NCH, NS, (TPR > 3 ? 3 * CPT : 0), (TPR > 3 ? 4 * CPT : 0)>(p, xr, acc);
-    rt_cats<NCH, NS, (TPR > 3 ? 3 : 0), TPR>(p, xr, s_wcat, acc);
+    rt_slice<NCH, NS, NA, (TPR > 3 ? 3 * CPT : 0), (TPR > 3 ? 4 * CPT : 0)>(p, xr, acc);
+    rt_cats<NCH, NS, NA, (TPR > 3 ? 3 : 0), TPR>(p, xr, s_wcat, acc);
   }
+}
+
+// a folded plan's row whose folded score is not finite: the stored value is the unfolded vote, scored again from the
+// whole row in the tile with the per-model tables.  A non-finite input poisons the folded and the per-model scores alike
+// (the status word does not change), but the vote of the poisoned scores can differ from the folded score: +Inf under
+// weights +1 and -3 with votes 1/2, 1/2 gives NaN unfolded and -Inf folded.  Finite rows never get here.
+// Inlined with rolled loops rather than called: a call in the epilogue makes every row pay for the registers it keeps live.
+template <int NCH, int NS, typename Row>
+__device__ __forceinline__ double rt_unfolded_vote(const RTParams<NCH, NS>& p, const Row& row, const double* __restrict__ s_wcat) {
+  double acc[NS];
+#pragma unroll
+  for (int k = 0; k < NS; ++k) acc[k] = 0.0;
+#pragma unroll 1
+  for (int ch = 0; ch < NCH; ++ch) {
+    const float4 v = row.chunk(ch);
+    const float xs[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int c = ch * 4 + u;
+      const float x = !(fabsf(xs[u]) <= p.lim[c]) ? p.fill[c] : xs[u];  // as rt_slice
+#pragma unroll
+      for (int k = 0; k < NS; ++k) acc[k] = fma(p.w[c][k], (double)x, acc[k]);
+    }
+  }
+#pragma unroll 1
+  for (int cc = 0; cc < p.n_cat_cols; ++cc) {  // a search over the column's categories finds what rt_cats finds
+    float x = row.at2(p.cat_off[cc], p.cat_sw[cc]);
+    x = (x != x) ? p.cat_fill[cc] : x;
+    int j = p.n_cat;  // the zero row
+    for (int qq = p.cat_cnt[cc] - 1; qq >= 0; --qq) j = (x == p.cat_val[p.cat_base[cc] + qq]) ? p.cat_base[cc] + qq : j;
+#pragma unroll
+    for (int k = 0; k < NS; ++k) acc[k] += s_wcat[(size_t)j * NS + k];
+  }
+  double s = 0.0;
+#pragma unroll
+  for (int k = 0; k < NS; ++k) s = __dadd_rn(s, __dmul_rn(__dadd_rn(acc[k], p.bias[k]), p.vote_w[k]));
+  return s;
 }
 
 // ---- TMA (bulk async copy) + mbarrier helpers: one 1-D bulk copy per event row lands in the padded tile
@@ -325,11 +376,15 @@ __global__ void __launch_bounds__(128 * TPR, TPR >= 4 ? 2 : (TPR == 2 ? 3 : 4))
   extern __shared__ __align__(16) unsigned char smem[];
   uint64_t* s_bar = reinterpret_cast<uint64_t*>(smem);  // 4 mbarriers (bulk variant); 64 bytes reserved
   double* s_wcat = reinterpret_cast<double*>(smem + 64);
-  const size_t wcat_bytes = 64 + (((size_t)(p.n_cat + 1) * NS * 8 + 15) / 16) * 16;
+  const bool fold = NS >= 2 && p.folded;  // (uniform)
+  const size_t wcat_model_bytes = (((size_t)(p.n_cat + 1) * NS * 8 + 15) / 16) * 16;
+  double* s_wcatf = reinterpret_cast<double*>(smem + 64 + wcat_model_bytes);  // folded rows (folded plans)
+  const size_t wcat_bytes = 64 + wcat_model_bytes + (fold ? (((size_t)(p.n_cat + 1) * 8 + 15) / 16) * 16 : 0);
   // With the tensor-map loader and TPR > 1 the tile loop has ONE barrier per tile (between the partial sums
   // and their combination): that barrier also proves the tile's stage is drained, so the next load into it is
   // issued right there, and the partial sums are double-buffered instead of fenced by a second barrier.
-  const bool one_sync = (LM == 2) && TPR > 1 && p.one_sync;
+  // Folded plans keep two barriers: rt_unfolded_vote reads the tile in the epilogue, after the partial-sum barrier.
+  const bool one_sync = (LM == 2) && TPR > 1 && p.one_sync && !fold;
   constexpr size_t part_words = (size_t)(TPR - 1) * 128 * NS;
   double* s_part = reinterpret_cast<double*>(smem + wcat_bytes);  // [one_sync ? 2 : 1][(TPR-1)][128][NS]
   float* s_tiles = reinterpret_cast<float*>(smem + wcat_bytes + (one_sync ? 2 : 1) * part_words * 8);
@@ -470,6 +525,8 @@ __global__ void __launch_bounds__(128 * TPR, TPR >= 4 ? 2 : (TPR == 2 ? 3 : 4))
   uint32_t phase_bits = 0;  // bit s: parity to wait for on stage s
   for (int i = tid; i < p.n_cat * NS; i += blockDim.x) s_wcat[i] = p.wcat[i];
   for (int i = tid; i < NS; i += blockDim.x) s_wcat[p.n_cat * NS + i] = 0.0;
+  if (fold)
+    for (int i = tid; i <= p.n_cat; i += blockDim.x) s_wcatf[i] = i < p.n_cat ? p.wcat_f[i] : 0.0;
   if (one_sync) __syncthreads();  // the weight rows are read before the loop's first barrier
 
   int stage = 0;
@@ -510,76 +567,88 @@ __global__ void __launch_bounds__(128 * TPR, TPR >= 4 ? 2 : (TPR == 2 ? 3 : 4))
         xr[i].xr = tile + ri * p.pitch;
       }
     }
-    double acc[RPT][NS];
+    // the tile's dot products, their combination and the epilogue, with NA = NS score slots or (folded) one
+    auto score_tile = [&](auto na) {
+      constexpr int NA = decltype(na)::value;
+      constexpr bool F = NA != NS;
+      const double* s_w = F ? s_wcatf : s_wcat;
+      double acc[RPT][NA];
 #pragma unroll
-    for (int i = 0; i < RPT; ++i)
+      for (int i = 0; i < RPT; ++i)
 #pragma unroll
-      for (int k = 0; k < NS; ++k) acc[i][k] = 0.0;
-    if (any_live) {
-      // trailing chunks without a model input are not multiplied at all: the live chunks are split evenly over the row's
-      // threads (a uniform branch picks the fully unrolled version for 0, 2 or 4 skipped chunks)
-      if constexpr (LM == 2 && RPT == 1 && NCH >= 8 && (TPR == 1 || TPR == 2)) {  // (the tensor-map variants only: build time)
-        if (p.dead_tail >= 4) rt_row_slices<NCH, NS, TPR, NCH - 4>(p, q, xr, s_wcat, acc);
-        else if (p.dead_tail >= 2) rt_row_slices<NCH, NS, TPR, NCH - 2>(p, q, xr, s_wcat, acc);
-        else rt_row_slices<NCH, NS, TPR, NCH>(p, q, xr, s_wcat, acc);
-      } else {
-        rt_row_slices<NCH, NS, TPR, NCH>(p, q, xr, s_wcat, acc);
-      }
-    }
-    if (TPR > 1) {  // combine the row's slices in a fixed order (deterministic fp64 sum)
-      double* s_part_cur = s_part + (one_sync ? (size_t)(iter & 1) * part_words : 0);
-      if (q > 0) {
-#pragma unroll
-        for (int i = 0; i < RPT; ++i) {
-          double* part = s_part_cur + ((size_t)(q - 1) * 128 + r + i * TRT) * NS;
-#pragma unroll
-          for (int k = 0; k < NS; ++k) part[k] = acc[i][k];
-        }
-      }
-      __syncthreads();
-      if (one_sync) issue_bulk(stage, (t + (int64_t)S * gridDim.x) * TR);  // every read of this stage is behind the barrier
-      if (q == 0) {
-#pragma unroll
-        for (int i = 0; i < RPT; ++i)
-#pragma unroll
-          for (int qq = 1; qq < TPR; ++qq) {
-            const double* o = s_part_cur + ((size_t)(qq - 1) * 128 + r + i * TRT) * NS;
-#pragma unroll
-            for (int k = 0; k < NS; ++k) acc[i][k] += o[k];
-          }
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < RPT; ++i) {
-      const int64_t row = row0 + (r + i * TRT);
-      if (q == 0 && r + i * TRT < live_rows) {
-        uint32_t st = 0;
-#pragma unroll
-        for (int k = 0; k < NS; ++k) {
-          acc[i][k] += p.bias[k];
-          st |= (fabs(acc[i][k]) <= 1.7976931348623157e308) ? 0u : 1u;
-        }
-        if (LM == 1) st |= ((unknown_bits >> stage) & 1u) << 2;  // B2S_ROW_UNKNOWN_KEY
-        if (p.fast_epilogue) {
-          if (p.vote_kind == 1) {  // VotingEnsemble._mean_vote: sum_m w[m] * pred[m], model order
-            double s = 0.0;
-#pragma unroll
-            for (int k = 0; k < NS; ++k) s = __dadd_rn(s, __dmul_rn(acc[i][k], p.vote_w[k]));
-            store_word(p, row, 0, __float_as_uint((float)s));
-          } else {
-#pragma unroll
-            for (int k = 0; k < NS; ++k)
-              if (k < p.n_models) store_word(p, row, k, __float_as_uint((float)acc[i][k]));
-          }
-          if (p.status) p.status[row] = (int32_t)st;
+        for (int k = 0; k < NA; ++k) acc[i][k] = 0.0;
+      if (any_live) {
+        // trailing chunks without a model input are not multiplied at all: the live chunks are split evenly over the row's
+        // threads (a uniform branch picks the fully unrolled version for 0, 2 or 4 skipped chunks)
+        if constexpr (LM == 2 && RPT == 1 && NCH >= 8 && (TPR == 1 || TPR == 2)) {  // (the tensor-map variants only: build time)
+          if (p.dead_tail >= 4) rt_row_slices<NCH, NS, NA, TPR, NCH - 4>(p, q, xr, s_w, acc);
+          else if (p.dead_tail >= 2) rt_row_slices<NCH, NS, NA, TPR, NCH - 2>(p, q, xr, s_w, acc);
+          else rt_row_slices<NCH, NS, NA, TPR, NCH>(p, q, xr, s_w, acc);
         } else {
-          double sl[NS];
-#pragma unroll
-          for (int k = 0; k < NS; ++k) sl[k] = acc[i][k];
-          rt_generic_epilogue(p, sl, row, st);
+          rt_row_slices<NCH, NS, NA, TPR, NCH>(p, q, xr, s_w, acc);
         }
       }
-    }
+      if (TPR > 1) {  // combine the row's slices in a fixed order (deterministic fp64 sum)
+        double* s_part_cur = s_part + (one_sync ? (size_t)(iter & 1) * part_words : 0);
+        if (q > 0) {
+#pragma unroll
+          for (int i = 0; i < RPT; ++i) {
+            double* part = s_part_cur + ((size_t)(q - 1) * 128 + r + i * TRT) * NA;
+#pragma unroll
+            for (int k = 0; k < NA; ++k) part[k] = acc[i][k];
+          }
+        }
+        __syncthreads();
+        if (one_sync) issue_bulk(stage, (t + (int64_t)S * gridDim.x) * TR);  // every read of this stage is behind the barrier
+        if (q == 0) {
+#pragma unroll
+          for (int i = 0; i < RPT; ++i)
+#pragma unroll
+            for (int qq = 1; qq < TPR; ++qq) {
+              const double* o = s_part_cur + ((size_t)(qq - 1) * 128 + r + i * TRT) * NA;
+#pragma unroll
+              for (int k = 0; k < NA; ++k) acc[i][k] += o[k];
+            }
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < RPT; ++i) {
+        const int64_t row = row0 + (r + i * TRT);
+        if (q == 0 && r + i * TRT < live_rows) {
+          uint32_t st = 0;
+#pragma unroll
+          for (int k = 0; k < NA; ++k) {
+            acc[i][k] += F ? p.bias_f : p.bias[k];
+            st |= (fabs(acc[i][k]) <= 1.7976931348623157e308) ? 0u : 1u;
+          }
+          if (LM == 1) st |= ((unknown_bits >> stage) & 1u) << 2;  // B2S_ROW_UNKNOWN_KEY
+          if constexpr (F) {  // a folded plan is a mean vote with the fast epilogue
+            const double s = (st & 1u) ? rt_unfolded_vote<NCH, NS>(p, xr[i], s_wcat) : acc[i][0];
+            store_word(p, row, 0, __float_as_uint((float)s));
+            if (p.status) p.status[row] = (int32_t)st;
+          } else if (p.fast_epilogue) {
+            if (p.vote_kind == 1) {  // VotingEnsemble._mean_vote: sum_m w[m] * pred[m], model order
+              double s = 0.0;
+#pragma unroll
+              for (int k = 0; k < NS; ++k) s = __dadd_rn(s, __dmul_rn(acc[i][k], p.vote_w[k]));
+              store_word(p, row, 0, __float_as_uint((float)s));
+            } else {
+#pragma unroll
+              for (int k = 0; k < NS; ++k)
+                if (k < p.n_models) store_word(p, row, k, __float_as_uint((float)acc[i][k]));
+            }
+            if (p.status) p.status[row] = (int32_t)st;
+          } else {
+            double sl[NS];
+#pragma unroll
+            for (int k = 0; k < NS; ++k) sl[k] = acc[i][k];
+            rt_generic_epilogue(p, sl, row, st);
+          }
+        }
+      }
+    };
+    if (NS >= 2 && fold) score_tile(std::integral_constant<int, 1>{});
+    else score_tile(std::integral_constant<int, NS>{});
     ++stage;
     ++iter;
     if (stage == S) stage = 0;

@@ -206,6 +206,7 @@ struct b2s_plan_s {
   bool rt_ok = false;
   int rt_cat_cols = 0;  // one-hot source columns of the row-thread plan
   int rt_NCH = 0, rt_NS = 0, rt_grid = 0, rt_smem = 0, rt_pitch = 0;
+  bool rt_folded = false;     // the mean vote is folded into one linear model (fold_mean_vote)
   std::vector<char> rt_blob;  // an RTParams<NCH, NS>
   // fused ensemble-merge targets (P2P)
   std::vector<void*> peers;
@@ -367,7 +368,43 @@ struct RTTables {  // what rt_build needs from finalize
   const double* d_vote_w;
   const ModelDesc* d_models;
   const int32_t* d_classes;
+  const std::vector<double>* wnum_f;  // folded plans (fold_mean_vote): [n_in]; null otherwise
+  double bias_f;
+  const double* d_wcat_f;             // [n_cat]
 };
+
+// A weighted mean of linear models is one linear model:  sum_k v_k (b_k + sum_c w_ck x_c) = sum_c w'_c x_c + b'.
+// Folded once here, the row-thread kernel computes one dot product per row instead of NS.  Every folded constant
+// (w'_c, the one-hot rows w'_j and b') is summed in double-double (TwoSum, fma TwoProduct) and rounded once.
+// Declined when a weight, a bias or a folded magnitude sum_k |v_k w_k| reaches 2^880: below that, with float32 inputs
+// (|x| < 2^128) and at most 145 terms, no per-model score, product v_k * score or folded score can overflow, so the
+// folded score is non-finite exactly when a model input is, and the status words are those of the unfolded plan.
+static bool fold_mean_vote(int NS, const std::vector<double>& vote_w, const std::vector<double>& wnum,
+                           const std::vector<double>& wcat, const std::vector<double>& bias, std::vector<double>& wnum_f,
+                           std::vector<double>& wcat_f, double& bias_f) {
+  constexpr double kBound = 0x1p880;
+  const int M = (int)vote_w.size();  // score slot k is model k (one score each); slots M .. NS - 1 are zero
+  auto fold = [&](const double* w, double& out) {
+    double hi = 0.0, lo = 0.0, mag = 0.0;
+    for (int k = 0; k < M; ++k) {
+      if (!(std::fabs(w[k]) < kBound)) return false;
+      const double pr = vote_w[k] * w[k], pe = std::fma(vote_w[k], w[k], -pr);
+      const double sum = hi + pr, bv = sum - hi, se = (hi - (sum - bv)) + (pr - bv);
+      hi = sum;
+      lo += se + pe;
+      mag += std::fabs(pr);
+    }
+    out = hi + lo;
+    return mag < kBound;  // false for NaN too
+  };
+  wnum_f.assign(wnum.size() / NS, 0.0);
+  wcat_f.assign(wcat.size() / NS, 0.0);
+  for (size_t c = 0; c < wnum_f.size(); ++c)
+    if (!fold(&wnum[c * NS], wnum_f[c])) return false;
+  for (size_t j = 0; j < wcat_f.size(); ++j)
+    if (!fold(&wcat[j * NS], wcat_f[j])) return false;
+  return fold(bias.data(), bias_f);
+}
 
 // threads per row: 2 for wide rows (more warps than 1, less combine overhead than 4)
 constexpr int rt_tpr(int NCH) { return NCH >= 8 ? 2 : 1; }
@@ -440,6 +477,15 @@ static void rt_build(b2s_plan_s* p, const RTTables& t) {
     if (last_live < 0) r.dead_tail = 0;
   }
   for (int i = 0; i < r.n_cat; ++i) r.cat_val[i] = (*t.cat_val)[i];
+  p->rt_folded = NS >= 2 && t.wnum_f != nullptr;
+  if (p->rt_folded) {
+    r.folded = 1;
+    for (int c = 0; c < t.n_in; ++c) r.wf[c] = (*t.wnum_f)[c];
+    r.bias_f = t.bias_f;
+    r.wcat_f = t.d_wcat_f;
+    for (int cc = 0; cc < ncc; ++cc) r.catf[cc].woff_fb = r.cat_base[cc] * 8;
+    r.zero_woff_fb = r.n_cat * 8;
+  }
 }
 
 struct LaunchCtx {             // per-launch context (launches of one plan may be issued from several threads at once)
@@ -519,7 +565,8 @@ static cudaError_t rt_launch_t(b2s_plan_s* p, const void* rows, int64_t stride, 
   const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(p->rt_grid, tiles));  // persistent CTAs
   r.use_bulk = mode;
   // single-barrier tile loop: measured better with 4 score columns (0.0506 vs 0.0512 ms, r2o) and worse with one
-  // (0.0481 vs 0.0454 ms, r2q / r2o): it follows the number of score columns
+  // (0.0481 vs 0.0454 ms, r2q / r2o): it follows the number of score columns (folded plans have one: the kernel keeps
+  // them on two barriers)
   r.one_sync = NS >= 4 ? 1 : 0;
   for (int cc = 0; cc < r.n_cat_cols; ++cc) {  // tile-relative position of each categorical column
     const int col = r.cat_col[cc], ch = col >> 2;
@@ -1473,6 +1520,12 @@ extern "C" int b2s_plan_finalize(b2s_plan_t p) {
           }
       }
     }
+    bool simple = true;  // identity scorers of one score each
+    for (auto& m : p->models) simple = simple && m.link == B2S_LINK_IDENTITY && m.n_scores == 1;
+    std::vector<double> wnum_f, wcat_f;
+    double bias_f = 0.0;
+    const bool folded = p->mode == MODE_LINEAR && p->vote_kind == B2S_VOTE_MEAN && simple && NS >= 2 &&
+                        fold_mean_vote(NS, p->vote_w, wnum, wcat, bias, wnum_f, wcat_f, bias_f);
     // ---- upload one blob
     BlobBuilder bb;
     const size_t o_dwh = bb.add(dense_wh), o_dwm = bb.add(dense_wm), o_dwl = bb.add(dense_wl);
@@ -1482,7 +1535,7 @@ extern "C" int b2s_plan_finalize(b2s_plan_t p) {
                  o_bias = bb.add(bias), o_models = bb.add(descs), o_classes = bb.add(classes),
                  o_votew = bb.add(p->vote_w), o_wgen = bb.add(wgen), o_nodes = bb.add(nodes), o_leaf = bb.add(leaf),
                  o_troot = bb.add(tree_root), o_tslot = bb.add(tree_slot), o_tscale = bb.add(tree_scale),
-                 o_chunk = bb.add(chunk_kind);
+                 o_chunk = bb.add(chunk_kind), o_wcatf = bb.add(wcat_f);
     B2S_CUDA_TRY(cudaSetDevice(G.device));
     if (int rc = allocate(p->d_blob, bb.data.size())) return rc;
     B2S_CUDA_TRY(cudaMemcpy(p->d_blob.get(), bb.data.data(), bb.data.size(), cudaMemcpyHostToDevice));
@@ -1543,8 +1596,6 @@ extern "C" int b2s_plan_finalize(b2s_plan_t p) {
         d.labels[kk] = kk;
       }
       {
-        bool simple = true;  // every model: one identity score
-        for (auto& m : p->models) simple = simple && m.link == B2S_LINK_IDENTITY && m.n_scores == 1;
         d.epi = DENSE_EPI_GENERIC;
         if (simple && p->vote_kind == B2S_VOTE_NONE) d.epi = DENSE_EPI_SCORES;
         if (simple && p->vote_kind == B2S_VOTE_MEAN) {
@@ -1661,20 +1712,21 @@ extern "C" int b2s_plan_finalize(b2s_plan_t p) {
         p->rt_NCH = nch <= 4 ? 4 : (nch <= 8 ? 8 : (nch <= 16 ? 16 : 32));
         p->rt_NS = NS;
         p->rt_cat_cols = n_cat_cols;
-        bool simple = true;
-        for (auto& m : p->models) simple = simple && m.link == B2S_LINK_IDENTITY && m.n_scores == 1;
         RTTables t{n_in, p->out_cols, M, p->vote_kind, p->out_is_int, (simple && p->vote_kind != B2S_VOTE_MAJORITY) ? 1 : 0, NS,
-                   &p->fill, &flags, &wnum, &bias, &p->vote_w, &cat_off, &cat_val, k.wcat, k.vote_w, k.models, k.classes};
+                   &p->fill, &flags, &wnum, &bias, &p->vote_w, &cat_off, &cat_val, k.wcat, k.vote_w, k.models, k.classes,
+                   folded ? &wnum_f : nullptr, bias_f, (const double*)(B + o_wcatf)};
         rt_build_any(p, t);
         int rpitch = p->rt_NCH * 4 + 4;
         if (((rpitch / 4) & 1) == 0) rpitch += 4;
         p->rt_pitch = rpitch;
         {
-          const size_t fixed = 1024 + 64 + align_up((size_t)(cat_val.size() + 1) * NS * 8, 16);
+          // folded plans: the folded one-hot rows too, and one partial-sum buffer (never the single-barrier loop)
+          const size_t fixed = 1024 + 64 + align_up((size_t)(cat_val.size() + 1) * NS * 8, 16) +
+                               (p->rt_folded ? align_up((size_t)(cat_val.size() + 1) * 8, 16) : 0);
           const size_t part = (size_t)(rt_tpr(p->rt_NCH) - 1) * 128 * NS * 8;
           // padded tiles + one partial-sum buffer (LDGSTS / per-row bulk), or swizzled tiles + two (tensor map)
           const size_t padded = fixed + part + (size_t)kRTStages * kRTTileRows * rpitch * 4;
-          const size_t swizzled = fixed + 2 * part + (size_t)kRTStages * kRTTileRows * p->rt_NCH * 16;
+          const size_t swizzled = fixed + (p->rt_folded ? 1 : 2) * part + (size_t)kRTStages * kRTTileRows * p->rt_NCH * 16;
           p->rt_smem = (int)std::max(padded, swizzled);
         }
         int occ = 0;
@@ -1706,7 +1758,7 @@ extern "C" const char* b2s_plan_kernel(b2s_plan_t p) {
   const bool tmap = p->rt_NCH >= 8 && p->n_in == p->rt_NCH * 4 && tensor_map_encoder();
   if (p->dense_ok) snprintf(buf, sizeof(buf), "dense_head_kernel<N=%d> (wgmma tf32, %s, register accumulator groups; %d scores over %d columns)", p->dense.n_pad, p->dense.exact ? "exact 3-term input split" : "2-term input split", p->dense.n_scores, p->dense.n_in);
   else if (p->t3_ok) snprintf(buf, sizeof(buf), "t3_prep_kernel + trees3_kernel<D=%d,%s%s> + t3_vote_kernel (%d parts resident in shared memory, %d walking warps)", p->t3_D, p->t3_miss ? "NaN routing" : "floats", p->t3_cat ? ",categorical" : "", p->t3_parts, p->t3.warps);
-  else if (p->rt_ok) snprintf(buf, sizeof(buf), "rowthread_kernel<NCH=%d,NS=%d,TPR=%d,%s>", p->rt_NCH, p->rt_NS, rt_tpr(p->rt_NCH), tmap ? "TMA tensor-map loads" : "TMA bulk loads");
+  else if (p->rt_ok) snprintf(buf, sizeof(buf), "rowthread_kernel<NCH=%d,NS=%d,TPR=%d,%s>%s", p->rt_NCH, p->rt_NS, rt_tpr(p->rt_NCH), tmap ? "TMA tensor-map loads" : "TMA bulk loads", p->rt_folded ? ", mean vote folded" : "");
   else snprintf(buf, sizeof(buf), "rows_kernel<%s,NS=%d>%s", p->mode == MODE_LINEAR ? "LINEAR" : (p->mode == MODE_TREES ? "TREES" : "STORE"), p->NS, p->any_cat ? " (categorical splits)" : "");
   return buf;
 }
